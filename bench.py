@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the LumixEngine hot path on B200 (contract: task brief "Measurement").
+"""bench.py — headline benchmark of the LumixEngine hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, liblumix_b200.so)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU cull on the host cores
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's visible set as DIR/*.npy
 
 Metric (BASELINE.json): M entities culled/s.  Workload at N=1: configs[1] = "10M static entities, 1 camera frustum cull,
-single B200" (scene C2 of SURVEY.md §8d).  A step = one CullingSystem::cull of the whole scene for one frustum.
+single GPU" (scene C2 of SURVEY.md §8d).  A step = one CullingSystem::cull of the whole scene for one frustum.
 N>1 (torchrun, one rank per GPU): weak scaling — every rank owns its own 10 M-entity shard (whole cell pages, no
 data-path collective for the cull itself) and each step carries the one exchange the path has (SURVEY.md §8e): the visibility
 bitmask + per-type counts of every rank reach every other rank, stored into peer memory over NVLink by the cull kernel itself
@@ -19,6 +20,7 @@ step on the host).  `parity`: the C2 digest against the reference build; at N>1 
 DESIGN.md section 7 describes every field.
 """
 import argparse
+import atexit
 import json
 import os
 import statistics
@@ -35,7 +37,7 @@ if ROOT not in sys.path:
 
 N_ENTITIES = 10_000_000
 WORKLOAD = "C2: 10M static entities, 1 camera frustum cull (BASELINE.json configs[1]); per GPU at N>1"
-REPLICAS = 8  # scene copies rotated through by successive culls: 8 x ~200 MB > 126 MB L2
+REPLICAS = 8  # scene copies rotated through by successive culls: 8 x ~225 MB, each alone 4x the 50 MB L2
 
 
 _REAL_STDOUT = None
@@ -68,22 +70,11 @@ def measured_peaks():
             return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write bytes)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
-
-
-def traffic_from_profile(kernel):
-    """dram bytes per launch from the committed ncu capture, if any (profiles/traffic.json)."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(kernel)
-        except Exception:
-            return None
-    return None
+    return 3350.0, "data sheet (H100 SXM: 3.35 TB/s HBM3; not a measured peak)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons while the GPU is under our load (B200_PROFILING.md 'clocks line')."""
+    """nvidia-smi clocks / throttle reasons while the GPU is under our load."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, device):
@@ -95,6 +86,7 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.device}", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-lms", "50"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self._kill)  # the sampler never outlives bench.py, whatever ends the run
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -104,14 +96,19 @@ class ClockSampler:
         for line in self.proc.stdout:
             self.lines.append((time.time(), line.strip()))
 
+    def _kill(self):
+        if self.proc and self.proc.poll() is None:
+            self.proc.terminate()
+            try:
+                self.proc.wait(timeout=2)
+            except Exception:
+                self.proc.kill()
+                self.proc.wait()
+
     def stop(self, t0, t1):
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
-        self.proc.terminate()
-        try:
-            self.proc.wait(timeout=2)
-        except Exception:
-            self.proc.kill()
+        self._kill()
         sm, mx, reasons = [], [], set()
         for ts, line in self.lines:
             parts = [p.strip() for p in line.split(",")]
@@ -218,6 +215,18 @@ def reference_arm(a, rank):
     emit(line)
 
 
+def dump_outputs(ctx, cs, out_dir):
+    """What the last cull of the timed region handed its caller (lb200_culling_last_result): the visible ids, type after type, and the
+    count of every renderable type.  Within a type the kernel's output order depends on which block claims its slots first, so each
+    type's ids are written sorted; ids < 2^53 are exact in float64."""
+    ptr, res = cs.last_result()
+    counts = np.ctypeslib.as_array(res.type_count).copy()
+    ids = [np.sort(ctx.copy_to_host(ptr + 4 * int(res.type_offset[t]), int(counts[t]), np.uint32)) for t in np.nonzero(counts)[0]]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "visible_ids.npy"), np.concatenate(ids).astype(np.float64) if ids else np.zeros(0, np.float64))
+    np.save(os.path.join(out_dir, "type_count.npy"), counts.astype(np.float64))
+
+
 def time_region(ctx, fn, steps):
     e0, e1 = ctx.event(), ctx.event()
     ctx.synchronize()
@@ -235,7 +244,7 @@ def secondary_paths(ctx, lb, scenes, peak, steps, warmup):
     # --- propagate ---
     parents, locals_, roots = scenes.hierarchy_forest(1_000_000, 8, 7, seed=3)
     hs = []
-    for _ in range(5):  # 5 x 112 MB of locals + globals > 4 x the 126 MB L2: successive steps never find their hierarchy in L2
+    for _ in range(5):  # 5 x 112 MB of locals + globals, each > 2 x the 50 MB L2: successive steps never find their hierarchy in L2
         h = lb.Hierarchy(ctx, parents)
         h.setLocalTransforms(locals_)
         h.setRootTransforms(roots)
@@ -476,8 +485,8 @@ def ours(a, rank, world):
 
     dist = None
     if world > 1:
-        # exchange steps of a lane wait for the peers' flags: more lanes in flight hide more of that (N=2: 14.5 us per step with 3 lanes, 11.1 with 6, 10.1 with 8;
-        # profiles/r2_N2_time_exchange.log).  Read once by the library when the first culling system is created.
+        # exchange steps of a lane wait for the peers' flags: more lanes in flight hide more of that (8 lanes: not yet measured on H100).
+        # Read once by the library when the first culling system is created.
         os.environ.setdefault("LB200_CULL_LANES", "8")
         os.environ.setdefault("NCCL_DEBUG", "WARN")  # keep NCCL's version banner off stdout: the contract is ONE JSON line
         import torch
@@ -575,6 +584,8 @@ def ours(a, rank, world):
         ms_total = float(t.item())
         dist.barrier()
     ms_step = ms_total / a.steps
+    if a.dump_outputs:
+        dump_outputs(ctx, cs, a.dump_outputs)
 
     # N>1, bitmask exchange: one exchanged step is checked — what every rank sees of rank r's slab (per-type counts, visibility rows by page
     # id) must be what rank r holds itself, and rank r's own rows must say exactly what its own cull made visible
@@ -706,7 +717,7 @@ def ours(a, rank, world):
         "config": {**shared_config(visible), "pages": n_pages_c2,
                    "l2": f"{REPLICAS} rotating copies of the page arrays ({REPLICAS} x ~{n_pages_c2 * 4064 // 1_000_000} MB): successive culls never re-read an L2-resident scene",
                    "parallelism": f"dp{world}: whole cell pages per rank" + (("; exchanged each step: " + exchange_desc) if world > 1 else ""),
-                   "submission": "K culls = one lb200_culling_cull_device_n call: consecutive (independent) culls on 3 streams / output lanes, half-occupancy grids, programmatic dependent launch" if world == 1 else f"K exchange steps = one lb200_culling_cull_exchange_n call (steps on {os.environ.get('LB200_CULL_LANES', '3')} streams / output lanes, 3 x lanes exchange buffers per rank)",
+                   "submission": f"K culls = one lb200_culling_cull_device_n call: consecutive (independent) culls on {os.environ.get('LB200_CULL_LANES', '2')} streams / output lanes, half-occupancy grids, programmatic dependent launch" if world == 1 else f"K exchange steps = one lb200_culling_cull_exchange_n call (steps on {os.environ.get('LB200_CULL_LANES', '2')} streams / output lanes, 3 x lanes exchange buffers per rank)",
                    "lone_cull_ms": ms_lone, "lone_empty_interval_ms": lone["empty_interval"], "lone_empty_kernel_ms": lone["empty_kernel"],
                    "scene_build_s": build_s, "page_stats": stats},
         "gpu_launches": int(launches),
@@ -720,13 +731,12 @@ def ours(a, rank, world):
                               # 8 B of ids; the radix sort's 32 B per pair and pass stay in L2 (12 MB) and are not counted
                               "algorithmic_bytes": int(176 * int(visible) + 56 * int(sk_res.n_instances) + 16 * int(sk_res.n_keys)),
                               "hbm_frac": (176 * int(visible) + 56 * int(sk_res.n_instances) + 16 * int(sk_res.n_keys)) / ms_keys / 1e6 / peak,
-                              "traffic": (traffic_from_profile("create_keys_kernel") or 0) + (traffic_from_profile("radix_sort_kernel") or 0),
                               "note": "counts of the last frame of the loop: the lod smoothing state evolves from frame to frame (both arms start from the same state; "
                                       "equality per frame is what tests/test_sortkeys_gpu.py checks)"},
                 "ids_to_host_ms": e2e_ids_s * 1e3, "ids_to_host_d2h_bytes": int(r.total) * 4 + 264 * 4,
                 "ids_to_host_api": "CullingSystem.cull(frustum): visible ids + counts written into pinned host memory by the device right behind the cull (the round-1 e2e)"},
         "roofline": {"bound": "hbm", "achieved": alg_bytes / ms_kernel / 1e6, "peak": peak, "unit": "GB/s", "frac": alg_bytes / ms_kernel / 1e6 / peak,
-                     "traffic": traffic_from_profile("cull_pages_kernel"), "kernel": "cull_pages_kernel", "kernel_ms": ms_kernel, "algorithmic_bytes": int(alg_bytes),
+                     "kernel": "cull_pages_kernel", "kernel_ms": ms_kernel, "algorithmic_bytes": int(alg_bytes),
                      "peak_source": peak_src,
                      "lone_frac": alg_bytes / ms_lone / 1e6 / peak, "lone_ms": ms_lone,
                      "lone_note": "one cull, device to itself, CUDA events (1 us ticks) around it; the interval costs lone_empty_interval_ms with nothing in it and lone_empty_kernel_ms with one empty kernel",
@@ -782,11 +792,16 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--only-cull", action="store_true", help="skip the secondary paths and the CPU baseline leg (profiling runs)")
     ap.add_argument("--no-c5", action="store_true", help="skip the 50M + 1M mixed scene (BASELINE configs[4])")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the visible set of the last timed cull as DIR/visible_ids.npy + DIR/type_count.npy (float64)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
-    claim_stdout()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    if a.dump_outputs and (world > 1 or a.impl != "ours"):
+        ap.error("--dump-outputs is for the single-GPU run of --impl ours")
+    claim_stdout()
     if a.impl == "reference":
         reference_arm(a, rank)
     else:

@@ -1,4 +1,4 @@
-/* lumix_b200.h — C-ABI of the B200-native LumixEngine hot path (cull / hierarchy propagate / pose + skin palette).
+/* lumix_b200.h — C-ABI of the H100-native LumixEngine hot path (cull / hierarchy propagate / pose + skin palette).
  *
  * Plain C: pointers and sizes only, no C++/torch types.  Every entry point returns LB200_OK (0) or a negative
  * lb200_status; lb200_last_error() gives the text.  There is no CPU fallback: without a CUDA device every compute
@@ -178,7 +178,7 @@ LB200_API int lb200_culling_cull_end(lb200_culling* cs, lb200_cull_result* resul
 
 /* Device-resident form: the same cull, result left in HBM (no D2H of ids).  *out_dev_ids receives the device pointer of the
  * id buffer: per-type segments, ids of type t at [type_offset[t], type_offset[t] + type_count[t]).  The buffer belongs to one of the
- * object's output lanes (3 by default, LB200_CULL_LANES): it stays valid through the next lanes - 1 culls, the cull after that reuses
+ * object's output lanes (2 by default, LB200_CULL_LANES): it stays valid through the next lanes - 1 culls, the cull after that reuses
  * it.  Counts land in `result` (a 2 KB D2H).  With want_counts = 0 nothing is
  * read back and the call is fully asynchronous on the context stream (result may be NULL). */
 LB200_API int lb200_culling_cull_device(lb200_culling* cs, const lb200_shifted_frustum* frustum, uint8_t type, const uint32_t** out_dev_ids,

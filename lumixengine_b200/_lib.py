@@ -128,7 +128,7 @@ def recorded_source_hash():
 
 
 def build():
-    """Compile liblumix_b200.so for sm_100a (nvcc cross-compiles without a GPU) and record the hash of the sources next to it."""
+    """Compile liblumix_b200.so for sm_90a (nvcc cross-compiles without a GPU) and record the hash of the sources next to it."""
     subprocess.check_call(["make", "-s", "-C", os.path.join(HERE, "csrc"), "-j8"])
     with open(SO_PATH + ".srchash", "w") as f:
         f.write(source_hash() + "\n")

@@ -8,7 +8,7 @@ static char g_init_error[512] = {0};
 uint32_t lb200_cull_lanes() {
 	static const uint32_t lanes = [] {
 		const char* e = getenv("LB200_CULL_LANES");
-		const int v = e ? atoi(e) : 3;
+		const int v = e ? atoi(e) : 2; // H100: 2 lanes x 2 blocks/SM beat 3 / 4 / 6 lanes (DESIGN.md 4.1)
 		return (uint32_t)(v < 1 ? 1 : (v > LB200_MAX_LANES ? LB200_MAX_LANES : v));
 	}();
 	return lanes;

@@ -85,7 +85,7 @@ struct EmitParams {
 	lb200_sk_view view;
 	uint32_t type_base[4]; // offsets of the MESH / DECAL / LOCAL_LIGHT / CURVE_DECAL segments inside out_ids
 	uint32_t cap_keys, cap_recs, cap_pose, cap_dirty;
-	uint32_t prefetch_ahead; // records requested into L2 this many grid strides ahead of their use (0 = off; LB200_SK_PREFETCH, default 1)
+	uint32_t prefetch_ahead; // records requested into L2 this many grid strides ahead of their use (0 = off; LB200_SK_PREFETCH, default 0)
 };
 
 // :57-60
@@ -955,7 +955,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	EP.view = *view;
 	for (int t = 0; t < 4; ++t) EP.type_base[t] = type_base[t];
 	EP.cap_keys = sk->cap_keys; EP.cap_recs = sk->cap_recs; EP.cap_pose = sk->max_entities; EP.cap_dirty = sk->max_entities;
-	static const uint32_t prefetch_ahead = [] { const char* e = getenv("LB200_SK_PREFETCH"); const int v = e ? atoi(e) : 1; return (uint32_t)std::max(0, std::min(v, 4)); }();
+	static const uint32_t prefetch_ahead = [] { const char* e = getenv("LB200_SK_PREFETCH"); const int v = e ? atoi(e) : 0; return (uint32_t)std::max(0, std::min(v, 4)); }(); // off: on H100 the prefetch slows the pass (DESIGN.md 4.5)
 	EP.prefetch_ahead = prefetch_ahead;
 	const bool in_smem = n_groups <= SK_SMEM_GROUPS;
 	size_t smem = in_smem ? sizeof(uint32_t) * n_groups : 0;
@@ -965,7 +965,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 		if (rc) return rc;
 	}
 	const uint32_t work = type_counts[RT_MESH] + type_counts[RT_DECAL] + type_counts[RT_CURVE_DECAL]; // upper bound of visible renderables
-	static const uint32_t blocks_per_sm = [] { const char* e = getenv("LB200_SK_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 0; return (uint32_t)std::max(0, v); }(); // tuning: fewer resident blocks than fit
+	static const uint32_t blocks_per_sm = [] { const char* e = getenv("LB200_SK_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 2; return (uint32_t)std::max(0, v); }(); // fewer resident blocks than fit (0 = all): 2 is fastest on H100
 	uint32_t grid = std::max(1u, std::min(blocks_per_sm ? std::min(limit, blocks_per_sm * (uint32_t)ctx->sm_count) : limit, (work + SK_THREADS - 1) / SK_THREADS));
 	EmitArgs EA = {sk->d_ent, sk->d_decal_sort_key, sk->d_decal_layer, sk->d_models, sk->d_meshes, sk->d_keys[0], sk->d_values[0], sk->d_counts,
 		sk->d_group_count, sk->d_group_offset, sk->d_group_cursor, sk->d_group_layer, sk->d_group_renderables, sk->d_instance_data, sk->d_pose_list, sk->d_dirty_list, sk->d_stash, sk->d_stash4, sk->max_entities, sk->d_bar};
