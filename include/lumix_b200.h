@@ -292,6 +292,14 @@ LB200_API int lb200_sortkeys_move_device(lb200_sortkeys* sk, const int32_t* dev_
  * since the last call; lb200_sortkeys_prev_transforms hands out the per-entity device array of those transforms. */
 LB200_API int lb200_sortkeys_end_frame(lb200_sortkeys* sk);
 LB200_API int lb200_sortkeys_prev_transforms(lb200_sortkeys* sk, const lb200_transform** dev_prev);
+/* The stable LSD radix sort create_keys and the device re-binning use, on caller device buffers, on the context stream: sorts
+ * n = min(*dev_count, cap) (u64 key, u64 value) pairs in place (the count is read on the device, like the two callers do).
+ * max_blocks caps the cooperative grid (0 = as many as are co-resident; the grid is also at most ceil(cap / 2048)); force_tiled != 0 takes
+ * the tiled path at any n.  The register path is taken iff !force_tiled && n <= grid * 512 * 16.  *out_grid (may be NULL) = blocks launched.
+ * Entries [n, cap) are left untouched.  The scratch is kept in the context, grows to the largest cap (waiting for the stream when it
+ * does) and is freed by lb200_shutdown. */
+LB200_API int lb200_radix_sort_device(lb200_ctx* ctx, uint64_t* dev_keys, uint64_t* dev_values, const uint32_t* dev_count, uint32_t cap, uint32_t max_blocks,
+                                      int force_tiled, uint32_t* out_grid);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Multi-GPU (one process per GPU; SURVEY.md §8e).  NCCL is dlopen()ed; the unique id travels through the caller

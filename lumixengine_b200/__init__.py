@@ -12,5 +12,5 @@ from ._lib import (Context, LumixB200Error, NoDeviceError, PALETTE_DUAL_QUAT, PA
 from .culling import CullingSystem, CullResult, frustum_from_viewport, frustum_ortho, frustum_perspective  # noqa: F401
 from .hierarchy import Hierarchy, TRANSFORM_DTYPE  # noqa: F401
 from .animation import AnimationClip, AnimationSystem, SkinnedMesh, Skeleton  # noqa: F401
-from .sortkeys import SortKeys  # noqa: F401
+from .sortkeys import SortKeys, radix_sort  # noqa: F401
 from . import sortkeys  # noqa: F401

@@ -77,6 +77,7 @@ void lb200_shutdown(lb200_ctx* ctx) {
 	cudaSetDevice(ctx->device);
 	if (ctx->stream) { cudaStreamSynchronize(ctx->stream); cudaStreamDestroy(ctx->stream); }
 	if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
+	cudaFree(ctx->sort_scratch);
 	delete ctx;
 }
 

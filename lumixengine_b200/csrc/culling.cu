@@ -1866,7 +1866,7 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 			cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, cs->hash_cap);
 		LB200_CHECK_LAUNCH(ctx);
 		rc = lb200_radix_sort_pairs(ctx, s, cs->d_rb_keys[0], cs->d_rb_keys[1], cs->d_rb_vals[0], cs->d_rb_vals[1], C + RB_N_CHANGERS, cs->changers_cap, cs->d_rb_sort_state,
-			cs->d_rb_block_hist, cs->rb_sort_blocks);
+			cs->d_rb_block_hist, cs->rb_sort_blocks, false, nullptr);
 		if (rc) return rc;
 		LB200_CUDA(ctx, cudaMemsetAsync(C + RB_WORDS - 1, 0, sizeof(uint32_t), s)); // the new-page cursor of this batch
 		rebin_plan_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 8u, (n_changers + 127) / 128)), 128, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, dev_pos3, cs->d_desc,

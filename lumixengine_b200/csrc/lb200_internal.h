@@ -22,6 +22,9 @@ struct lb200_ctx {
 	int sm_count = 0;
 	std::atomic<uint64_t> launches{0};
 	char error[512] = {0};
+	// scratch of lb200_radix_sort_device (sortkeys.cu) for up to sort_scratch_cap pairs; freed by lb200_shutdown
+	void* sort_scratch = nullptr;
+	uint32_t sort_scratch_cap = 0;
 	// NCCL (dlopen) state, see comm.cu
 	void* nccl_lib = nullptr;
 	void* nccl_comm = nullptr;
@@ -63,10 +66,11 @@ struct lb200_range {
 };
 // culling.cu: where the last cull left its result (device: ids, counters; host: per-type segment bases and entity counts, 256 each)
 int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, const uint32_t** counters, const uint32_t** type_base, const uint32_t** type_counts);
-// sortkeys.cu: stable LSD radix sort of (u64 key, u64 value) pairs, count read on the device; the result ends in buffer 0
+// sortkeys.cu: stable LSD radix sort of (u64 key, u64 value) pairs, count read on the device; the result ends in buffer 0.
+// force_tiled: the tiled path at any n (the register path is taken iff !force_tiled && n <= grid * 512 * 16); *out_grid (may be null) = blocks launched
 size_t lb200_radix_sort_state_bytes();
 int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t stream, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
-	void* state, uint32_t* block_hist, uint32_t blocks);
+	void* state, uint32_t* block_hist, uint32_t blocks, bool force_tiled, uint32_t* out_grid);
 int lb200_comm_check(lb200_ctx* ctx); // comm.cu: LB200_ERR_NCCL (and reset) if a peer wait timed out since the last check
 uint32_t lb200_cull_lanes(); // LB200_CULL_LANES, default 2, 1..LB200_MAX_LANES (context.cu)
 

@@ -728,22 +728,71 @@ int coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem
 
 // Stable LSD radix sort of n = min(*count_dev, cap) (key, value) pairs of 64 bits, one cooperative launch on `stream`, n read on the device.
 // The sorted pairs end in buffer 0.  state: lb200_radix_sort_state_bytes() bytes, block_hist: 256 x blocks words; at most `blocks` blocks
-// are launched.  (Also used by the device re-binning of the culling structure, culling.cu.)
+// are launched.  force_tiled: the tiled path at any n.  *out_grid (may be null): the blocks launched.  (Also used by the device re-binning
+// of the culling structure, culling.cu, and by lb200_radix_sort_device.)
 size_t lb200_radix_sort_state_bytes() { return sizeof(SortState); }
 
-int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t s, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
-	void* state, uint32_t* block_hist, uint32_t blocks)
-{
+static int radix_sort_grid_limit(lb200_ctx* ctx, uint32_t* out) {
 	static uint32_t limit = 0; // blocks of radix_sort_kernel that are co-resident (one device kind per process)
 	if (!limit) { const int rc = coop_grid_limit(ctx, (const void*)radix_sort_kernel, RS_THREADS, 0, &limit); if (rc) return rc; }
+	*out = limit;
+	return LB200_OK;
+}
+
+int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t s, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
+	void* state, uint32_t* block_hist, uint32_t blocks, bool force_tiled, uint32_t* out_grid)
+{
+	uint32_t limit = 0;
+	const int rc = radix_sort_grid_limit(ctx, &limit);
+	if (rc) return rc;
 	SortState* st = (SortState*)state;
 	LB200_CUDA(ctx, cudaMemsetAsync(st, 0, sizeof(SortState), s));
 	uint32_t grid = std::max(1u, std::min(std::min(limit, blocks), (cap + RS_TILE - 1) / RS_TILE));
-	static const uint32_t reg_items = [] { const char* e = getenv("LB200_SORT_TILED"); return (e && atoi(e) != 0) ? 0u : (uint32_t)RS_REG_ITEMS; }(); // LB200_SORT_TILED=1: always the tiled path
-	uint32_t reg_items_arg = reg_items;
-	void* args[] = {&keys0, &keys1, &values0, &values1, &count_dev, &cap, &st, &block_hist, &reg_items_arg};
+	uint32_t reg_items = force_tiled ? 0u : (uint32_t)RS_REG_ITEMS;
+	void* args[] = {&keys0, &keys1, &values0, &values1, &count_dev, &cap, &st, &block_hist, &reg_items};
 	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)radix_sort_kernel, dim3(grid), dim3(RS_THREADS), args, 0, s));
 	LB200_CHECK_LAUNCH(ctx);
+	if (out_grid) *out_grid = grid;
+	return LB200_OK;
+}
+
+// Scratch of lb200_radix_sort_device, kept in the context and grown to the largest cap asked for: the second key / value buffers,
+// then the SortState and the block histograms of the largest grid.
+struct SortScratch { uint64_t* keys1; uint64_t* values1; SortState* state; uint32_t* block_hist; };
+static size_t sort_scratch_bytes(uint32_t cap, uint32_t blocks) { return 2 * sizeof(uint64_t) * (size_t)cap + sizeof(SortState) + sizeof(uint32_t) * 256 * (size_t)blocks; }
+static SortScratch sort_scratch_at(void* base, uint32_t cap) {
+	char* p = (char*)base;
+	SortScratch s;
+	s.keys1 = (uint64_t*)p;
+	s.values1 = (uint64_t*)(p + sizeof(uint64_t) * (size_t)cap);
+	s.state = (SortState*)(p + 2 * sizeof(uint64_t) * (size_t)cap);
+	s.block_hist = (uint32_t*)(s.state + 1);
+	return s;
+}
+
+extern "C" int lb200_radix_sort_device(lb200_ctx* ctx, uint64_t* dev_keys, uint64_t* dev_values, const uint32_t* dev_count, uint32_t cap, uint32_t max_blocks, int force_tiled,
+	uint32_t* out_grid)
+{
+	if (!ctx || !dev_keys || !dev_values || !dev_count) return LB200_ERR_INVALID;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	uint32_t limit = 0;
+	int rc = radix_sort_grid_limit(ctx, &limit);
+	if (rc) return rc;
+	const uint32_t scratch_cap = std::max(cap, 1u);
+	if (scratch_cap > ctx->sort_scratch_cap) { // the stream may still use the old scratch
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		cudaFree(ctx->sort_scratch);
+		ctx->sort_scratch = nullptr;
+		ctx->sort_scratch_cap = 0;
+		LB200_CUDA(ctx, cudaMalloc(&ctx->sort_scratch, sort_scratch_bytes(scratch_cap, limit)));
+		ctx->sort_scratch_cap = scratch_cap;
+	}
+	const SortScratch sc = sort_scratch_at(ctx->sort_scratch, ctx->sort_scratch_cap);
+	uint32_t grid = 0;
+	rc = lb200_radix_sort_pairs(ctx, ctx->stream, dev_keys, sc.keys1, dev_values, sc.values1, dev_count, cap, sc.state, sc.block_hist, max_blocks ? max_blocks : limit,
+		force_tiled != 0, &grid);
+	if (rc) return rc;
+	if (out_grid) *out_grid = grid;
 	return LB200_OK;
 }
 
@@ -974,7 +1023,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	LB200_CHECK_LAUNCH(ctx);
 	if (sort) {
 		lb200_range r2("radixSort"); // pipeline.cpp:4101
-		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->d_sort_state, sk->d_block_hist, sk->sort_blocks);
+		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->d_sort_state, sk->d_block_hist, sk->sort_blocks, false, nullptr);
 		if (rc) return rc;
 	}
 	if (want_counts) {

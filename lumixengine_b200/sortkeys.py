@@ -40,6 +40,31 @@ def make_view(camera_pos, lod_ref_point, time_delta, lod_multiplier, frame_numbe
     return v
 
 
+def radix_sort_device(ctx, dev_keys, dev_values, dev_count, cap, max_blocks=0, tiled=False):
+    """lb200_radix_sort_device: enqueues the stable sort of min(*dev_count, cap) (u64 key, u64 value) pairs in place on the context stream
+    (device pointers as ints) and returns the blocks launched.  Nothing waits unless the context's scratch has to grow to `cap`."""
+    grid = C.c_uint32()
+    check(ctx.L.lb200_radix_sort_device(ctx.h, vp(dev_keys), vp(dev_values), vp(dev_count), C.c_uint32(cap), C.c_uint32(max_blocks), C.c_int(1 if tiled else 0),
+                                        C.byref(grid)), ctx.h)
+    return int(grid.value)
+
+
+def radix_sort(ctx, keys, values, count=None, max_blocks=0, tiled=False):
+    """The device sort on host arrays of `cap = len(keys)` pairs: sorts the first min(count, cap) (count defaults to cap) and leaves the rest.
+    -> (keys, values, grid): host copies of all cap pairs after the sort, and the blocks launched."""
+    keys = np.ascontiguousarray(keys, np.uint64)
+    values = np.ascontiguousarray(values, np.uint64)
+    assert keys.shape == values.shape and keys.ndim == 1
+    cap = len(keys)
+    dev = [ctx.to_device(a) for a in (keys, values, np.array([cap if count is None else count], np.uint32))]
+    try:
+        grid = radix_sort_device(ctx, dev[0], dev[1], dev[2], cap, max_blocks, tiled)
+        return ctx.copy_to_host(dev[0], cap, np.uint64), ctx.copy_to_host(dev[1], cap, np.uint64), grid
+    finally:
+        for p in dev:
+            ctx.free_device(p)
+
+
 class SortKeys:
     def __init__(self, ctx, max_entities, max_groups, max_keys=0, max_instances=0):
         self.ctx, self.L = ctx, ctx.L

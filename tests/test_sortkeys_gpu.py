@@ -66,10 +66,10 @@ def test_sort_keys_match_oracle_over_frames(ctx, oracle, n, seed, is_shadow, key
     cs.close()
 
 
-def test_device_radix_sort_alone(ctx, oracle):
-    """Many equal keys, all 64 bits in play, sizes around the tile and block boundaries: sorted and a permutation of the input."""
-    rng = np.random.default_rng(8)
-    n = 50_000
+def _sort_createsortkeys_output(ctx, n):
+    """createSortKeys with its sort on a scene of n entities, all MOVED and all visible (few distinct keys in long runs, bucket << 56 | mesh
+    sort key): the keys come out sorted and the (key, value) pairs are a permutation of the unsorted output of the same pass.  The order among
+    equal keys is not checked here (the unsorted order is not reproducible); tests/test_radix_sort_gpu.py checks stability.  -> n_keys"""
     scene = scenes.cull_scene(n, (400.0, 100.0, 400.0), seed=2, type_probs=(1.0,))
     # every entity MOVED -> one key per visible mesh, keys = mesh sort key | bucket << 56: few distinct keys, long runs
     sk = scenes.sortkey_setup(n, scene["types"], scene["pos"], n_models=6, seed=9, skinned_fraction=0.0, moved_fraction=1.1, dirty_fraction=0.0)
@@ -95,6 +95,22 @@ def test_device_radix_sort_alone(ctx, oracle):
     assert len(np.unique(got["keys"])) < 100
     S.close()
     cs.close()
+    return res.n_keys
+
+
+def test_device_radix_sort_alone(ctx):
+    """The sort behind createSortKeys on the keys of a 50 k-entity scene (register path): sorted and a permutation of the unsorted pass."""
+    _sort_createsortkeys_output(ctx, 50_000)
+
+
+def test_device_radix_sort_tiled_through_create_sort_keys(ctx):
+    """The same on a 1.5 M-entity scene whose keys are more than the register path holds, so that createSortKeys' sort takes the tiled path."""
+    n_keys = _sort_createsortkeys_output(ctx, 1_500_000)
+    # createSortKeys launches as many sort blocks as are co-resident, like an unconstrained lb200_radix_sort_device: above grid * 8192 keys
+    # the tiled path sorts
+    cap = 1 << 20
+    _, _, grid = lb.radix_sort(ctx, np.zeros(cap, np.uint64), np.zeros(cap, np.uint64), count=0)
+    assert n_keys > grid * 512 * 16, f"{n_keys} keys stay on the register path of a {grid}-block sort"
 
 
 def test_pose_to_attachment_to_cull_chain_on_device(ctx, oracle):
