@@ -525,7 +525,7 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 					// lane and immediate offsets per row — no ballots, no ranks
 					const int* src = ep + lane;
 					uint32_t* d = dst + lane;
-					int id[ROWS];
+					int id[ROWS] = {}; // zeroed per page: unassigned elements were otherwise kept live across pages, and spilled
 #pragma unroll
 					for (int k = 0; k < ROWS; ++k) if ((uint32_t)(k * 32 + lane) < count) id[k] = ldg_stream_i32(src + k * 32);
 #pragma unroll
@@ -537,7 +537,7 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 					uint32_t bal[ROWS];
 #pragma unroll
 					for (int k = 0; k < ROWS; ++k) bal[k] = s_bal[iw][k];
-					int id[ROWS];
+					int id[ROWS] = {}; // zeroed per page: unassigned elements were otherwise kept live across pages, and spilled
 #pragma unroll
 					for (int k = 0; k < ROWS; ++k) if ((bal[k] >> lane) & 1u) id[k] = ldg_stream_i32(ep + k * 32 + lane);
 					uint32_t prefix = 0;

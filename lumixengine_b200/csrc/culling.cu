@@ -651,8 +651,10 @@ void parseCounts(lb200_culling* cs, lb200_cull_result* result) {
 	res.entities_tested = cs->h_counters[256 + ST_ENT_TESTED];
 	res.entities_inside = cs->h_counters[256 + ST_ENT_INSIDE];
 	cs->has_last = true;
-	// DESIGN.md §4: descriptor per page + 16 B per tested sphere + (4 B id read + 4 B id write) per visible + 32 B mask per page
-	cs->last_bytes = (uint64_t)cs->last_pages * 32 + (uint64_t)res.entities_tested * 16 + (uint64_t)res.total * 8 + (uint64_t)cs->last_pages * 32;
+	// DESIGN.md §4.1: descriptor per page + 16 B per sphere the kernel reads (pages left to test after plane masking) + (4 B id read +
+	// 4 B id write) per visible + 32 B mask per page
+	const uint64_t streamed = cs->h_counters[256 + ST_ENT_STREAMED];
+	cs->last_bytes = (uint64_t)cs->last_pages * 32 + streamed * 16 + (uint64_t)res.total * 8 + (uint64_t)cs->last_pages * 32;
 	if (result) *result = res;
 }
 
