@@ -213,9 +213,6 @@ LB200_API uint32_t lb200_culling_last_rebin_changers(const lb200_culling* cs);
  * device reaches it (no host launch latency inside the interval, nothing overlapping the cull).  mode 0 = the cull, 1 = nothing between
  * the two event records, 2 = one empty kernel of the cull's grid (the fixed costs the first number contains). */
 LB200_API int lb200_culling_time_lone_cull(lb200_culling* cs, const lb200_shifted_frustum* frustum, uint8_t type, uint32_t iters, int mode, float* out_ms);
-/* Profiling aid: %globaltimer stamps (ns) of the phase boundaries of the last cull issued while LB200_CULL_TRACE=1 was set:
- * out[2 kernels][2048 blocks][8 points] (cull_kernel.cuh trace_point). */
-LB200_API int lb200_culling_read_trace(lb200_culling* cs, uint64_t* out);
 LB200_API uint64_t lb200_culling_last_algorithmic_bytes(const lb200_culling* cs);
 
 /* ------------------------------------------------------------------------------------------------------------
@@ -343,7 +340,7 @@ LB200_API uint32_t lb200_culling_gather_stride_words(const lb200_culling* cs, ui
 LB200_API int lb200_culling_cull_exchange(lb200_culling* cs, const lb200_shifted_frustum* frustum, uint8_t type, const uint32_t** out_dev_ids,
                                           const uint32_t** out_dev_slabs, uint32_t* out_slab_stride_words);
 /* n independent exchange steps issued from one call: step (epoch) e runs on internal stream e % lanes on every rank, so the remote
- * stores, fences and flag round trip of one step overlap the culls of its neighbours (2 x lanes exchange buffers per rank).  Forks
+ * stores, fences and flag round trip of one step overlap the culls of its neighbours (3 x lanes exchange buffers per rank).  Forks
  * from and joins back into the context stream; the out parameters describe the LAST step. */
 LB200_API int lb200_culling_cull_exchange_n(lb200_culling* cs, const lb200_shifted_frustum* frustum, uint8_t type, uint32_t n,
                                             const uint32_t** out_dev_ids, const uint32_t** out_dev_slabs, uint32_t* out_slab_stride_words);

@@ -9,9 +9,7 @@
 //       ShiftedFrustum::containsAABB / intersectsAABB arithmetic (geometry.cpp:99-118,159-178), the plane mask, and for pages that need
 //       sphere tests the plane offsets re-based to the cell origin (ShiftedFrustum::getRelative, geometry.cpp:121-149 — only d
 //       changes); pages with work go to a block-local list in shared memory.
-//   B   test, one WARP per listed page: the <=200 spheres as 7 x 128-bit streaming loads per lane (default, STAGE_DEPTH = 0) or staged in
-//       shared memory through the bulk-copy engine (STAGE_DEPTH = 1 | 2: TMA, cp.async.bulk + mbarrier, up to two pages in flight per warp;
-//       measured slower on 3.2 KB pages, LB200_CULL_STAGE); the planes of the mask are walked by a
+//   B   test, one WARP per listed page: the <=200 spheres as 7 x 128-bit streaming loads per lane; the planes of the mask are walked by a
 //       warp-uniform loop with the rows unrolled inside (no branch per sphere; rows 4-6 only for pages with more than 128 spheres), the
 //       reference's op order and sign-bit test (culling_system.cpp:284-295, simd.h:119); ballots kept in shared memory.
 //   C   claim: one global atomic per (warp, renderable type) reserves the output range of the warp's pages.
@@ -55,11 +53,10 @@ struct CullParams {
 	uint32_t chunk;         // pages per block per round, <= MAX_CHUNK
 	uint32_t plane_masking; // 1 unless some sphere has a negative / NaN radius
 	uint32_t item_cap;      // record capacity of an exchange slab (>= n_pages)
-	uint32_t trace;         // profiling: stamp phase boundaries into g_trace
 	// exchange mode (n_ranks > 0): {page, row} records go straight into every rank's slab (peer memory)
 	uint32_t n_ranks;
 	uint32_t* xdst[LB200_MAX_RANKS]; // rank r's exchange buffer of this epoch, already offset to MY slab inside it
-	// fused exchange steps (one kernel per step, lb200_culling_cull_exchange_n with LB200_EXCHANGE_FUSED): this cull also publishes the lane's
+	// fused exchange steps (one kernel per step, lb200_culling_cull_exchange_n on two or more lanes): this cull also publishes the lane's
 	// PREVIOUS epoch (pub_epoch != 0) and holds its record stores back until every rank has published wait_epoch (!= 0)
 	uint32_t pub_epoch, wait_epoch, n_buffers, rank;
 	uint32_t* xprev[LB200_MAX_RANKS];  // rank r's exchange buffer of pub_epoch, offset to MY slab
@@ -75,39 +72,7 @@ __device__ __forceinline__ int ldg_stream_i32(const int* p) {
 	return r;
 }
 
-// ---- shared-memory staging with the bulk-copy engine (TMA, 1-D form) ----
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-	uint32_t done;
-	do {
-		asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-	} while (!done);
-}
-// global -> shared, `bytes` a multiple of 16, both addresses 16-byte aligned; completion is counted on the mbarrier
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-
 enum { CLS_SKIP = 0, CLS_COPY = 1, CLS_TEST = 2 };
-
-// Profiling aid (LB200_CULL_TRACE=1, lb200_culling_read_trace): thread 0 of every block stamps %globaltimer at the phase boundaries.
-constexpr int TRACE_BLOCKS = 2048, TRACE_POINTS = 8;
-__device__ unsigned long long g_trace[2][TRACE_BLOCKS][TRACE_POINTS];
-__device__ __forceinline__ void trace_point(uint32_t on, int kernel, int point) {
-#ifdef LB200_CULL_TRACE_BUILD // make NVFLAGS+=-DLB200_CULL_TRACE_BUILD: the stamps cost ~4 % of the kernel's instructions, so they are not in the default build
-	if (on && threadIdx.x == 0 && blockIdx.x < TRACE_BLOCKS) {
-		unsigned long long t;
-		asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-		g_trace[kernel][blockIdx.x][point] = t;
-	}
-#endif
-}
 
 struct WorkItem { // 32 B
 	uint32_t page;
@@ -116,22 +81,16 @@ struct WorkItem { // 32 B
 };
 static_assert(sizeof(WorkItem) == 32, "");
 
-// STAGE_DEPTH = pages in flight per warp through the bulk-copy engine; 0 = the sphere rows are loaded straight into registers
-// (ld.global.nc, 7 x 128 bit per lane).  Dynamic shared memory = the staged rows.
-constexpr size_t cull_smem_bytes(int stage_depth) { return sizeof(float4) * LB200_PAGE_SLOTS * (size_t)stage_depth * CULL_WARPS; }
-
 __device__ __forceinline__ float4 ldg_stream(const float4* p) {
 	float4 r;
 	asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
 	return r;
 }
 
-template <int STAGE_DEPTH>
-__global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_pages_kernel(const __grid_constant__ CullParams P,
+__global__ void __launch_bounds__(CULL_THREADS, 4) cull_pages_kernel(const __grid_constant__ CullParams P,
 	const lb200_page_desc* __restrict__ desc, const float4* __restrict__ spheres, const int* __restrict__ entities,
 	uint32_t* __restrict__ out_ids, uint32_t* __restrict__ counters, uint32_t* __restrict__ next_counters, uint32_t* __restrict__ mask_out)
 {
-	extern __shared__ __align__(128) unsigned char s_dyn[];
 	__shared__ WorkItem s_item[MAX_CHUNK];
 	__shared__ __align__(16) uint32_t s_bal[MAX_CHUNK][ROWS + 1]; // the 256-bit visibility row of a tested page ([ROWS] = 0)
 	__shared__ uint32_t s_off[MAX_CHUNK];                         // visible ids of the page, then its offset inside out_ids
@@ -139,7 +98,6 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 	__shared__ uint32_t s_stats[N_STATS];
 	__shared__ uint32_t s_zpage[MAX_CHUNK]; // page whose mask row is zero (ends without work), or ~0
 	__shared__ uint32_t s_ntest, s_ncopy, s_ncand;
-	__shared__ __align__(8) uint64_t s_bar[CULL_WARPS][STAGE_DEPTH > 0 ? STAGE_DEPTH : 1];
 
 	// let the next cull of the stream start its read-only prologue as soon as SM resources free up
 	cudaTriggerProgrammaticLaunchCompletion();
@@ -148,20 +106,10 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 	const int lane = tid & 31;
 	const int warp = tid >> 5;
 	const uint32_t lt_mask = (1u << lane) - 1u;
-	float4* stage = reinterpret_cast<float4*>(s_dyn) + (size_t)warp * STAGE_DEPTH * LB200_PAGE_SLOTS;
 
 	if (tid < N_STATS) s_stats[tid] = 0;
 	if (tid == 0) { s_ntest = 0; s_ncopy = 0; s_ncand = 0; }
-	if (STAGE_DEPTH > 0) {
-		if (lane == 0) {
-#pragma unroll
-			for (int b = 0; b < STAGE_DEPTH; ++b) mbar_init(smem_u32(&s_bar[warp][b]), 1);
-		}
-		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	}
 	__syncthreads();
-	uint32_t parity = 0; // bit b: phase parity of stage barrier b
-	trace_point(P.trace, 0, 0);
 
 	// Pages are dealt to blocks round-robin (page = j * gridDim + block): pages that always need sphere tests (is_big cells) and
 	// frustum-boundary cells cluster in page-id space, and contiguous chunks left a few blocks with twice the work of the rest.
@@ -218,7 +166,6 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 			s_zpage[tid] = zpage;
 		}
 		__syncthreads();
-		trace_point(P.trace, 0, 1);
 
 		// ---------------- A2. exact classification of the candidates (dense threads) ----------------
 		if ((uint32_t)tid < s_ncand) {
@@ -313,32 +260,13 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 			else s_zpage[t0] = page;
 		}
 		__syncthreads();
-		trace_point(P.trace, 0, 2);
 		const uint32_t n_test = s_ntest;
 		const uint32_t n_work = n_test + s_ncopy;
 		// listed page w: s_item[item_index(w)] — the COPY pages sit at the back of the array
 #define LB_ITEM(w) ((w) < n_test ? (w) : (uint32_t)MAX_CHUNK - 1u - ((w) - n_test))
 
 		// ---------------- B. sphere tests: one warp per listed TEST page (w = warp, warp + CULL_WARPS, ... < n_test) ----------------
-		// STAGE_DEPTH > 0: the rows are staged in shared memory by the bulk-copy engine, up to STAGE_DEPTH pages in flight per warp.
 		{
-			uint32_t next_load = warp; // next listed page whose spheres have not been requested
-			uint32_t in_flight = 0, head = 0, tail = 0; // ring of stage buffers: tail = next to fill, head = next to consume
-			auto issue = [&]() {
-				if (STAGE_DEPTH == 0) return;
-				while (in_flight < (uint32_t)STAGE_DEPTH && next_load < n_test) {
-					if (lane == 0) {
-						const uint32_t bar = smem_u32(&s_bar[warp][tail]);
-						const uint32_t bytes = (s_item[next_load].meta & 0xffu) * 16u;
-						mbar_expect_tx(bar, bytes);
-						bulk_load(smem_u32(stage + (size_t)tail * LB200_PAGE_SLOTS), spheres + (size_t)s_item[next_load].page * LB200_PAGE_SLOTS, bytes, bar);
-					}
-					tail = tail + 1 == (uint32_t)STAGE_DEPTH ? 0 : tail + 1;
-					++in_flight;
-					next_load += CULL_WARPS;
-				}
-			};
-			issue();
 			for (uint32_t iw = warp; iw < n_test; iw += CULL_WARPS) {
 				const uint4 ia = *reinterpret_cast<const uint4*>(&s_item[iw]);
 				const uint32_t count = ia.y & 0xffu;
@@ -346,31 +274,13 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 				const uint32_t need = ia.y >> 24;
 				const bool upper = count > 128u; // rows 4-6 exist (warp-uniform): half of the tested pages of a typical scene stop before
 				float4 s[ROWS];
-				if (STAGE_DEPTH > 0) {
-					const float4* sp = stage + (size_t)head * LB200_PAGE_SLOTS;
-					mbar_wait(smem_u32(&s_bar[warp][head]), (parity >> head) & 1u);
+				const float4* sp = spheres + (size_t)ia.x * LB200_PAGE_SLOTS;
+				const uint32_t last = count - 1u; // count >= 1 for listed pages
 #pragma unroll
-					for (int k = 0; k < 4; ++k) s[k] = sp[k * 32 + lane]; // slots past `count` hold stale rows: masked at the ballot
-					if (upper) {
+				for (int k = 0; k < 4; ++k) { const uint32_t slot = k * 32 + lane; s[k] = ldg_stream(sp + (slot < last ? slot : last)); } // lanes past the page re-read its last sphere
+				if (upper) {
 #pragma unroll
-						for (int k = 4; k < ROWS; ++k) { const int slot = k * 32 + lane; s[k] = sp[slot < LB200_PAGE_SLOTS ? slot : LB200_PAGE_SLOTS - 1]; }
-					}
-					// the rows are in registers: the stage buffer can take the next page
-					__syncwarp();
-					parity ^= 1u << head;
-					head = head + 1 == (uint32_t)STAGE_DEPTH ? 0 : head + 1;
-					--in_flight;
-					issue();
-				}
-				else {
-					const float4* sp = spheres + (size_t)ia.x * LB200_PAGE_SLOTS;
-					const uint32_t last = count - 1u; // count >= 1 for listed pages
-#pragma unroll
-					for (int k = 0; k < 4; ++k) { const uint32_t slot = k * 32 + lane; s[k] = ldg_stream(sp + (slot < last ? slot : last)); } // lanes past the page re-read its last sphere
-					if (upper) {
-#pragma unroll
-						for (int k = 4; k < ROWS; ++k) { const uint32_t slot = k * 32 + lane; s[k] = ldg_stream(sp + (slot < last ? slot : last)); }
-					}
+					for (int k = 4; k < ROWS; ++k) { const uint32_t slot = k * 32 + lane; s[k] = ldg_stream(sp + (slot < last ? slot : last)); }
 				}
 				if (!upper) {
 #pragma unroll
@@ -443,7 +353,7 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 		}
 		// nothing above wrote global memory (A and B read scene data, results sit in shared memory); everything below does
 		// (counters, ids, mask rows) and has to wait for the previous kernel of the stream
-		if (round == 0) { trace_point(P.trace, 0, 3); cudaGridDependencySynchronize(); trace_point(P.trace, 0, 4); }
+		if (round == 0) cudaGridDependencySynchronize();
 		if (round == 0 && P.n_ranks && (P.pub_epoch | P.wait_epoch)) {
 			// Fused exchange step.  Behind the grid dependency the lane's previous cull is complete: its records lie in the peers' slabs, its
 			// counters still in `next_counters` (zeroed at the end of THIS kernel, behind the round barrier every warp of block 0 passes).
@@ -563,7 +473,6 @@ __global__ void __launch_bounds__(CULL_THREADS, STAGE_DEPTH >= 2 ? 3 : 4) cull_p
 		if (tid == 0) { s_ntest = 0; s_ncopy = 0; s_ncand = 0; }
 		__syncthreads();
 	}
-	trace_point(P.trace, 0, 5);
 
 	if (tid < N_STATS && s_stats[tid]) atomicAdd(&counters[256 + tid], s_stats[tid]);
 	// the other counter buffer is the next cull's: zero it now so no memset sits between two culls

@@ -12,7 +12,6 @@
 #include <string.h>
 
 #define LB200_MAX_RANKS 8
-#define LB200_CULL_STAGE_DEFAULT 0 // pages in flight per warp through the bulk-copy engine (cull_kernel.cuh); LB200_CULL_STAGE overrides
 #define LB200_MAX_LANES 8  // concurrent culls (streams / output lanes); exchange buffers = 3 x lanes
 
 struct lb200_ctx {
@@ -34,12 +33,14 @@ struct lb200_ctx {
 	struct Peer {
 		bool ready = false;
 		size_t slab_words = 0;            // capacity of one rank's slab (header + ids)
-		// Exchange epoch e uses buffer e % n_buffers, n_buffers = 3 x lanes.  With lanes > 1 (lb200_culling_cull_exchange_n) epoch e is
-		// issued on stream e % lanes as ONE kernel: the cull of e publishes the lane's previous epoch (e - lanes) from its prologue and
-		// holds its record stores back until every rank has published e - 2 x lanes.  So a rank overwrites buffer b for epoch e only after
-		// every rank published e - 2 x lanes, which a rank does from its cull of e - lanes — issued behind whatever consumed e - 3 x lanes,
-		// the previous owner of b.  tests/test_exchange_protocol_model.py replays this (and the two-kernel forms culling.cu keeps as
-		// options) under a random scheduler, and shows that fewer buffers or no flow control would not do.
+		// Exchange epoch e uses buffer e % n_buffers, n_buffers = 3 x lanes.  A batch of lb200_culling_cull_exchange_n with lanes > 1 and
+		// n > 1 issues epoch e on stream e % lanes as ONE kernel: the cull of e publishes the lane's previous epoch (e - lanes) from its
+		// prologue and holds its record stores back until every rank has published e - 2 x lanes.  So a rank overwrites buffer b for epoch
+		// e only after every rank published e - 2 x lanes, which a rank does from its cull of e - lanes — issued behind whatever consumed
+		// e - 3 x lanes, the previous owner of b.  Every other step (lb200_culling_cull_exchange, and batches with one lane or one step)
+		// runs on the context stream as the cull followed by publish_wait_kernel, after everything issued before it has finished waiting.
+		// tests/test_exchange_protocol_model.py replays both kinds, mixed as callers issue them, under a random scheduler, and shows that
+		// fewer buffers or no flow control would not do.
 		uint32_t lanes = 1, n_buffers = 3;
 		void* local_block = nullptr;      // this rank's allocation: [flags n_buffers x 8 x u32 in 512 B][gather 0] .. [gather n_buffers-1]
 		uint32_t* gather[3 * LB200_MAX_LANES][LB200_MAX_RANKS] = {}; // gather[b][r] = rank r's buffer b as seen from this process

@@ -418,19 +418,3 @@ def test_device_rebinning_equals_host_set(ctx, oracle):
                 alive[gone] = False
             assert np.array_equal(seen, alive)
     cs.close()
-
-
-@pytest.mark.parametrize("depth", [1, 2])
-def test_bulk_copy_staged_rows_variant_matches_oracle(ctx, oracle, depth, monkeypatch):
-    """LB200_CULL_STAGE=1|2: the same kernel with the sphere rows of TEST pages staged in shared memory by the bulk-copy engine
-    (cp.async.bulk + mbarrier) instead of straight loads — not the default (slower on 3.2 KB pages), same results."""
-    monkeypatch.setenv("LB200_CULL_STAGE", str(depth))  # read when a culling system first touches the device
-    scene = scenes.cull_scene(150_000, (3000.0, 300.0, 3000.0), seed=5 + depth, big_fraction=0.01, type_probs=(0.6, 0.2, 0.1, 0.1))
-    cs, oc = _both(ctx, oracle, scene)
-    for name, args in _frustums():
-        f = lb.frustum_perspective(**args)
-        res = cs.cull(f)
-        oids, otys, st = oc.cull(lb.culling.frustum_bytes(f))
-        _assert_same(res, oids, otys)
-        assert res.stats["pages_tested"] == st["pages_tested"] and res.stats["entities_tested"] == st["entities_tested"]
-    cs.close()

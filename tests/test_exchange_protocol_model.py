@@ -1,7 +1,6 @@
 """Model check of the bitmask-exchange protocol (DESIGN.md section 5; lb200_ctx::Peer in csrc/lb200_internal.h): R ranks, L lanes per
-rank, 2L exchange buffers per rank, epoch e on lane e % L and buffer e % 2L; a step = [store rows of epoch e into every rank's buffer,
-publish flag e everywhere, wait until every rank's flag for e is here]; batches of steps fork from / join into a rank's main stream,
-and the consumer of a batch's LAST step reads its buffer on the main stream before the next batch forks.
+rank, 3L exchange buffers per rank, epoch e in buffer e % 3L; batches of steps run on a rank's main stream or fork from / join into it,
+and the consumer of a batch's LAST step reads its buffer on the main stream before the next batch starts.
 
 A random scheduler interleaves everything that stream order allows (lanes of one rank progress independently, ranks drift apart) and the
 model asserts what the kernels rely on: a consumer always finds, in every slab of its buffer, the rows of exactly the epoch it waits for
@@ -11,16 +10,13 @@ import random
 import pytest
 
 
-def simulate(ranks, lanes, batches, rng, pipelined=False, deferred=False, fused=False):
-    """pipelined=False: the one-stream-per-lane form (store, publish, wait in lane order; 2L buffers).
-    pipelined=True: lb200_culling_cull_exchange_n's form — the wait of epoch e runs on a second stream of the lane, the lane itself only
-    holds publish(e) back until wait(e - L) is over and store(e) until wait(e - 2L) is over; 3L buffers."""
-    """deferred=True: lb200_culling_cull_exchange_n's default form — everything stays on the lane's stream, but the wait a step issues is the one
-    of the lane's PREVIOUS step, between its own store and publish: store(e), wait(e - L), publish(e); the batch ends with the waits still
-    owed; 3L buffers."""
-    """fused=True: one kernel per step — the cull of epoch e first waits for the flags of e - 2L, then stores its records while one of its warps
-    publishes the lane's PREVIOUS epoch (either order); a batch ends with publish + wait of every lane's last epoch; 3L buffers."""
-    nbuf = (3 if (pipelined or deferred or fused) else 2) * lanes
+def simulate(ranks, lanes, batches, rng):
+    """Each batch is dispatched the way lb200_culling_cull_exchange_n does it (a single lb200_culling_cull_exchange is a batch of one):
+    - lanes >= 2 and n >= 2: fused steps, epoch e on lane e % L — the cull of e first waits for the flags of e - 2L, then stores its
+      records while one of its warps publishes the lane's PREVIOUS epoch (either order); the batch ends with publish + wait of every
+      lane's last epoch;
+    - otherwise: two-kernel steps on the main stream — store, then publish + wait of the same epoch."""
+    nbuf = 3 * lanes
     # rows[r][b][src] = epoch whose rows rank `src` last stored into buffer b of rank r; flags likewise
     rows = [[[0] * ranks for _ in range(nbuf)] for _ in range(ranks)]
     flags = [[[0] * ranks for _ in range(nbuf)] for _ in range(ranks)]
@@ -29,8 +25,6 @@ def simulate(ranks, lanes, batches, rng, pipelined=False, deferred=False, fused=
     progs = []
     for r in range(ranks):
         ops, last_on = [], {}   # last_on[stream] = id of the previous op on that stream
-        wait_of = {}            # pipelined form: epoch -> id of its wait op
-        owed = {}               # deferred form: lane -> epoch whose wait has not been issued yet
 
         def add(stream, kind, epoch, extra=()):
             deps = [last_on[stream]] if stream in last_on else []
@@ -40,52 +34,35 @@ def simulate(ranks, lanes, batches, rng, pipelined=False, deferred=False, fused=
             return len(ops) - 1
         epoch = 0
         for n in batches:
+            if lanes < 2 or n < 2:
+                for _ in range(n):
+                    epoch += 1
+                    for kind in ("store", "publish", "wait"):
+                        add("main", kind, epoch)
+                add("main", "consume", epoch)
+                continue
             fork = add("main", "fork", 0)
-            tails = []
             used = set()
+            owed = {}  # lane -> its previous epoch, published by the lane's next cull or at the end of the batch
             for _ in range(n):
                 epoch += 1
                 lane = ("lane", epoch % lanes)
                 first = lane not in used
                 used.add(lane)
-                if fused:
-                    if epoch - 2 * lanes >= 1:
-                        add(lane, "wait", epoch - 2 * lanes, extra=[fork] if first else ())
-                        first = False
-                    todo = [("store", epoch)] + ([("publish", owed.pop(lane))] if lane in owed else [])
-                    rng.shuffle(todo)
-                    for kind, ep in todo:
-                        add(lane, kind, ep, extra=[fork] if first else ())
-                        first = False
-                    owed[lane] = epoch
-                elif deferred:
-                    s = add(lane, "store", epoch, extra=[fork] if first else ())
-                    if lane in owed:
-                        add(lane, "wait", owed.pop(lane))
-                    p = add(lane, "publish", epoch)
-                    owed[lane] = epoch
-                elif not pipelined:
-                    s = add(lane, "store", epoch, extra=[fork] if first else ())
-                    p = add(lane, "publish", epoch)
-                    w = add(lane, "wait", epoch)
-                else:
-                    side = ("wait", epoch % lanes)
-                    used.add(side)
-                    dep2 = [wait_of[epoch - 2 * lanes]] if epoch - 2 * lanes in wait_of else []
-                    dep1 = [wait_of[epoch - lanes]] if epoch - lanes in wait_of else []
-                    s = add(lane, "store", epoch, extra=([fork] if first else []) + dep2)
-                    p = add(lane, "publish", epoch, extra=dep1)
-                    wait_of[epoch] = add(side, "wait", epoch, extra=[p])
-            if deferred:  # the batch's consumer needs every step it issued complete: the owed waits go out before the join
-                for lane in list(owed):
-                    add(lane, "wait", owed.pop(lane))
-            if fused:  # the trailing publish + wait of every lane's last epoch
-                for lane in list(owed):
-                    ep = owed.pop(lane)
-                    add(lane, "publish", ep)
-                    add(lane, "wait", ep)
-            tails = [last_on[l] for l in used]
-            join = add("main", "join", 0, extra=tails)
+                if epoch - 2 * lanes >= 1:
+                    add(lane, "wait", epoch - 2 * lanes, extra=[fork] if first else ())
+                    first = False
+                todo = [("store", epoch)] + ([("publish", owed.pop(lane))] if lane in owed else [])
+                rng.shuffle(todo)
+                for kind, ep in todo:
+                    add(lane, kind, ep, extra=[fork] if first else ())
+                    first = False
+                owed[lane] = epoch
+            for lane in list(owed):  # the trailing publish + wait of every lane's last epoch
+                ep = owed.pop(lane)
+                add(lane, "publish", ep)
+                add(lane, "wait", ep)
+            add("main", "join", 0, extra=[last_on[l] for l in used])
             add("main", "consume", epoch)  # the out parameters describe the LAST step of the batch
         progs.append(ops)
     pending = sum(len(p) for p in progs)
@@ -117,78 +94,41 @@ def simulate(ranks, lanes, batches, rng, pipelined=False, deferred=False, fused=
     return steps
 
 
-@pytest.mark.parametrize("ranks,lanes", [(2, 1), (2, 2), (2, 3), (3, 3), (8, 3), (4, 4)])
+def _batches(rng, longest):
+    # single steps (two-kernel steps on the main stream) between batches of fused steps, as callers mix cull_exchange and cull_exchange_n
+    return [rng.choice((1, rng.randint(2, longest))) for _ in range(rng.randint(2, 6))]
+
+
+@pytest.mark.parametrize("ranks,lanes", [(2, 1), (2, 2), (2, 3), (3, 3), (8, 3), (4, 4), (8, 6), (8, 8)])
 def test_no_early_overwrite_and_no_deadlock(ranks, lanes):
     rng = random.Random(1000 * ranks + lanes)
     for trial in range(12 if ranks < 8 else 3):
-        batches = [rng.randint(1, 9) for _ in range(rng.randint(2, 5))]
-        simulate(ranks, lanes, batches, rng)
-
-
-@pytest.mark.parametrize("ranks,lanes", [(2, 1), (2, 2), (2, 3), (3, 3), (8, 3), (4, 4), (8, 6)])
-def test_pipelined_waits_no_early_overwrite_and_no_deadlock(ranks, lanes):
-    rng = random.Random(77 * ranks + lanes)
-    for trial in range(12 if ranks < 8 else 3):
-        batches = [rng.randint(1, 14) for _ in range(rng.randint(2, 5))]
-        simulate(ranks, lanes, batches, rng, pipelined=True)
-
-
-@pytest.mark.parametrize("ranks,lanes", [(2, 1), (2, 2), (2, 3), (3, 3), (8, 3), (4, 4), (8, 8)])
-def test_deferred_waits_no_early_overwrite_and_no_deadlock(ranks, lanes):
-    rng = random.Random(31 * ranks + lanes)
-    for trial in range(12 if ranks < 8 else 3):
-        batches = [rng.randint(1, 20) for _ in range(rng.randint(2, 5))]
-        simulate(ranks, lanes, batches, rng, deferred=True)
+        simulate(ranks, lanes, _batches(rng, 20), rng)
 
 
 @pytest.mark.parametrize("ranks,lanes", [(2, 1), (2, 2), (2, 3), (3, 3), (8, 3), (4, 4), (8, 8)])
 def test_fused_publish_no_early_overwrite_and_no_deadlock(ranks, lanes):
+    """Long batches back to back, a single step only where a batch size of 1 is drawn: with two or more lanes nearly every step is
+    fused, so between a fast rank and a slow one there is little but the fused steps' flow control and the batches' closing waits."""
     rng = random.Random(53 * ranks + lanes)
     for trial in range(12 if ranks < 8 else 3):
         batches = [rng.randint(1, 20) for _ in range(rng.randint(2, 5))]
-        simulate(ranks, lanes, batches, rng, fused=True)
+        simulate(ranks, lanes, batches, rng)
+
+
+def _broken(replace, by):
+    src = __import__("inspect").getsource(simulate)
+    assert replace in src
+    g = dict(simulate.__globals__)
+    exec(src.replace(replace, by), g)
+    return g["simulate"]
 
 
 def test_the_model_catches_a_fused_form_without_its_flow_control():
     """Without the wait for e - 2L inside the cull a fast rank laps a slow one and overwrites the slab its consumer is about to read."""
-    def broken(ranks, lanes, batches, rng):
-        g = dict(simulate.__globals__)
-        src = __import__("inspect").getsource(simulate).replace("if epoch - 2 * lanes >= 1:", "if False:")
-        exec(src, g)
-        return g["simulate"](ranks, lanes, batches, rng, fused=True)
+    broken = _broken("if epoch - 2 * lanes >= 1:", "if False:")
     failures = 0
     for seed in range(80):
-        try:
-            broken(2, 2, [9, 9, 9], random.Random(seed))
-        except AssertionError:
-            failures += 1
-    assert failures > 0
-
-
-def test_the_model_catches_too_few_buffers_for_deferred_waits():
-    def broken(ranks, lanes, batches, rng):
-        g = dict(simulate.__globals__)
-        src = __import__("inspect").getsource(simulate).replace("nbuf = (3 if (pipelined or deferred or fused) else 2) * lanes", "nbuf = 2 * lanes - 1")
-        exec(src, g)
-        return g["simulate"](ranks, lanes, batches, rng, deferred=True)
-    failures = 0
-    for seed in range(80):
-        try:
-            broken(2, 2, [9, 9, 9], random.Random(seed))
-        except AssertionError:
-            failures += 1
-    assert failures > 0
-
-
-def test_the_model_catches_too_few_buffers_for_pipelined_waits():
-    """With the waits off the lane streams, 2L buffers are not enough any more: a fast rank overwrites rows a slow rank still waits for."""
-    def broken(ranks, lanes, batches, rng):
-        g = dict(simulate.__globals__)
-        src = __import__("inspect").getsource(simulate).replace("nbuf = (3 if (pipelined or deferred or fused) else 2) * lanes", "nbuf = 2 * lanes")
-        exec(src, g)
-        return g["simulate"](ranks, lanes, batches, rng, pipelined=True)
-    failures = 0
-    for seed in range(60):
         try:
             broken(2, 2, [9, 9, 9], random.Random(seed))
         except AssertionError:
@@ -197,17 +137,12 @@ def test_the_model_catches_too_few_buffers_for_pipelined_waits():
 
 
 def test_the_model_catches_too_few_buffers():
-    """Sanity of the model itself: with only L buffers (instead of 2L) a fast rank does overwrite rows a slow rank has not consumed."""
-    def broken(ranks, lanes, batches, rng):
-        import types
-        g = dict(simulate.__globals__)
-        src = __import__("inspect").getsource(simulate).replace("nbuf = (3 if (pipelined or deferred or fused) else 2) * lanes", "nbuf = lanes")
-        exec(src, g)
-        return g["simulate"](ranks, lanes, batches, rng)
+    """Sanity of the model itself: with 2L buffers instead of 3L a fast rank does overwrite rows a slow rank has not consumed."""
+    broken = _broken("nbuf = 3 * lanes", "nbuf = 2 * lanes")
     failures = 0
-    for seed in range(40):
+    for seed in range(80):
         try:
-            broken(2, 2, [4, 4, 4], random.Random(seed))
+            broken(2, 2, [9, 9, 9], random.Random(seed))
         except AssertionError:
             failures += 1
     assert failures > 0
