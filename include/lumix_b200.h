@@ -458,6 +458,12 @@ LB200_API int lb200_animation_set_instances(lb200_animation* a, const uint32_t* 
 LB200_API int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t palette_flags);
 /* evaluateSkin (model.cpp:103-109) for every vertex of every instance from the matrix palette; output stays in HBM. */
 LB200_API int lb200_animation_skin(lb200_animation* a);
+/* Launch shape of later updates and skins, for tests and tuning.  pose_lanes = lanes per instance of the pose kernel (4, 8, 16 or 32);
+ * with 4 lanes, a skeleton whose poses do not fit in shared memory (more than 192 bones) still runs on 8.  skin_group = instances per
+ * skinning block (4, 8 or 16).  0 keeps the default: the LB200_POSE_LANES / LB200_SKIN_GROUP environment switch if set, else 8.
+ * Any other value is LB200_ERR_INVALID.  get_launch reports what the last update and the last skin launched (0 before the first). */
+LB200_API int lb200_animation_set_launch(lb200_animation* a, int pose_lanes, int skin_group);
+LB200_API int lb200_animation_get_launch(lb200_animation* a, int* pose_lanes, int* skin_group);
 /* Read-backs (host buffers).  Instances [first, first+count). */
 LB200_API int lb200_animation_get_dual_quats(lb200_animation* a, uint32_t first, uint32_t count, float* out8);
 LB200_API int lb200_animation_get_matrices(lb200_animation* a, uint32_t first, uint32_t count, float* out16);

@@ -328,6 +328,17 @@ class AnimationSystem:
     def skin(self):
         check(self.L.lb200_animation_skin(self.h), self.ctx.h)
 
+    def setLaunch(self, pose_lanes=0, skin_group=0):
+        """Launch shape of later update() / skin() calls: pose lanes per instance (4, 8, 16, 32) and skinning instances per block
+        (4, 8, 16); 0 keeps the default (environment switch, else 8).  More than 192 bones run 4 pose lanes as 8."""
+        check(self.L.lb200_animation_set_launch(self.h, C.c_int(pose_lanes), C.c_int(skin_group)), self.ctx.h)
+
+    def lastLaunch(self):
+        """(pose lanes of the last update, instances per block of the last skin); 0 where none has run."""
+        g, s = C.c_int(), C.c_int()
+        check(self.L.lb200_animation_get_launch(self.h, C.byref(g), C.byref(s)), self.ctx.h)
+        return int(g.value), int(s.value)
+
     def _get(self, fn, width, first, count, dtype=np.float32):
         count = self.n - first if count is None else count
         out = np.empty((count, self.skeleton.bone_count, width), dtype)

@@ -230,7 +230,8 @@ __global__ void __launch_bounds__(256) decode_clips_kernel(const __grid_constant
 constexpr int POSE_THREADS = 128;
 
 // G lanes cooperate on one instance (32 / G instances per warp): per-bone phases stride the bones by G, the absolute pass
-// walks depth levels with up to G bones of a level in flight.  G is chosen on the host from the skeleton's level widths.
+// walks depth levels with up to G bones of a level in flight.  G is 8 unless LB200_POSE_LANES or lb200_animation_set_launch asks
+// for another (lb200_animation_update).
 template <int G>
 __global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimParams P) {
 	extern __shared__ float4 smem4[];
@@ -560,6 +561,9 @@ struct lb200_animation {
 	float4* d_key_pos = nullptr; float4* d_key_rot = nullptr; unsigned char* d_key_flags = nullptr;
 	short* d_parents = nullptr; unsigned char* d_level_bones = nullptr; uint32_t* d_level_start = nullptr;
 	int lanes_per_instance = 8;
+	// lb200_animation_set_launch (0 = environment switch, else the default) and what the last update / skin launched
+	int pose_lanes = 0, skin_group = 0;
+	int last_pose_lanes = 0, last_skin_group = 0;
 	uint32_t* d_clip_index = nullptr; uint32_t* d_time = nullptr;
 	uint32_t n_layers = 0; uint32_t* d_layer_clip = nullptr; uint32_t* d_layer_time = nullptr; float* d_layer_weight = nullptr;
 	float* d_dq = nullptr; float* d_mtx = nullptr; float* d_pos = nullptr; float* d_rot = nullptr;
@@ -600,15 +604,10 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		for (uint32_t i = first; i < B; ++i) if (levels[i] == l) level_bones.push_back((unsigned char)i);
 	}
 	level_start[max_level + 1] = (uint32_t)level_bones.size();
-	// lanes per instance: minimise the lane-steps of the absolute pass, G * sum_l ceil(width_l / G), keeping >= 8 lanes for occupancy
-	int best_g = 8;
-	uint64_t best_cost = ~0ull;
-	for (int g = 8; g <= 32; g *= 2) {
-		uint64_t steps = 0;
-		for (uint32_t l = 1; l <= max_level; ++l) steps += (level_start[l + 1] - level_start[l] + g - 1) / g;
-		const uint64_t cost = steps * g;
-		if (cost < best_cost) { best_cost = cost; best_g = g; }
-	}
+	// lanes per instance: the choice minimises the lane-steps of the absolute pass, G * sum_l ceil(width_l / G), over G >= 8 (fewer
+	// lanes cost occupancy).  G * ceil(w / G) never falls as G doubles, and a tie keeps the smaller G, so that choice is always 8.
+	// G = 4, 16 and 32 run only when asked for (LB200_POSE_LANES, lb200_animation_set_launch).
+	const int best_g = 8;
 	std::vector<DevClip> dc(n_clips);
 	std::vector<DevTrack> tracks;
 	std::vector<float4> cts, cr_values;
@@ -806,7 +805,7 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 	P.dt_ticks = (uint32_t)((P.dt_negative ? -time_delta : time_delta) * (float)(1 << 15));
 	P.advance = 1;
 	static const int g_env = [] { const char* e = getenv("LB200_POSE_LANES"); const int v = e ? atoi(e) : 0; return (v == 4 || v == 8 || v == 16 || v == 32) ? v : 0; }();
-	int G = g_env ? g_env : a->lanes_per_instance;
+	int G = a->pose_lanes ? a->pose_lanes : g_env ? g_env : a->lanes_per_instance;
 	if (G == 4) { // 32 instances per block: only while their poses fit in shared memory
 		const uint32_t bp = (a->bone_count + 3u) & ~3u;
 		if (sizeof(float4) * (2 * (size_t)bp * (POSE_THREADS / 4) + 2 * bp + 128) > 200 * 1024) G = 8;
@@ -822,6 +821,7 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 	else if (G == 16) pose_palette_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
 	else pose_palette_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
 	LB200_CHECK_LAUNCH(ctx);
+	a->last_pose_lanes = G;
 	return LB200_OK;
 }
 
@@ -833,7 +833,8 @@ int lb200_animation_skin(lb200_animation* a) {
 	if (!a->n_instances) return LB200_OK;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	if (!a->d_skinned) ANIM_MALLOC(a->d_skinned, sizeof(float) * 3 * (size_t)a->max_instances * a->n_vertices);
-	static const int group = [] { const char* e = getenv("LB200_SKIN_GROUP"); const int v = e ? atoi(e) : 8; return (v == 4 || v == 16) ? v : 8; }();
+	static const int g_env = [] { const char* e = getenv("LB200_SKIN_GROUP"); const int v = e ? atoi(e) : 8; return (v == 4 || v == 16) ? v : 8; }();
+	const int group = a->skin_group ? a->skin_group : g_env;
 	const dim3 grid((a->n_vertices + SKIN_THREADS - 1) / SKIN_THREADS, (a->n_instances + group - 1) / group);
 	if (grid.y > 65535) { lb200_set_error(ctx, "too many instances for one skin launch"); return LB200_ERR_INVALID; }
 	const size_t smem = sizeof(float4) * 3 * a->bone_count * group;
@@ -841,6 +842,29 @@ int lb200_animation_skin(lb200_animation* a) {
 	if (group == 4) LB200_SKIN_LAUNCH(4); else if (group == 16) LB200_SKIN_LAUNCH(16); else LB200_SKIN_LAUNCH(8);
 #undef LB200_SKIN_LAUNCH
 	LB200_CHECK_LAUNCH(ctx);
+	a->last_skin_group = group;
+	return LB200_OK;
+}
+
+int lb200_animation_set_launch(lb200_animation* a, int pose_lanes, int skin_group) {
+	if (!a) return LB200_ERR_INVALID;
+	if (pose_lanes != 0 && pose_lanes != 4 && pose_lanes != 8 && pose_lanes != 16 && pose_lanes != 32) {
+		lb200_set_error(a->ctx, "set_launch: pose_lanes %d is not 0, 4, 8, 16 or 32", pose_lanes);
+		return LB200_ERR_INVALID;
+	}
+	if (skin_group != 0 && skin_group != 4 && skin_group != 8 && skin_group != 16) {
+		lb200_set_error(a->ctx, "set_launch: skin_group %d is not 0, 4, 8 or 16", skin_group);
+		return LB200_ERR_INVALID;
+	}
+	a->pose_lanes = pose_lanes;
+	a->skin_group = skin_group;
+	return LB200_OK;
+}
+
+int lb200_animation_get_launch(lb200_animation* a, int* pose_lanes, int* skin_group) {
+	if (!a) return LB200_ERR_INVALID;
+	if (pose_lanes) *pose_lanes = a->last_pose_lanes;
+	if (skin_group) *skin_group = a->last_skin_group;
 	return LB200_OK;
 }
 

@@ -84,12 +84,20 @@ def hierarchy_forest(n_total=1_000_000, depth=8, fanout=7, seed=3, root_extent=(
     return parents.astype(np.int32), locals_, globals_
 
 
-def skeleton(n_bones=64, seed=4):
-    """C4 skeleton: root + chains hanging off a 4-ary tree, parent < child."""
+def skeleton(n_bones=64, seed=4, parents=None):
+    """C4 skeleton: root + chains hanging off a 4-ary tree, parent < child.  `parents` gives any other topology instead (parent < child,
+    roots first, -1 = root); n_bones is then its length."""
     rng = np.random.default_rng(seed)
-    parents = np.full(n_bones, -1, np.int16)
-    for i in range(1, n_bones):
-        parents[i] = (i - 1) // 4 if i < 21 else i - 4  # 4-ary tree for the first 21 bones, then 4 parallel chains
+    if parents is None:
+        parents = np.full(n_bones, -1, np.int16)
+        for i in range(1, n_bones):
+            parents[i] = (i - 1) // 4 if i < 21 else i - 4  # 4-ary tree for the first 21 bones, then 4 parallel chains
+    else:
+        parents = np.array(parents, np.int16)
+        n_bones = len(parents)
+        nonroot = np.nonzero(parents >= 0)[0]
+        assert np.all(parents[nonroot] < nonroot), "every parent must come before its child"
+        assert len(nonroot) == 0 or np.all(parents[nonroot[0]:] >= 0), "roots must come first"
     rel_pos = (rng.random((n_bones, 3), np.float32) - np.float32(0.5)) * np.float32(0.6)
     rel_rot = random_unit_quats(rng, n_bones)
     from .animation import _qmul, _rotate
