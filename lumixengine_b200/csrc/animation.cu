@@ -14,6 +14,7 @@
 #include "lb200_internal.h"
 #include "lb200_math.cuh"
 
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -551,30 +552,43 @@ __global__ void __launch_bounds__(256) bone_attachments_kernel(const float* __re
 struct lb200_animation {
 	lb200_ctx* ctx = nullptr;
 	uint32_t bone_count = 0, max_level = 0, n_clips = 0, max_instances = 0, n_instances = 0, n_vertices = 0;
-	DevClip* d_clips = nullptr;
-	DevTrack* d_tracks = nullptr;
-	float4* d_const_t = nullptr;
-	float4* d_const_r_value = nullptr;
-	uint32_t* d_const_r_bone = nullptr;
-	uint32_t* d_stream = nullptr;
-	float4* d_bind = nullptr; // bind_pos[B], bind_rot[B], inv_bind_pos[B], inv_bind_rot[B]
-	float4* d_key_pos = nullptr; float4* d_key_rot = nullptr; unsigned char* d_key_flags = nullptr;
-	short* d_parents = nullptr; unsigned char* d_level_bones = nullptr; uint32_t* d_level_start = nullptr;
+	// every table created with the system gets an address, 16 bytes when it has no entries (TABLE_MIN_BYTES)
+	DeviceArray<DevClip> d_clips;
+	DeviceArray<DevTrack> d_tracks;
+	DeviceArray<float4> d_const_t;
+	DeviceArray<float4> d_const_r_value;
+	DeviceArray<uint32_t> d_const_r_bone;
+	DeviceArray<uint32_t> d_stream;
+	DeviceArray<float4> d_bind; // bind_pos[B], bind_rot[B], inv_bind_pos[B], inv_bind_rot[B]
+	DeviceArray<float4> d_key_pos, d_key_rot; DeviceArray<unsigned char> d_key_flags;
+	DeviceArray<short> d_parents; DeviceArray<unsigned char> d_level_bones; DeviceArray<uint32_t> d_level_start;
 	int lanes_per_instance = 8;
 	// lb200_animation_set_launch (0 = environment switch, else the default) and what the last update / skin launched
 	int pose_lanes = 0, skin_group = 0;
 	int last_pose_lanes = 0, last_skin_group = 0;
-	uint32_t* d_clip_index = nullptr; uint32_t* d_time = nullptr;
-	uint32_t n_layers = 0; uint32_t* d_layer_clip = nullptr; uint32_t* d_layer_time = nullptr; float* d_layer_weight = nullptr;
-	float* d_dq = nullptr; float* d_mtx = nullptr; float* d_pos = nullptr; float* d_rot = nullptr;
-	float* d_rel_pos = nullptr; float* d_rel_rot = nullptr; // Pose::computeRelative of d_pos / d_rot
+	DeviceArray<uint32_t> d_clip_index, d_time;
+	uint32_t n_layers = 0; DeviceArray<uint32_t> d_layer_clip, d_layer_time; DeviceArray<float> d_layer_weight; // all three or none
+	// palettes and poses, allocated by the first update that asks for them; d_pos / d_rot and d_rel_pos / d_rel_rot go in pairs
+	DeviceArray<float> d_dq, d_mtx, d_pos, d_rot;
+	DeviceArray<float> d_rel_pos, d_rel_rot; // Pose::computeRelative of d_pos / d_rot
 	uint32_t first_nonroot = 0;
-	float* d_mesh_pos = nullptr; float4* d_mesh_w = nullptr; short* d_mesh_idx = nullptr;
-	float* d_skinned = nullptr;
-	unsigned long long* d_checksum = nullptr;
+	DeviceArray<float> d_mesh_pos; DeviceArray<float4> d_mesh_w; DeviceArray<short> d_mesh_idx;
+	DeviceArray<float> d_skinned;
+	DeviceArray<unsigned long long> d_checksum;
 };
 
-#define ANIM_MALLOC(ptr, bytes) LB200_CUDA(ctx, cudaMalloc(&(ptr), (size_t)(bytes) > 0 ? (size_t)(bytes) : (size_t)16))
+namespace {
+constexpr size_t TABLE_MIN_BYTES = 16;
+
+// a pair of pose buffers (positions 3 floats, rotations 4 floats per bone and instance): both or neither
+int allocPosePair(lb200_ctx* ctx, DeviceArray<float>& pos, DeviceArray<float>& rot, size_t nb) {
+	DeviceArray<float> p, r;
+	LB200_CUDA(ctx, p.alloc(3 * nb));
+	LB200_CUDA(ctx, r.alloc(4 * nb));
+	pos = std::move(p); rot = std::move(r);
+	return LB200_OK;
+}
+} // namespace
 
 extern "C" {
 
@@ -666,20 +680,19 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		if (key_entries > 0x7fffffffull) { lb200_set_error(ctx, "decoded clips exceed 2^31 keyframe entries"); return LB200_ERR_INVALID; }
 	}
 
-	lb200_animation* a = new (std::nothrow) lb200_animation;
-	if (!a) return LB200_ERR_CUDA;
 	// any early return below (allocation or copy failure) releases what has been allocated so far
-	struct Guard { lb200_animation* a; ~Guard() { if (a) lb200_animation_destroy(a); } } guard{a};
+	std::unique_ptr<lb200_animation, decltype(&lb200_animation_destroy)> a(new (std::nothrow) lb200_animation, lb200_animation_destroy);
+	if (!a) return LB200_ERR_CUDA;
 	a->ctx = ctx; a->bone_count = B; a->max_level = max_level; a->n_clips = n_clips; a->max_instances = max_instances;
 	a->first_nonroot = first;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	ANIM_MALLOC(a->d_clips, sizeof(DevClip) * n_clips);
-	ANIM_MALLOC(a->d_tracks, sizeof(DevTrack) * tracks.size());
-	ANIM_MALLOC(a->d_const_t, sizeof(float4) * cts.size());
-	ANIM_MALLOC(a->d_const_r_value, sizeof(float4) * cr_values.size());
-	ANIM_MALLOC(a->d_const_r_bone, sizeof(uint32_t) * cr_bones.size());
-	ANIM_MALLOC(a->d_stream, sizeof(uint32_t) * stream.size());
-	ANIM_MALLOC(a->d_bind, sizeof(float4) * 4 * B);
+	LB200_CUDA(ctx, a->d_clips.alloc(n_clips, TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_tracks.alloc(tracks.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_const_t.alloc(cts.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_const_r_value.alloc(cr_values.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_const_r_bone.alloc(cr_bones.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_stream.alloc(stream.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_bind.alloc(4 * B, TABLE_MIN_BYTES));
 	std::vector<float4> bind(4 * (size_t)B);
 	for (uint32_t i = 0; i < B; ++i) {
 		const float* r = sk->bind_relative7 + 7 * (size_t)i;
@@ -689,13 +702,13 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		bind[2 * B + i] = make_float4(v[0], v[1], v[2], 0.f);
 		bind[3 * B + i] = make_float4(v[3], v[4], v[5], v[6]);
 	}
-	ANIM_MALLOC(a->d_parents, sizeof(short) * B);
-	ANIM_MALLOC(a->d_level_bones, level_bones.size());
-	ANIM_MALLOC(a->d_level_start, sizeof(uint32_t) * level_start.size());
+	LB200_CUDA(ctx, a->d_parents.alloc(B, TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_level_bones.alloc(level_bones.size(), TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_level_start.alloc(level_start.size(), TABLE_MIN_BYTES));
 	a->lanes_per_instance = best_g;
-	ANIM_MALLOC(a->d_clip_index, sizeof(uint32_t) * max_instances);
-	ANIM_MALLOC(a->d_time, sizeof(uint32_t) * max_instances);
-	ANIM_MALLOC(a->d_checksum, sizeof(unsigned long long));
+	LB200_CUDA(ctx, a->d_clip_index.alloc(max_instances, TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_time.alloc(max_instances, TABLE_MIN_BYTES));
+	LB200_CUDA(ctx, a->d_checksum.alloc(1, TABLE_MIN_BYTES));
 	cudaStream_t st = ctx->stream;
 	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_clips, dc.data(), sizeof(DevClip) * n_clips, cudaMemcpyHostToDevice, st));
 	if (!tracks.empty()) LB200_CUDA(ctx, cudaMemcpyAsync(a->d_tracks, tracks.data(), sizeof(DevTrack) * tracks.size(), cudaMemcpyHostToDevice, st));
@@ -710,20 +723,20 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 	if (mesh && mesh->n_vertices) {
 		a->n_vertices = mesh->n_vertices;
 		for (uint32_t v = 0; v < mesh->n_vertices * 4; ++v) if (mesh->indices4[v] < 0 || (uint32_t)mesh->indices4[v] >= B) return LB200_ERR_INVALID;
-		ANIM_MALLOC(a->d_mesh_pos, sizeof(float) * 3 * mesh->n_vertices);
-		ANIM_MALLOC(a->d_mesh_w, sizeof(float4) * mesh->n_vertices);
-		ANIM_MALLOC(a->d_mesh_idx, sizeof(short) * 4 * mesh->n_vertices);
+		LB200_CUDA(ctx, a->d_mesh_pos.alloc(3 * mesh->n_vertices, TABLE_MIN_BYTES));
+		LB200_CUDA(ctx, a->d_mesh_w.alloc(mesh->n_vertices, TABLE_MIN_BYTES));
+		LB200_CUDA(ctx, a->d_mesh_idx.alloc(4 * mesh->n_vertices, TABLE_MIN_BYTES));
 		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_mesh_pos, mesh->positions3, sizeof(float) * 3 * mesh->n_vertices, cudaMemcpyHostToDevice, st));
 		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_mesh_w, mesh->weights4, sizeof(float4) * mesh->n_vertices, cudaMemcpyHostToDevice, st));
 		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_mesh_idx, mesh->indices4, sizeof(short) * 4 * mesh->n_vertices, cudaMemcpyHostToDevice, st));
 	}
 	{
-		ANIM_MALLOC(a->d_key_pos, sizeof(float4) * key_entries);
-		ANIM_MALLOC(a->d_key_rot, sizeof(float4) * key_entries);
-		ANIM_MALLOC(a->d_key_flags, (size_t)n_clips * Bp);
-		uint32_t* d_fc = nullptr; uint32_t* d_fi = nullptr;
-		ANIM_MALLOC(d_fc, sizeof(uint32_t) * frame_clip.size());
-		ANIM_MALLOC(d_fi, sizeof(uint32_t) * frame_index.size());
+		LB200_CUDA(ctx, a->d_key_pos.alloc(key_entries, TABLE_MIN_BYTES));
+		LB200_CUDA(ctx, a->d_key_rot.alloc(key_entries, TABLE_MIN_BYTES));
+		LB200_CUDA(ctx, a->d_key_flags.alloc((size_t)n_clips * Bp, TABLE_MIN_BYTES));
+		DeviceArray<uint32_t> d_fc, d_fi;
+		LB200_CUDA(ctx, d_fc.alloc(frame_clip.size(), TABLE_MIN_BYTES));
+		LB200_CUDA(ctx, d_fi.alloc(frame_index.size(), TABLE_MIN_BYTES));
 		LB200_CUDA(ctx, cudaMemcpyAsync(d_fc, frame_clip.data(), sizeof(uint32_t) * frame_clip.size(), cudaMemcpyHostToDevice, st));
 		LB200_CUDA(ctx, cudaMemcpyAsync(d_fi, frame_index.data(), sizeof(uint32_t) * frame_index.size(), cudaMemcpyHostToDevice, st));
 		DecodeParams D;
@@ -733,8 +746,7 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		D.frame_clip = d_fc; D.frame_index = d_fi; D.bone_count = B;
 		decode_clips_kernel<<<(unsigned)frame_clip.size(), 256, 0, st>>>(D);
 		LB200_CHECK_LAUNCH(ctx);
-		LB200_CUDA(ctx, cudaStreamSynchronize(st));
-		cudaFree(d_fc); cudaFree(d_fi);
+		LB200_CUDA(ctx, cudaStreamSynchronize(st)); // before d_fc / d_fi are freed
 	}
 	LB200_CUDA(ctx, cudaStreamSynchronize(st));
 	{
@@ -748,8 +760,7 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * 196 * 3 * sizeof(float4))));
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(8 * 196 * 3 * sizeof(float4))));
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(16 * 196 * 3 * sizeof(float4))));
-	guard.a = nullptr;
-	*out = a;
+	*out = a.release();
 	return LB200_OK;
 }
 
@@ -757,10 +768,6 @@ void lb200_animation_destroy(lb200_animation* a) {
 	if (!a) return;
 	cudaSetDevice(a->ctx->device);
 	cudaStreamSynchronize(a->ctx->stream);
-	cudaFree(a->d_clips); cudaFree(a->d_tracks); cudaFree(a->d_const_t); cudaFree(a->d_const_r_value); cudaFree(a->d_const_r_bone); cudaFree(a->d_stream);
-	cudaFree(a->d_bind); cudaFree(a->d_key_pos); cudaFree(a->d_key_rot); cudaFree(a->d_key_flags); cudaFree(a->d_parents); cudaFree(a->d_level_bones); cudaFree(a->d_level_start);
-	cudaFree(a->d_clip_index); cudaFree(a->d_time); cudaFree(a->d_layer_clip); cudaFree(a->d_layer_time); cudaFree(a->d_layer_weight); cudaFree(a->d_dq); cudaFree(a->d_mtx); cudaFree(a->d_pos); cudaFree(a->d_rot); cudaFree(a->d_rel_pos); cudaFree(a->d_rel_rot);
-	cudaFree(a->d_mesh_pos); cudaFree(a->d_mesh_w); cudaFree(a->d_mesh_idx); cudaFree(a->d_skinned); cudaFree(a->d_checksum);
 	delete a;
 }
 
@@ -784,9 +791,12 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 	if (!a->n_instances) return LB200_OK;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	const size_t nb = (size_t)a->max_instances * a->bone_count;
-	if ((flags & LB200_PALETTE_DUAL_QUAT) && !a->d_dq) ANIM_MALLOC(a->d_dq, sizeof(float) * 8 * nb);
-	if ((flags & LB200_PALETTE_MATRIX) && !a->d_mtx) ANIM_MALLOC(a->d_mtx, sizeof(float) * 16 * nb);
-	if ((flags & LB200_PALETTE_POSE) && !a->d_pos) { ANIM_MALLOC(a->d_pos, sizeof(float) * 3 * nb); ANIM_MALLOC(a->d_rot, sizeof(float) * 4 * nb); }
+	if ((flags & LB200_PALETTE_DUAL_QUAT) && !a->d_dq) LB200_CUDA(ctx, a->d_dq.alloc(8 * nb));
+	if ((flags & LB200_PALETTE_MATRIX) && !a->d_mtx) LB200_CUDA(ctx, a->d_mtx.alloc(16 * nb));
+	if ((flags & LB200_PALETTE_POSE) && (!a->d_pos || !a->d_rot)) {
+		const int rc = allocPosePair(ctx, a->d_pos, a->d_rot, nb);
+		if (rc) return rc;
+	}
 	AnimParams P;
 	P.clips = a->d_clips; P.tracks = a->d_tracks; P.const_t = a->d_const_t; P.const_r_value = a->d_const_r_value; P.const_r_bone = a->d_const_r_bone; P.stream = a->d_stream;
 	P.key_pos = a->d_key_pos; P.key_rot = a->d_key_rot; P.key_flags = a->d_key_flags;
@@ -794,10 +804,10 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 	P.bone_count = a->bone_count; P.max_level = a->max_level; P.n_instances = a->n_instances;
 	P.clip_index = a->d_clip_index; P.time_ticks = a->d_time;
 	P.n_layers = a->n_layers; P.layer_clip = a->d_layer_clip; P.layer_time = a->d_layer_time; P.layer_weight = a->d_layer_weight;
-	P.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq : nullptr;
-	P.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx : nullptr;
-	P.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos : nullptr;
-	P.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot : nullptr;
+	P.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
+	P.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
+	P.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
+	P.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
 	// Time::fromSeconds: u32(time * ONE_SECOND), animation.h:21-24 (:462 uses -time_delta for rewinds)
 	// animation_module.cpp:458 `if (time_delta > 0) ... else ...`: zero takes the rewind branch too, which leaves a time below the clip
 	// length alone and wraps one at or beyond it (time % length), exactly as the reference does on every update
@@ -832,7 +842,7 @@ int lb200_animation_skin(lb200_animation* a) {
 	if (!a->n_vertices || !a->d_mtx) { lb200_set_error(ctx, "skin needs a mesh and a matrix palette (update with LB200_PALETTE_MATRIX first)"); return LB200_ERR_STATE; }
 	if (!a->n_instances) return LB200_OK;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!a->d_skinned) ANIM_MALLOC(a->d_skinned, sizeof(float) * 3 * (size_t)a->max_instances * a->n_vertices);
+	if (!a->d_skinned) LB200_CUDA(ctx, a->d_skinned.alloc(3 * (size_t)a->max_instances * a->n_vertices));
 	static const int g_env = [] { const char* e = getenv("LB200_SKIN_GROUP"); const int v = e ? atoi(e) : 8; return (v == 4 || v == 16) ? v : 8; }();
 	const int group = a->skin_group ? a->skin_group : g_env;
 	const dim3 grid((a->n_vertices + SKIN_THREADS - 1) / SKIN_THREADS, (a->n_instances + group - 1) / group);
@@ -879,13 +889,13 @@ static int readBack(lb200_animation* a, const void* dev, size_t elem_bytes, uint
 }
 
 int lb200_animation_get_dual_quats(lb200_animation* a, uint32_t first, uint32_t count, float* out8) {
-	return readBack(a, a ? a->d_dq : nullptr, sizeof(float) * 8 * (a ? a->bone_count : 0), first, count, out8);
+	return readBack(a, a ? a->d_dq.get() : nullptr, sizeof(float) * 8 * (a ? a->bone_count : 0), first, count, out8);
 }
 int lb200_animation_get_matrices(lb200_animation* a, uint32_t first, uint32_t count, float* out16) {
-	return readBack(a, a ? a->d_mtx : nullptr, sizeof(float) * 16 * (a ? a->bone_count : 0), first, count, out16);
+	return readBack(a, a ? a->d_mtx.get() : nullptr, sizeof(float) * 16 * (a ? a->bone_count : 0), first, count, out16);
 }
 int lb200_animation_get_pose(lb200_animation* a, uint32_t first, uint32_t count, float* out_pos3, float* out_rot4) {
-	int rc = readBack(a, a ? a->d_pos : nullptr, sizeof(float) * 3 * (a ? a->bone_count : 0), first, count, out_pos3);
+	int rc = readBack(a, a ? a->d_pos.get() : nullptr, sizeof(float) * 3 * (a ? a->bone_count : 0), first, count, out_pos3);
 	if (rc) return rc;
 	return readBack(a, a->d_rot, sizeof(float) * 4 * a->bone_count, first, count, out_rot4);
 }
@@ -898,9 +908,13 @@ int lb200_animation_set_layers(lb200_animation* a, uint32_t n_layers, const uint
 	const size_t n = (size_t)a->n_instances * n_layers;
 	for (size_t i = 0; i < n; ++i) if (clip_index[i] >= a->n_clips) { lb200_set_error(ctx, "layer entry %zu: clip %u out of range", i, clip_index[i]); return LB200_ERR_INVALID; }
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFree(a->d_layer_clip); cudaFree(a->d_layer_time); cudaFree(a->d_layer_weight);
-	a->d_layer_clip = nullptr; a->d_layer_time = nullptr; a->d_layer_weight = nullptr; a->n_layers = 0;
-	ANIM_MALLOC(a->d_layer_clip, sizeof(uint32_t) * n); ANIM_MALLOC(a->d_layer_time, sizeof(uint32_t) * n); ANIM_MALLOC(a->d_layer_weight, sizeof(float) * n);
+	a->d_layer_clip.reset(); a->d_layer_time.reset(); a->d_layer_weight.reset(); // all three go before any is allocated again
+	a->n_layers = 0;
+	DeviceArray<uint32_t> layer_clip, layer_time; DeviceArray<float> layer_weight;
+	LB200_CUDA(ctx, layer_clip.alloc(n));
+	LB200_CUDA(ctx, layer_time.alloc(n));
+	LB200_CUDA(ctx, layer_weight.alloc(n));
+	a->d_layer_clip = std::move(layer_clip); a->d_layer_time = std::move(layer_time); a->d_layer_weight = std::move(layer_weight);
 	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_layer_clip, clip_index, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_layer_time, time_ticks, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_layer_weight, weight, sizeof(float) * n, cudaMemcpyHostToDevice, ctx->stream));
@@ -921,25 +935,20 @@ int lb200_animation_bone_attachments(lb200_animation* a, uint32_t n, const uint3
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	// one staging allocation per call: [instance n][bone n][relative 7n][scale 3n] u32/f32, [parent n][out n] transforms
 	const size_t words = (size_t)n * (1 + 1 + 7 + 3);
-	uint32_t* d_words = nullptr;
-	lb200_transform* d_tr = nullptr;
-	LB200_CUDA(ctx, cudaMalloc(&d_words, sizeof(uint32_t) * words));
-	if (cudaMalloc(&d_tr, sizeof(lb200_transform) * 2 * (size_t)n) != cudaSuccess) { cudaGetLastError(); cudaFree(d_words); lb200_set_error(ctx, "bone_attachments: out of device memory"); return LB200_ERR_CUDA; }
-	cudaError_t e = cudaMemcpyAsync(d_words, instance, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d_words + n, bone, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d_words + 2 * (size_t)n, relative7, sizeof(float) * 7 * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d_words + 9 * (size_t)n, original_scale3, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (e == cudaSuccess) e = cudaMemcpyAsync(d_tr, parent_transforms, sizeof(lb200_transform) * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (e == cudaSuccess) {
-		bone_attachments_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(a->d_pos, a->d_rot, a->bone_count, d_words, d_words + n,
-			reinterpret_cast<const float*>(d_words + 2 * (size_t)n), d_tr, reinterpret_cast<const float*>(d_words + 9 * (size_t)n), n, d_tr + n);
-		ctx->launches.fetch_add(1, std::memory_order_relaxed);
-		e = cudaGetLastError();
-	}
-	if (e == cudaSuccess) e = cudaMemcpyAsync(out_transforms, d_tr + n, sizeof(lb200_transform) * n, cudaMemcpyDeviceToHost, ctx->stream);
-	if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-	cudaFree(d_words); cudaFree(d_tr);
-	if (e != cudaSuccess) { lb200_set_error(ctx, "bone_attachments failed: %s", cudaGetErrorString(e)); return LB200_ERR_CUDA; }
+	DeviceArray<uint32_t> d_words;
+	DeviceArray<lb200_transform> d_tr;
+	LB200_CUDA(ctx, d_words.alloc(words));
+	LB200_CUDA(ctx, d_tr.alloc(2 * (size_t)n));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_words, instance, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_words + n, bone, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_words + 2 * (size_t)n, relative7, sizeof(float) * 7 * n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_words + 9 * (size_t)n, original_scale3, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_tr, parent_transforms, sizeof(lb200_transform) * n, cudaMemcpyHostToDevice, ctx->stream));
+	bone_attachments_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(a->d_pos, a->d_rot, a->bone_count, d_words, d_words + n,
+		reinterpret_cast<const float*>(d_words + 2 * (size_t)n), d_tr, reinterpret_cast<const float*>(d_words + 9 * (size_t)n), n, d_tr + n);
+	LB200_CHECK_LAUNCH(ctx);
+	LB200_CUDA(ctx, cudaMemcpyAsync(out_transforms, d_tr + n, sizeof(lb200_transform) * n, cudaMemcpyDeviceToHost, ctx->stream));
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // before the staging is freed
 	return LB200_OK;
 }
 
@@ -964,7 +973,10 @@ int lb200_animation_compute_relative(lb200_animation* a) {
 	if (!a->d_pos || !a->n_instances) { lb200_set_error(ctx, "compute_relative needs absolute poses (update with LB200_PALETTE_POSE)"); return LB200_ERR_STATE; }
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	const size_t nb = (size_t)a->max_instances * a->bone_count;
-	if (!a->d_rel_pos) { ANIM_MALLOC(a->d_rel_pos, sizeof(float) * 3 * nb); ANIM_MALLOC(a->d_rel_rot, sizeof(float) * 4 * nb); }
+	if (!a->d_rel_pos || !a->d_rel_rot) {
+		const int rc = allocPosePair(ctx, a->d_rel_pos, a->d_rel_rot, nb);
+		if (rc) return rc;
+	}
 	const size_t n = (size_t)a->n_instances * a->bone_count;
 	pose_relative_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(a->d_pos, a->d_rot, a->d_parents, a->bone_count, a->first_nonroot, n, a->d_rel_pos, a->d_rel_rot);
 	LB200_CHECK_LAUNCH(ctx);
@@ -972,7 +984,7 @@ int lb200_animation_compute_relative(lb200_animation* a) {
 }
 
 int lb200_animation_get_relative_pose(lb200_animation* a, uint32_t first, uint32_t count, float* out_pos3, float* out_rot4) {
-	int rc = readBack(a, a ? a->d_rel_pos : nullptr, sizeof(float) * 3 * (a ? a->bone_count : 0), first, count, out_pos3);
+	int rc = readBack(a, a ? a->d_rel_pos.get() : nullptr, sizeof(float) * 3 * (a ? a->bone_count : 0), first, count, out_pos3);
 	if (rc) return rc;
 	return readBack(a, a->d_rel_rot, sizeof(float) * 4 * a->bone_count, first, count, out_rot4);
 }
@@ -994,10 +1006,10 @@ int lb200_animation_blend_pose(lb200_animation* a, const lb200_animation* b, flo
 }
 
 int lb200_animation_get_times(lb200_animation* a, uint32_t first, uint32_t count, uint32_t* out_ticks) {
-	return readBack(a, a ? a->d_time : nullptr, sizeof(uint32_t), first, count, out_ticks);
+	return readBack(a, a ? a->d_time.get() : nullptr, sizeof(uint32_t), first, count, out_ticks);
 }
 int lb200_animation_get_skinned(lb200_animation* a, uint32_t first, uint32_t count, float* out_pos3) {
-	return readBack(a, a ? a->d_skinned : nullptr, sizeof(float) * 3 * (a ? a->n_vertices : 0), first, count, out_pos3);
+	return readBack(a, a ? a->d_skinned.get() : nullptr, sizeof(float) * 3 * (a ? a->n_vertices : 0), first, count, out_pos3);
 }
 
 int lb200_animation_skinned_checksum(lb200_animation* a, uint64_t* out) {
@@ -1007,7 +1019,7 @@ int lb200_animation_skinned_checksum(lb200_animation* a, uint64_t* out) {
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	LB200_CUDA(ctx, cudaMemsetAsync(a->d_checksum, 0, sizeof(unsigned long long), ctx->stream));
 	const size_t n = (size_t)a->n_instances * a->n_vertices * 3;
-	checksum_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(reinterpret_cast<const uint32_t*>(a->d_skinned), n, a->d_checksum);
+	checksum_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(reinterpret_cast<const uint32_t*>(a->d_skinned.get()), n, a->d_checksum);
 	LB200_CHECK_LAUNCH(ctx);
 	unsigned long long v = 0;
 	LB200_CUDA(ctx, cudaMemcpyAsync(&v, a->d_checksum, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));

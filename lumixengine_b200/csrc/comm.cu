@@ -68,8 +68,9 @@ int lb200_comm_allgather_u32(lb200_ctx* ctx, const uint32_t* send, uint32_t* rec
 
 int lb200_comm_check(lb200_ctx* ctx) {
 	lb200_ctx::Peer& P = ctx->peer;
-	if (!P.h_timeout || !*(volatile uint32_t*)P.h_timeout) return LB200_OK;
-	*(volatile uint32_t*)P.h_timeout = 0;
+	volatile uint32_t* timeout = P.h_timeout;
+	if (!timeout || !*timeout) return LB200_OK;
+	*timeout = 0;
 	lb200_set_error(ctx, "multi-GPU exchange: a peer's slab did not arrive within the wait limit (~4 s); the exchanged slabs of that step are incomplete");
 	return LB200_ERR_NCCL;
 }
@@ -105,13 +106,8 @@ int lb200_comm_init(lb200_ctx* ctx, int n_ranks, int rank, const uint8_t unique_
 
 // Map every rank's gather buffers into every process (CUDA IPC over NVLink peer access).  Collective: all ranks call it with the same
 // max_slab_ids.  The IPC handles travel through one ncclAllGather, so the caller needs no extra side channel.
-int lb200_comm_enable_p2p(lb200_ctx* ctx, uint32_t max_slab_ids) {
-	if (!ctx) return LB200_ERR_INVALID;
-	if (!ctx->nccl_comm) { lb200_set_error(ctx, "lb200_comm_init has not been called"); return LB200_ERR_STATE; }
+static int enableP2p(lb200_ctx* ctx, uint32_t max_slab_ids) {
 	const int R = ctx->n_ranks;
-	if (R > LB200_MAX_RANKS) { lb200_set_error(ctx, "peer exchange supports up to %d ranks (one NVSwitch box)", LB200_MAX_RANKS); return LB200_ERR_INVALID; }
-	if (ctx->peer.ready) return LB200_OK;
-	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	lb200_ctx::Peer& P = ctx->peer;
 	P.slab_words = (256 + (size_t)max_slab_ids + 63) & ~(size_t)63;
 	const size_t flag_bytes = 1024;
@@ -120,28 +116,28 @@ int lb200_comm_enable_p2p(lb200_ctx* ctx, uint32_t max_slab_ids) {
 	P.n_buffers = 3 * P.lanes;
 	static_assert(3 * LB200_MAX_LANES * LB200_MAX_RANKS * sizeof(uint32_t) <= 1024, "flag block");
 	const size_t total = flag_bytes + P.n_buffers * buf_bytes;
-	LB200_CUDA(ctx, cudaMalloc(&P.local_block, total));
+	LB200_CUDA(ctx, P.local_block.alloc(total));
 	LB200_CUDA(ctx, cudaMemsetAsync(P.local_block, 0, flag_bytes, ctx->stream));
-	LB200_CUDA(ctx, cudaMalloc(&P.done_counter, sizeof(uint32_t) * LB200_MAX_LANES));
+	LB200_CUDA(ctx, P.done_counter.alloc(LB200_MAX_LANES));
 	LB200_CUDA(ctx, cudaMemsetAsync(P.done_counter, 0, sizeof(uint32_t) * LB200_MAX_LANES, ctx->stream));
-	LB200_CUDA(ctx, cudaHostAlloc(&P.h_timeout, sizeof(uint32_t), cudaHostAllocMapped));
+	LB200_CUDA(ctx, P.h_timeout.alloc(1));
 	*P.h_timeout = 0;
 	LB200_CUDA(ctx, cudaHostGetDevicePointer((void**)&P.d_timeout, P.h_timeout, 0));
 	cudaIpcMemHandle_t mine;
 	LB200_CUDA(ctx, cudaIpcGetMemHandle(&mine, P.local_block));
 	// exchange the 64-byte handles with NCCL
 	static_assert(sizeof(cudaIpcMemHandle_t) == 64, "");
-	uint32_t* d_h = nullptr;
-	LB200_CUDA(ctx, cudaMalloc(&d_h, 64 * (size_t)(R + 1)));
+	DeviceArray<uint32_t> d_h;
+	LB200_CUDA(ctx, d_h.alloc(16 * (size_t)(R + 1)));
 	LB200_CUDA(ctx, cudaMemcpyAsync(d_h + 16 * (size_t)R, &mine, 64, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_NCCL(ctx, p_ncclAllGather(d_h + 16 * (size_t)R, d_h, 16, ncclUint32_dt, (ncclComm_t)ctx->nccl_comm, ctx->stream));
 	cudaIpcMemHandle_t all[LB200_MAX_RANKS];
 	LB200_CUDA(ctx, cudaMemcpyAsync(all, d_h, 64 * (size_t)R, cudaMemcpyDeviceToHost, ctx->stream));
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFree(d_h);
+	d_h.reset();
 	for (int r = 0; r < R; ++r) {
 		char* base;
-		if (r == ctx->rank) base = (char*)P.local_block;
+		if (r == ctx->rank) base = P.local_block;
 		else {
 			void* p = nullptr;
 			LB200_CUDA(ctx, cudaIpcOpenMemHandle(&p, all[r], cudaIpcMemLazyEnablePeerAccess));
@@ -152,27 +148,42 @@ int lb200_comm_enable_p2p(lb200_ctx* ctx, uint32_t max_slab_ids) {
 		for (uint32_t b = 0; b < P.n_buffers; ++b) P.gather[b][r] = (uint32_t*)(base + flag_bytes + b * buf_bytes);
 	}
 	// nobody may start pushing before every rank has mapped every buffer (and zeroed its flags): one more collective as a barrier
-	uint32_t* d_b = nullptr;
-	LB200_CUDA(ctx, cudaMalloc(&d_b, sizeof(uint32_t) * (size_t)(R + 1)));
+	DeviceArray<uint32_t> d_b;
+	LB200_CUDA(ctx, d_b.alloc((size_t)(R + 1)));
 	LB200_NCCL(ctx, p_ncclAllGather(d_b + R, d_b, 1, ncclUint32_dt, (ncclComm_t)ctx->nccl_comm, ctx->stream));
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFree(d_b);
 	P.epoch = 0;
 	P.ready = true;
 	return LB200_OK;
+}
+
+static void releasePeer(lb200_ctx* ctx) {
+	// the peers' mappings are closed before this rank's block is freed
+	for (int r = 0; r < LB200_MAX_RANKS; ++r) if (ctx->peer.opened[r]) cudaIpcCloseMemHandle(ctx->peer.opened[r]);
+	ctx->peer.local_block.reset();
+	ctx->peer = lb200_ctx::Peer();
+}
+
+int lb200_comm_enable_p2p(lb200_ctx* ctx, uint32_t max_slab_ids) {
+	if (!ctx) return LB200_ERR_INVALID;
+	if (!ctx->nccl_comm) { lb200_set_error(ctx, "lb200_comm_init has not been called"); return LB200_ERR_STATE; }
+	if (ctx->n_ranks > LB200_MAX_RANKS) { lb200_set_error(ctx, "peer exchange supports up to %d ranks (one NVSwitch box)", LB200_MAX_RANKS); return LB200_ERR_INVALID; }
+	if (ctx->peer.ready) return LB200_OK;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	const int rc = enableP2p(ctx, max_slab_ids);
+	if (rc) { // a failed call leaves no peer state behind: a retry starts from scratch
+		cudaStreamSynchronize(ctx->stream);
+		releasePeer(ctx);
+	}
+	return rc;
 }
 
 void lb200_comm_destroy(lb200_ctx* ctx) {
 	if (!ctx || !ctx->nccl_comm) return;
 	cudaSetDevice(ctx->device);
 	cudaStreamSynchronize(ctx->stream);
-	if (ctx->peer.local_block) {
-		for (int r = 0; r < LB200_MAX_RANKS; ++r) if (ctx->peer.opened[r]) cudaIpcCloseMemHandle(ctx->peer.opened[r]);
-		cudaFree(ctx->peer.local_block);
-		cudaFree(ctx->peer.done_counter);
-		if (ctx->peer.h_timeout) cudaFreeHost(ctx->peer.h_timeout);
-		ctx->peer = lb200_ctx::Peer();
-	}
+	releasePeer(ctx);
+	// the NCCL communicator is a raw handle: it is created and destroyed here only, through the dlopen'ed library
 	p_ncclCommDestroy((ncclComm_t)ctx->nccl_comm);
 	ctx->nccl_comm = nullptr;
 	ctx->n_ranks = 1;

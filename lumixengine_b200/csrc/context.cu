@@ -60,8 +60,8 @@ static int initContext(int device_ordinal, int stream_priority_low, lb200_ctx** 
 	int prio_least = 0, prio_greatest = 0;
 	if ((e = cudaSetDevice(device_ordinal)) != cudaSuccess
 		|| (e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest)) != cudaSuccess
-		|| (e = cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, stream_priority_low ? prio_least : prio_greatest)) != cudaSuccess
-		|| (e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking)) != cudaSuccess
+		|| (e = cudaStreamCreateWithPriority(ctx->stream.create(), cudaStreamNonBlocking, stream_priority_low ? prio_least : prio_greatest)) != cudaSuccess
+		|| (e = cudaStreamCreateWithFlags(ctx->copy_stream.create(), cudaStreamNonBlocking)) != cudaSuccess
 		|| (e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device_ordinal)) != cudaSuccess) {
 		lb200_set_error(nullptr, "context creation failed: %s", cudaGetErrorString(e));
 		delete ctx;
@@ -75,9 +75,8 @@ void lb200_shutdown(lb200_ctx* ctx) {
 	if (!ctx) return;
 	lb200_comm_destroy(ctx);
 	cudaSetDevice(ctx->device);
-	if (ctx->stream) { cudaStreamSynchronize(ctx->stream); cudaStreamDestroy(ctx->stream); }
-	if (ctx->copy_stream) { cudaStreamSynchronize(ctx->copy_stream); cudaStreamDestroy(ctx->copy_stream); }
-	cudaFree(ctx->sort_scratch);
+	if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+	if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
 	delete ctx;
 }
 
@@ -95,6 +94,7 @@ int lb200_host_callback(lb200_ctx* ctx, void (*fn)(void*), void* user) {
 	return LB200_OK;
 }
 
+// The C API's allocations and events belong to the caller, who frees them with the matching call below: raw, not handles.
 void* lb200_host_alloc(lb200_ctx* ctx, size_t bytes) {
 	if (!ctx) return nullptr;
 	void* p = nullptr;
@@ -173,7 +173,7 @@ void lb200_event_destroy(lb200_ctx* ctx, void* event) {
 }
 
 uint64_t lb200_launch_count(const lb200_ctx* ctx) { return ctx ? ctx->launches.load() : 0; }
-uint64_t lb200_stream_handle(const lb200_ctx* ctx) { return ctx ? (uint64_t)(uintptr_t)ctx->stream : 0; }
+uint64_t lb200_stream_handle(const lb200_ctx* ctx) { return ctx ? (uint64_t)(uintptr_t)(cudaStream_t)ctx->stream : 0; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Frustum construction (host).  geometry.cpp:311-351 (setPoints / setPlanesFromPoints), :421-427 (setPlane),

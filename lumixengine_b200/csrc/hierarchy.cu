@@ -11,6 +11,7 @@
 #include "lb200_internal.h"
 #include "lb200_math.cuh"
 
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -191,42 +192,47 @@ __global__ void __launch_bounds__(HT) relative_matrices_kernel(SoaTransforms G, 
 	dst[3] = make_float4(m[12], m[13], m[14], m[15]);
 }
 
+// the arrays of one SoaTransforms, which is what the kernels take
+struct SoaArrays {
+	DeviceArray<double> px, py, pz;
+	DeviceArray<float4> rot;
+	DeviceArray<float> sx, sy, sz;
+	int alloc(lb200_ctx* ctx, uint32_t n) {
+		LB200_CUDA(ctx, px.alloc(n));
+		LB200_CUDA(ctx, py.alloc(n));
+		LB200_CUDA(ctx, pz.alloc(n));
+		LB200_CUDA(ctx, rot.alloc(n));
+		LB200_CUDA(ctx, sx.alloc(n));
+		LB200_CUDA(ctx, sy.alloc(n));
+		LB200_CUDA(ctx, sz.alloc(n));
+		return LB200_OK;
+	}
+	operator SoaTransforms() const { return SoaTransforms{px, py, pz, rot, sx, sy, sz}; }
+};
+
 } // namespace
 
 struct lb200_hierarchy {
 	lb200_ctx* ctx = nullptr;
 	uint32_t n = 0;
 	std::vector<uint32_t> level_start; // size depth + 1
-	uint32_t* d_order = nullptr;       // level position -> caller node index
-	uint32_t* d_pos_of_node = nullptr; // caller node index -> level position
-	// staging of set_subset: [node ids][transforms], pinned + device, two of each used in turn: an upload waits only for the upload before last
-	uint8_t* d_subset[2] = {nullptr, nullptr}; uint8_t* h_subset[2] = {nullptr, nullptr}; size_t subset_cap = 0; cudaEvent_t subset_done[2] = {nullptr, nullptr}; uint32_t subset_turn = 0;
-	int* d_parent = nullptr;           // level position -> parent's level position
-	SoaTransforms L, G;
-	lb200_transform* d_stage = nullptr; // n Transforms (API boundary)
-	float4* d_matrices = nullptr;       // n relative matrices (lb200_hierarchy_get_relative_matrices)
-	float* d_radius_in = nullptr;
-	double* d_sphere_pos = nullptr;
-	float* d_sphere_radius = nullptr;
+	DeviceArray<uint32_t> d_order;       // level position -> caller node index
+	DeviceArray<uint32_t> d_pos_of_node; // caller node index -> level position
+	// staging of set_subset: [node ids][transforms], pinned + device, two of each used in turn: an upload waits only for the upload before last.
+	// The four buffers are allocated and released together.
+	DeviceArray<uint8_t> d_subset[2]; PinnedArray<uint8_t> h_subset[2]; Event subset_done[2]; uint32_t subset_turn = 0;
+	DeviceArray<int> d_parent;           // level position -> parent's level position
+	SoaArrays L, G;
+	DeviceArray<lb200_transform> d_stage; // n Transforms (API boundary)
+	DeviceArray<float4> d_matrices;       // n relative matrices, 4 float4 each (lb200_hierarchy_get_relative_matrices)
+	// the inputs and outputs of spheres_kernel, allocated and released together
+	DeviceArray<float> d_radius_in;
+	DeviceArray<double> d_sphere_pos;
+	DeviceArray<float> d_sphere_radius;
 	uint64_t gather_bytes = 0;
 };
 
 namespace {
-
-int allocSoa(lb200_ctx* ctx, SoaTransforms& s, uint32_t n) {
-	LB200_CUDA(ctx, cudaMalloc(&s.px, sizeof(double) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.py, sizeof(double) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.pz, sizeof(double) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.rot, sizeof(float4) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.sx, sizeof(float) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.sy, sizeof(float) * n));
-	LB200_CUDA(ctx, cudaMalloc(&s.sz, sizeof(float) * n));
-	return LB200_OK;
-}
-
-void freeSoa(SoaTransforms& s) {
-	cudaFree(s.px); cudaFree(s.py); cudaFree(s.pz); cudaFree(s.rot); cudaFree(s.sx); cudaFree(s.sy); cudaFree(s.sz);
-}
 
 int upload(lb200_hierarchy* h, const lb200_transform* src, SoaTransforms dst, uint32_t count_levelorder) {
 	lb200_ctx* ctx = h->ctx;
@@ -234,6 +240,17 @@ int upload(lb200_hierarchy* h, const lb200_transform* src, SoaTransforms dst, ui
 	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_stage, src, sizeof(lb200_transform) * (size_t)h->n, cudaMemcpyHostToDevice, ctx->stream));
 	aos_to_soa_kernel<<<(count_levelorder + HT - 1) / HT, HT, 0, ctx->stream>>>(h->d_stage, h->d_order, count_levelorder, dst);
 	LB200_CHECK_LAUNCH(ctx);
+	return LB200_OK;
+}
+
+int allocSpheres(lb200_hierarchy* h) {
+	if (h->d_radius_in && h->d_sphere_pos && h->d_sphere_radius) return LB200_OK;
+	lb200_ctx* ctx = h->ctx;
+	DeviceArray<float> radius_in, sphere_radius; DeviceArray<double> sphere_pos;
+	LB200_CUDA(ctx, radius_in.alloc(h->n));
+	LB200_CUDA(ctx, sphere_pos.alloc(3 * (size_t)h->n));
+	LB200_CUDA(ctx, sphere_radius.alloc(h->n));
+	h->d_radius_in = std::move(radius_in); h->d_sphere_pos = std::move(sphere_pos); h->d_sphere_radius = std::move(sphere_radius);
 	return LB200_OK;
 }
 
@@ -274,7 +291,7 @@ int lb200_hierarchy_create(lb200_ctx* ctx, const int32_t* parents, uint32_t n, l
 	}
 	if (order.size() != n) { lb200_set_error(ctx, "hierarchy has a cycle (%zu of %u nodes reachable from roots)", order.size(), n); return LB200_ERR_INVALID; }
 
-	lb200_hierarchy* h = new (std::nothrow) lb200_hierarchy;
+	std::unique_ptr<lb200_hierarchy, decltype(&lb200_hierarchy_destroy)> h(new (std::nothrow) lb200_hierarchy, lb200_hierarchy_destroy);
 	if (!h) return LB200_ERR_CUDA;
 	h->ctx = ctx;
 	h->n = n;
@@ -287,20 +304,20 @@ int lb200_hierarchy_create(lb200_ctx* ctx, const int32_t* parents, uint32_t n, l
 	}
 	h->gather_bytes = distinct * 52;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	LB200_CUDA(ctx, cudaMalloc(&h->d_order, sizeof(uint32_t) * n));
-	LB200_CUDA(ctx, cudaMalloc(&h->d_parent, sizeof(int) * n));
-	LB200_CUDA(ctx, cudaMalloc(&h->d_stage, sizeof(lb200_transform) * (size_t)n));
-	int rc = allocSoa(ctx, h->L, n);
-	if (!rc) rc = allocSoa(ctx, h->G, n);
-	if (rc) { lb200_hierarchy_destroy(h); return rc; }
+	LB200_CUDA(ctx, h->d_order.alloc(n));
+	LB200_CUDA(ctx, h->d_parent.alloc(n));
+	LB200_CUDA(ctx, h->d_stage.alloc(n));
+	int rc = h->L.alloc(ctx, n);
+	if (!rc) rc = h->G.alloc(ctx, n);
+	if (rc) return rc;
 	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_order, order.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
 	std::vector<uint32_t> pos_of_node(n);
 	for (uint32_t i = 0; i < n; ++i) pos_of_node[order[i]] = i;
-	LB200_CUDA(ctx, cudaMalloc(&h->d_pos_of_node, sizeof(uint32_t) * n));
+	LB200_CUDA(ctx, h->d_pos_of_node.alloc(n));
 	LB200_CUDA(ctx, cudaMemcpy(h->d_pos_of_node, pos_of_node.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice));
 	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_parent, parent_pos.data(), sizeof(int) * n, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	*out = h;
+	*out = h.release();
 	return LB200_OK;
 }
 
@@ -308,9 +325,6 @@ void lb200_hierarchy_destroy(lb200_hierarchy* h) {
 	if (!h) return;
 	cudaSetDevice(h->ctx->device);
 	cudaStreamSynchronize(h->ctx->stream);
-	cudaFree(h->d_pos_of_node); for (int b = 0; b < 2; ++b) { cudaFree(h->d_subset[b]); if (h->h_subset[b]) cudaFreeHost(h->h_subset[b]); if (h->subset_done[b]) cudaEventDestroy(h->subset_done[b]); }
-	cudaFree(h->d_order); cudaFree(h->d_parent); cudaFree(h->d_stage); cudaFree(h->d_matrices); cudaFree(h->d_radius_in); cudaFree(h->d_sphere_pos); cudaFree(h->d_sphere_radius);
-	freeSoa(h->L); freeSoa(h->G);
 	delete h;
 }
 
@@ -382,11 +396,8 @@ int lb200_hierarchy_get_spheres(lb200_hierarchy* h, const float* bounding_radius
 	if (!h || !bounding_radius || !out_pos3 || !out_radius) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!h->d_radius_in) {
-		LB200_CUDA(ctx, cudaMalloc(&h->d_radius_in, sizeof(float) * h->n));
-		LB200_CUDA(ctx, cudaMalloc(&h->d_sphere_pos, sizeof(double) * 3 * (size_t)h->n));
-		LB200_CUDA(ctx, cudaMalloc(&h->d_sphere_radius, sizeof(float) * h->n));
-	}
+	int rc = allocSpheres(h);
+	if (rc) return rc;
 	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_radius_in, bounding_radius, sizeof(float) * h->n, cudaMemcpyHostToDevice, ctx->stream));
 	spheres_kernel<<<(h->n + HT - 1) / HT, HT, 0, ctx->stream>>>(h->G, h->d_order, h->d_radius_in, h->n, h->d_sphere_pos, h->d_sphere_radius);
 	LB200_CHECK_LAUNCH(ctx);
@@ -402,19 +413,19 @@ int lb200_hierarchy_set_subset(lb200_hierarchy* h, const uint32_t* nodes, const 
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	const size_t bytes = (sizeof(uint32_t) + sizeof(lb200_transform)) * (size_t)count + 16;
-	if (h->subset_cap < bytes) {
+	if (h->d_subset[1].size() < bytes) {
 		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		size_t cap = h->subset_cap ? h->subset_cap : 4096;
+		size_t cap = h->d_subset[1].size() ? h->d_subset[1].size() : 4096;
 		while (cap < bytes) cap *= 2;
+		for (int b = 0; b < 2; ++b) { h->d_subset[b].reset(); h->h_subset[b].reset(); } // before the new ones are allocated
+		DeviceArray<uint8_t> d_new[2]; PinnedArray<uint8_t> h_new[2];
 		for (int b = 0; b < 2; ++b) {
-			cudaFree(h->d_subset[b]); if (h->h_subset[b]) cudaFreeHost(h->h_subset[b]);
-			h->d_subset[b] = nullptr; h->h_subset[b] = nullptr;
-			LB200_CUDA(ctx, cudaMalloc(&h->d_subset[b], cap));
-			LB200_CUDA(ctx, cudaHostAlloc(&h->h_subset[b], cap, cudaHostAllocDefault));
-			if (!h->subset_done[b]) LB200_CUDA(ctx, cudaEventCreateWithFlags(&h->subset_done[b], cudaEventDisableTiming));
+			LB200_CUDA(ctx, d_new[b].alloc(cap));
+			LB200_CUDA(ctx, h_new[b].alloc(cap));
+			if (!h->subset_done[b]) LB200_CUDA(ctx, cudaEventCreateWithFlags(h->subset_done[b].create(), cudaEventDisableTiming));
 			LB200_CUDA(ctx, cudaEventRecord(h->subset_done[b], ctx->stream));
 		}
-		h->subset_cap = cap;
+		for (int b = 0; b < 2; ++b) { h->d_subset[b] = std::move(d_new[b]); h->h_subset[b] = std::move(h_new[b]); }
 	}
 	const uint32_t turn = h->subset_turn++ & 1u;
 	LB200_CUDA(ctx, cudaEventSynchronize(h->subset_done[turn])); // the upload before last has left this pair of buffers (no wait for the frame in flight)
@@ -434,12 +445,9 @@ int lb200_hierarchy_refresh_spheres(lb200_hierarchy* h, const float* bounding_ra
 	if (!h || !dev_pos3 || !dev_radius) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!h->d_radius_in) {
-		if (!bounding_radius) { lb200_set_error(ctx, "refresh_spheres: the first call needs the bounding radii"); return LB200_ERR_INVALID; }
-		LB200_CUDA(ctx, cudaMalloc(&h->d_radius_in, sizeof(float) * h->n));
-		LB200_CUDA(ctx, cudaMalloc(&h->d_sphere_pos, sizeof(double) * 3 * (size_t)h->n));
-		LB200_CUDA(ctx, cudaMalloc(&h->d_sphere_radius, sizeof(float) * h->n));
-	}
+	if (!h->d_radius_in && !bounding_radius) { lb200_set_error(ctx, "refresh_spheres: the first call needs the bounding radii"); return LB200_ERR_INVALID; }
+	int rc = allocSpheres(h);
+	if (rc) return rc;
 	if (bounding_radius) LB200_CUDA(ctx, cudaMemcpyAsync(h->d_radius_in, bounding_radius, sizeof(float) * h->n, cudaMemcpyHostToDevice, ctx->stream));
 	spheres_kernel<<<(h->n + HT - 1) / HT, HT, 0, ctx->stream>>>(h->G, h->d_order, h->d_radius_in, h->n, h->d_sphere_pos, h->d_sphere_radius);
 	LB200_CHECK_LAUNCH(ctx);
@@ -480,7 +488,7 @@ int lb200_hierarchy_get_relative_matrices(lb200_hierarchy* h, const double base_
 	if (!h || !base_pos || !out_matrices) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!h->d_matrices) LB200_CUDA(ctx, cudaMalloc(&h->d_matrices, sizeof(float) * 16 * (size_t)h->n));
+	if (!h->d_matrices) LB200_CUDA(ctx, h->d_matrices.alloc(4 * (size_t)h->n));
 	relative_matrices_kernel<<<(h->n + HT - 1) / HT, HT, 0, ctx->stream>>>(h->G, h->d_order, h->n, base_pos[0], base_pos[1], base_pos[2], h->d_matrices);
 	LB200_CHECK_LAUNCH(ctx);
 	LB200_CUDA(ctx, cudaMemcpyAsync(out_matrices, h->d_matrices, sizeof(float) * 16 * (size_t)h->n, cudaMemcpyDeviceToHost, ctx->stream));

@@ -10,19 +10,99 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
+#include <utility>
+
+// ---- Owning handles of the CUDA resources the library allocates for itself ----
+// A handle frees its resource when it is destroyed or re-allocated, so an object's destructor releases everything it owns.  An
+// empty handle makes no CUDA call at all: a culling system without a context never touches the runtime.  Arrays record their
+// element count, so no separate capacity can disagree with the pointer.  Handles convert to the raw pointer or handle, which is
+// what kernels, their parameter structs and the runtime calls take.
+struct lb200_device_mem {
+	static cudaError_t alloc(void** p, size_t bytes) { return cudaMalloc(p, bytes); }
+	static void release(void* p) { cudaFree(p); }
+};
+template <unsigned Flags> struct lb200_pinned_mem {
+	static cudaError_t alloc(void** p, size_t bytes) { return cudaHostAlloc(p, bytes, Flags); }
+	static void release(void* p) { cudaFreeHost(p); }
+};
+
+template <class T, class Mem> class lb200_array {
+public:
+	lb200_array() = default;
+	lb200_array(lb200_array&& o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+	lb200_array& operator=(lb200_array&& o) noexcept {
+		if (this != &o) { reset(); p_ = std::exchange(o.p_, nullptr); n_ = std::exchange(o.n_, 0); }
+		return *this;
+	}
+	~lb200_array() { reset(); }
+	void reset() {
+		if (p_) Mem::release(p_);
+		p_ = nullptr;
+		n_ = 0;
+	}
+	// Frees what the handle holds, then allocates n elements (bytes_if_empty bytes when n is 0, so that an empty table can still have
+	// an address).  Returns the runtime's error for LB200_CUDA to report; a failed allocation leaves the handle empty with size 0.
+	cudaError_t alloc(size_t n, size_t bytes_if_empty = 0) {
+		reset();
+		void* p = nullptr;
+		const cudaError_t e = Mem::alloc(&p, n ? sizeof(T) * n : bytes_if_empty);
+		if (e != cudaSuccess) {
+			cudaGetLastError(); // an allocation failure is reported here, not by the next kernel launch check
+			return e;
+		}
+		p_ = static_cast<T*>(p);
+		n_ = p ? n : 0;
+		return cudaSuccess;
+	}
+	size_t size() const { return n_; }
+	T* get() const { return p_; }
+	operator T*() const { return p_; }
+
+private:
+	T* p_ = nullptr;
+	size_t n_ = 0;
+};
+template <class T> using DeviceArray = lb200_array<T, lb200_device_mem>;
+template <class T, unsigned Flags = cudaHostAllocDefault> using PinnedArray = lb200_array<T, lb200_pinned_mem<Flags>>;
+
+template <class H, cudaError_t (*Destroy)(H)> class lb200_handle {
+public:
+	lb200_handle() = default;
+	lb200_handle(lb200_handle&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+	lb200_handle& operator=(lb200_handle&& o) noexcept {
+		if (this != &o) { reset(); h_ = std::exchange(o.h_, nullptr); }
+		return *this;
+	}
+	~lb200_handle() { reset(); }
+	void reset() {
+		if (h_) Destroy(h_);
+		h_ = nullptr;
+	}
+	// destroys what the handle holds and returns where a cudaEventCreate* / cudaStreamCreate* call stores the new one
+	H* create() {
+		reset();
+		return &h_;
+	}
+	operator H() const { return h_; }
+
+private:
+	H h_ = nullptr;
+};
+using Event = lb200_handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = lb200_handle<cudaStream_t, cudaStreamDestroy>;
 
 #define LB200_MAX_RANKS 8
 #define LB200_MAX_LANES 8  // concurrent culls (streams / output lanes); exchange buffers = 3 x lanes
 
 struct lb200_ctx {
 	int device = -1;
-	cudaStream_t stream = nullptr;
-	cudaStream_t copy_stream = nullptr;
+	Stream stream;
+	Stream copy_stream;
 	int sm_count = 0;
 	std::atomic<uint64_t> launches{0};
 	char error[512] = {0};
-	// scratch of lb200_radix_sort_device (sortkeys.cu) for up to sort_scratch_cap pairs; freed by lb200_shutdown
-	void* sort_scratch = nullptr;
+	// scratch of lb200_radix_sort_device (sortkeys.cu); its size in bytes follows the pair capacity sort_scratch_cap
+	DeviceArray<uint8_t> sort_scratch;
 	uint32_t sort_scratch_cap = 0;
 	// NCCL (dlopen) state, see comm.cu
 	void* nccl_lib = nullptr;
@@ -42,16 +122,17 @@ struct lb200_ctx {
 		// tests/test_exchange_protocol_model.py replays both kinds, mixed as callers issue them, under a random scheduler, and shows that
 		// fewer buffers or no flow control would not do.
 		uint32_t lanes = 1, n_buffers = 3;
-		void* local_block = nullptr;      // this rank's allocation: [flags n_buffers x 8 x u32 in 512 B][gather 0] .. [gather n_buffers-1]
+		DeviceArray<char> local_block;    // this rank's allocation: [flags n_buffers x 8 x u32 in 512 B][gather 0] .. [gather n_buffers-1]
 		uint32_t* gather[3 * LB200_MAX_LANES][LB200_MAX_RANKS] = {}; // gather[b][r] = rank r's buffer b as seen from this process
 		uint32_t* flags[LB200_MAX_RANKS] = {};     // flags[r] = rank r's flag block
-		void* opened[LB200_MAX_RANKS] = {};        // cudaIpcOpenMemHandle results to close
-		uint32_t* done_counter = nullptr; // local, one per lane, for the last-block election
+		// cudaIpcOpenMemHandle results, raw: comm.cu closes them before local_block is freed, an order the peer protocol depends on
+		void* opened[LB200_MAX_RANKS] = {};
+		DeviceArray<uint32_t> done_counter; // local, one per lane, for the last-block election
 		uint32_t epoch = 0;
 		// a wait kernel that gave up on a peer (~4 s) raises this word; page-locked + mapped so the host sees it without a copy.
 		// lb200_comm_check() turns it into LB200_ERR_NCCL and resets it (called by lb200_synchronize and every exchange entry point)
-		uint32_t* h_timeout = nullptr;
-		uint32_t* d_timeout = nullptr;
+		PinnedArray<uint32_t, cudaHostAllocMapped> h_timeout;
+		uint32_t* d_timeout = nullptr; // h_timeout as the device addresses it
 	} peer;
 };
 

@@ -31,6 +31,7 @@
 #include "lb200_math.cuh"
 
 #include <algorithm>
+#include <memory>
 #include <stdlib.h>
 #include <new>
 
@@ -781,10 +782,9 @@ extern "C" int lb200_radix_sort_device(lb200_ctx* ctx, uint64_t* dev_keys, uint6
 	const uint32_t scratch_cap = std::max(cap, 1u);
 	if (scratch_cap > ctx->sort_scratch_cap) { // the stream may still use the old scratch
 		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		cudaFree(ctx->sort_scratch);
-		ctx->sort_scratch = nullptr;
+		ctx->sort_scratch.reset();
 		ctx->sort_scratch_cap = 0;
-		LB200_CUDA(ctx, cudaMalloc(&ctx->sort_scratch, sort_scratch_bytes(scratch_cap, limit)));
+		LB200_CUDA(ctx, ctx->sort_scratch.alloc(sort_scratch_bytes(scratch_cap, limit)));
 		ctx->sort_scratch_cap = scratch_cap;
 	}
 	const SortScratch sc = sort_scratch_at(ctx->sort_scratch, ctx->sort_scratch_cap);
@@ -801,88 +801,79 @@ struct lb200_sortkeys {
 	uint32_t max_entities = 0, max_groups = 0;
 	uint32_t cap_keys = 0, cap_recs = 0;
 	// inputs
-	SkEntity* d_ent = nullptr;         // one 64-byte record per entity (transform, model / flags, lod and pose-frame state)
+	DeviceArray<SkEntity> d_ent;       // one 64-byte record per entity (transform, model / flags, lod and pose-frame state)
 	bool have_transforms = false;
-	uint32_t* d_decal_sort_key = nullptr; uint8_t* d_decal_layer = nullptr;
-	lb200_sk_model* d_models = nullptr; lb200_sk_mesh* d_meshes = nullptr; uint32_t n_models = 0, n_meshes = 0;
-	uint8_t* d_group_layer = nullptr;  // layer of the mesh material a sort key (= auto-instancer group) belongs to
+	DeviceArray<uint32_t> d_decal_sort_key; DeviceArray<uint8_t> d_decal_layer;
+	DeviceArray<lb200_sk_model> d_models; DeviceArray<lb200_sk_mesh> d_meshes; // both set or both empty (lb200_sortkeys_set_models)
+	DeviceArray<uint8_t> d_group_layer; // layer of the mesh material a sort key (= auto-instancer group) belongs to
 	// outputs
-	uint64_t *d_keys[2] = {}, *d_values[2] = {};
-	uint32_t* d_counts = nullptr; uint32_t* h_counts = nullptr; // pinned
-	uint32_t *d_group_count = nullptr, *d_group_offset = nullptr, *d_group_cursor = nullptr;
-	uint64_t* d_group_renderables = nullptr; float4* d_instance_data = nullptr;
-	uint32_t *d_pose_list = nullptr, *d_dirty_list = nullptr, *d_stash = nullptr; float4* d_stash4 = nullptr; // the two passes' hand-over: one word + 3 x float4 per visible renderable
-	float* d_lod = nullptr; uint32_t* d_pose_frame = nullptr; // unpacked on request (lb200_sortkeys_device_outputs)
-	uint32_t* d_moved_list = nullptr; uint32_t* d_moved_count = nullptr; lb200_transform* d_prev = nullptr; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move onwards)
-	GridBar* d_bar = nullptr;
-	SortState* d_sort_state = nullptr; uint32_t* d_block_hist = nullptr;
+	DeviceArray<uint64_t> d_keys[2], d_values[2];
+	DeviceArray<uint32_t> d_counts; PinnedArray<uint32_t> h_counts;
+	DeviceArray<uint32_t> d_group_count, d_group_offset, d_group_cursor;
+	DeviceArray<uint64_t> d_group_renderables; DeviceArray<float4> d_instance_data;
+	DeviceArray<uint32_t> d_pose_list, d_dirty_list, d_stash; DeviceArray<float4> d_stash4; // the two passes' hand-over: one word + 3 x float4 per visible renderable
+	DeviceArray<float> d_lod; DeviceArray<uint32_t> d_pose_frame; // unpacked on request (lb200_sortkeys_device_outputs)
+	DeviceArray<uint32_t> d_moved_list, d_moved_count; DeviceArray<lb200_transform> d_prev; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move onwards)
+	DeviceArray<GridBar> d_bar;
+	DeviceArray<SortState> d_sort_state; DeviceArray<uint32_t> d_block_hist;
 	uint32_t sort_blocks = 0;
 	uint32_t last_groups = 0;
 	uint32_t keys_grid_limit[2] = {0, 0}; // co-resident blocks of create_keys_kernel: group counters in shared memory / in HBM
 };
 
 namespace {
-// host array -> temporary device buffer on the context stream (setters are not on the per-frame path)
-template <typename T> int upload_temp(lb200_ctx* ctx, const T* host, size_t n, T** dev) {
-	*dev = nullptr;
+// host array (may be null: nothing to upload) -> temporary device buffer on the context stream (setters are not on the per-frame path)
+template <typename T> int upload_temp(lb200_ctx* ctx, const T* host, size_t n, DeviceArray<T>& dev) {
 	if (!host) return LB200_OK;
-	LB200_CUDA(ctx, cudaMalloc(dev, sizeof(T) * n));
-	LB200_CUDA(ctx, cudaMemcpyAsync(*dev, host, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, dev.alloc(n));
+	LB200_CUDA(ctx, cudaMemcpyAsync(dev, host, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
 	return LB200_OK;
 }
 } // namespace
 
 extern "C" {
 
-static int sortkeysAllocate(lb200_sortkeys* sk, lb200_ctx* ctx, uint32_t max_entities, uint32_t max_groups, uint32_t max_keys, uint32_t max_instances);
-
 int lb200_sortkeys_create(lb200_ctx* ctx, uint32_t max_entities, uint32_t max_groups, uint32_t max_keys, uint32_t max_instances, lb200_sortkeys** out) {
 	if (!ctx || !out || !max_entities || !max_groups) return LB200_ERR_INVALID;
 	*out = nullptr;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	lb200_sortkeys* sk = new (std::nothrow) lb200_sortkeys;
+	std::unique_ptr<lb200_sortkeys, decltype(&lb200_sortkeys_destroy)> sk(new (std::nothrow) lb200_sortkeys, lb200_sortkeys_destroy);
 	if (!sk) return LB200_ERR_CUDA;
 	sk->ctx = ctx;
-	const int rc = sortkeysAllocate(sk, ctx, max_entities, max_groups, max_keys, max_instances);
-	if (rc) { lb200_sortkeys_destroy(sk); return rc; } // whatever was allocated before the failure goes back (cudaFree(nullptr) is a no-op)
-	*out = sk;
-	return LB200_OK;
-}
-
-static int sortkeysAllocate(lb200_sortkeys* sk, lb200_ctx* ctx, uint32_t max_entities, uint32_t max_groups, uint32_t max_keys, uint32_t max_instances) {
 	sk->max_entities = max_entities; sk->max_groups = max_groups;
 	sk->cap_keys = max_keys ? max_keys : max_entities; sk->cap_recs = max_instances ? max_instances : max_entities;
 	const size_t E = max_entities;
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_ent, sizeof(SkEntity) * E));
+	LB200_CUDA(ctx, sk->d_ent.alloc(E));
 	ent_init_kernel<<<(uint32_t)((E + 255) / 256), 256, 0, ctx->stream>>>(sk->d_ent, max_entities);
 	LB200_CHECK_LAUNCH(ctx);
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_decal_sort_key, sizeof(uint32_t) * E));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_decal_layer, E));
+	LB200_CUDA(ctx, sk->d_decal_sort_key.alloc(E));
+	LB200_CUDA(ctx, sk->d_decal_layer.alloc(E));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_decal_sort_key, 0, sizeof(uint32_t) * E, ctx->stream));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_decal_layer, 0, E, ctx->stream));
 	for (int b = 0; b < 2; ++b) {
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_keys[b], sizeof(uint64_t) * sk->cap_keys));
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_values[b], sizeof(uint64_t) * sk->cap_keys));
+		LB200_CUDA(ctx, sk->d_keys[b].alloc(sk->cap_keys));
+		LB200_CUDA(ctx, sk->d_values[b].alloc(sk->cap_keys));
 	}
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_counts, sizeof(uint32_t) * CNT_WORDS));
-	LB200_CUDA(ctx, cudaHostAlloc(&sk->h_counts, sizeof(uint32_t) * CNT_WORDS, cudaHostAllocDefault));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_group_count, sizeof(uint32_t) * max_groups));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_group_offset, sizeof(uint32_t) * max_groups));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_group_cursor, sizeof(uint32_t) * max_groups));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_group_layer, max_groups));
+	LB200_CUDA(ctx, sk->d_counts.alloc(CNT_WORDS));
+	LB200_CUDA(ctx, sk->h_counts.alloc(CNT_WORDS));
+	LB200_CUDA(ctx, sk->d_group_count.alloc(max_groups));
+	LB200_CUDA(ctx, sk->d_group_offset.alloc(max_groups));
+	LB200_CUDA(ctx, sk->d_group_cursor.alloc(max_groups));
+	LB200_CUDA(ctx, sk->d_group_layer.alloc(max_groups));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_group_layer, 0, max_groups, ctx->stream));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_group_renderables, sizeof(uint64_t) * sk->cap_recs));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_instance_data, 48 * (size_t)sk->cap_recs));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_pose_list, sizeof(uint32_t) * E));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_dirty_list, sizeof(uint32_t) * E));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_stash, sizeof(uint32_t) * E));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_stash4, sizeof(float4) * 3 * E));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_bar, sizeof(GridBar)));
+	LB200_CUDA(ctx, sk->d_group_renderables.alloc(sk->cap_recs));
+	LB200_CUDA(ctx, sk->d_instance_data.alloc(3 * (size_t)sk->cap_recs)); // 48 bytes per instance
+	LB200_CUDA(ctx, sk->d_pose_list.alloc(E));
+	LB200_CUDA(ctx, sk->d_dirty_list.alloc(E));
+	LB200_CUDA(ctx, sk->d_stash.alloc(E));
+	LB200_CUDA(ctx, sk->d_stash4.alloc(3 * E));
+	LB200_CUDA(ctx, sk->d_bar.alloc(1));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_bar, 0, sizeof(GridBar), ctx->stream));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_sort_state, sizeof(SortState)));
+	LB200_CUDA(ctx, sk->d_sort_state.alloc(1));
 	sk->sort_blocks = (uint32_t)ctx->sm_count * 2;
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_block_hist, sizeof(uint32_t) * 256 * sk->sort_blocks));
+	LB200_CUDA(ctx, sk->d_block_hist.alloc(256 * (size_t)sk->sort_blocks));
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	*out = sk.release();
 	return LB200_OK;
 }
 
@@ -890,13 +881,6 @@ void lb200_sortkeys_destroy(lb200_sortkeys* sk) {
 	if (!sk) return;
 	cudaSetDevice(sk->ctx->device);
 	cudaStreamSynchronize(sk->ctx->stream);
-	cudaFree(sk->d_ent); cudaFree(sk->d_decal_sort_key); cudaFree(sk->d_decal_layer); cudaFree(sk->d_models); cudaFree(sk->d_meshes); cudaFree(sk->d_group_layer);
-	for (int b = 0; b < 2; ++b) { cudaFree(sk->d_keys[b]); cudaFree(sk->d_values[b]); }
-	cudaFree(sk->d_counts); if (sk->h_counts) cudaFreeHost(sk->h_counts);
-	cudaFree(sk->d_group_count); cudaFree(sk->d_group_offset); cudaFree(sk->d_group_cursor);
-	cudaFree(sk->d_group_renderables); cudaFree(sk->d_instance_data); cudaFree(sk->d_pose_list); cudaFree(sk->d_dirty_list); cudaFree(sk->d_stash); cudaFree(sk->d_stash4);
-	cudaFree(sk->d_lod); cudaFree(sk->d_pose_frame); cudaFree(sk->d_bar); cudaFree(sk->d_moved_list); cudaFree(sk->d_moved_count); cudaFree(sk->d_prev);
-	cudaFree(sk->d_sort_state); cudaFree(sk->d_block_hist);
 	delete sk;
 }
 
@@ -906,10 +890,11 @@ int lb200_sortkeys_set_models(lb200_sortkeys* sk, const lb200_sk_model* models, 
 	if (n_models > CODE_MODEL_MASK + 1u) { lb200_set_error(ctx, "%u models: the entity record keeps 24 bits of model index", n_models); return LB200_ERR_INVALID; }
 	for (uint32_t i = 0; i < n_meshes; ++i) if (meshes[i].sort_key >= sk->max_groups) { lb200_set_error(ctx, "mesh %u: sort key %u >= max_groups %u", i, meshes[i].sort_key, sk->max_groups); return LB200_ERR_INVALID; }
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-	cudaFree(sk->d_models); cudaFree(sk->d_meshes);
-	sk->d_models = nullptr; sk->d_meshes = nullptr;
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_models, sizeof(lb200_sk_model) * n_models));
-	LB200_CUDA(ctx, cudaMalloc(&sk->d_meshes, sizeof(lb200_sk_mesh) * n_meshes));
+	sk->d_models.reset(); sk->d_meshes.reset(); // both go before either is allocated again
+	DeviceArray<lb200_sk_model> d_models; DeviceArray<lb200_sk_mesh> d_meshes;
+	LB200_CUDA(ctx, d_models.alloc(n_models));
+	LB200_CUDA(ctx, d_meshes.alloc(n_meshes));
+	sk->d_models = std::move(d_models); sk->d_meshes = std::move(d_meshes);
 	LB200_CUDA(ctx, cudaMemcpyAsync(sk->d_models, models, sizeof(lb200_sk_model) * n_models, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaMemcpyAsync(sk->d_meshes, meshes, sizeof(lb200_sk_mesh) * n_meshes, cudaMemcpyHostToDevice, ctx->stream));
 	// a sort key stands for one (mesh, material) pair (RenderModule::computeSortKey): the layer a group's key is bucketed by (:3958-3969)
@@ -922,7 +907,6 @@ int lb200_sortkeys_set_models(lb200_sortkeys* sk, const lb200_sk_model* models, 
 	cudaStreamSynchronize(ctx->stream);
 	delete[] layer;
 	LB200_CUDA(ctx, e);
-	sk->n_models = n_models; sk->n_meshes = n_meshes;
 	return LB200_OK;
 }
 
@@ -933,41 +917,33 @@ int lb200_sortkeys_set_instances(lb200_sortkeys* sk, uint32_t n, const uint32_t*
 	if (!sk || n > sk->max_entities) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = sk->ctx;
 	if (!n) return LB200_OK;
-	uint32_t *t_model = nullptr, *t_pose = nullptr; float* t_lod = nullptr; uint8_t* t_flags = nullptr;
-	int rc = upload_temp(ctx, model_of, n, &t_model);
-	if (!rc) rc = upload_temp(ctx, lod, n, &t_lod);
-	if (!rc) rc = upload_temp(ctx, flags, n, &t_flags);
-	if (!rc) rc = upload_temp(ctx, pose_frame, n, &t_pose);
-	if (!rc && (t_model || t_lod || t_flags || t_pose)) {
-		ent_pack_fields_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, n, t_model, t_lod, t_flags, t_pose);
-		ctx->launches.fetch_add(1, std::memory_order_relaxed);
-		if (cudaGetLastError() != cudaSuccess) { lb200_set_error(ctx, "ent_pack_fields_kernel launch failed"); rc = LB200_ERR_CUDA; }
-	}
-	cudaError_t e = cudaSuccess;
-	if (!rc && decal_sort_key) e = cudaMemcpyAsync(sk->d_decal_sort_key, decal_sort_key, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream);
-	if (!rc && e == cudaSuccess && decal_layer) e = cudaMemcpyAsync(sk->d_decal_layer, decal_layer, n, cudaMemcpyHostToDevice, ctx->stream);
-	const cudaError_t e2 = cudaStreamSynchronize(ctx->stream);
-	cudaFree(t_model); cudaFree(t_lod); cudaFree(t_flags); cudaFree(t_pose);
+	DeviceArray<uint32_t> t_model, t_pose; DeviceArray<float> t_lod; DeviceArray<uint8_t> t_flags;
+	int rc = upload_temp(ctx, model_of, n, t_model);
+	if (!rc) rc = upload_temp(ctx, lod, n, t_lod);
+	if (!rc) rc = upload_temp(ctx, flags, n, t_flags);
+	if (!rc) rc = upload_temp(ctx, pose_frame, n, t_pose);
 	if (rc) return rc;
-	LB200_CUDA(ctx, e);
-	LB200_CUDA(ctx, e2);
+	if (t_model || t_lod || t_flags || t_pose) {
+		ent_pack_fields_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, n, t_model, t_lod, t_flags, t_pose);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	if (decal_sort_key) LB200_CUDA(ctx, cudaMemcpyAsync(sk->d_decal_sort_key, decal_sort_key, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+	if (decal_layer) LB200_CUDA(ctx, cudaMemcpyAsync(sk->d_decal_layer, decal_layer, n, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	return LB200_OK;
 }
 
 int lb200_sortkeys_set_transforms(lb200_sortkeys* sk, const lb200_transform* transforms, uint32_t n) {
 	if (!sk || !transforms || n > sk->max_entities) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = sk->ctx;
-	lb200_transform* tmp = nullptr;
-	int rc = upload_temp(ctx, transforms, n, &tmp);
-	if (!rc && n) {
-		ent_pack_transforms_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, tmp, n);
-		ctx->launches.fetch_add(1, std::memory_order_relaxed);
-		if (cudaGetLastError() != cudaSuccess) { lb200_set_error(ctx, "ent_pack_transforms_kernel launch failed"); rc = LB200_ERR_CUDA; }
-	}
-	const cudaError_t e = cudaStreamSynchronize(ctx->stream);
-	cudaFree(tmp);
+	DeviceArray<lb200_transform> tmp;
+	const int rc = upload_temp(ctx, transforms, n, tmp);
 	if (rc) return rc;
-	LB200_CUDA(ctx, e);
+	if (n) {
+		ent_pack_transforms_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, tmp, n);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // before tmp is freed
 	sk->have_transforms = true;
 	return LB200_OK;
 }
@@ -1042,9 +1018,11 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 int lb200_sortkeys_device_outputs(lb200_sortkeys* sk, lb200_sk_outputs* out) {
 	if (!sk || !out) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = sk->ctx;
-	if (!sk->d_lod) {
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_lod, sizeof(float) * (size_t)sk->max_entities));
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_pose_frame, sizeof(uint32_t) * (size_t)sk->max_entities));
+	if (!sk->d_lod || !sk->d_pose_frame) {
+		DeviceArray<float> lod; DeviceArray<uint32_t> pose_frame;
+		LB200_CUDA(ctx, lod.alloc(sk->max_entities));
+		LB200_CUDA(ctx, pose_frame.alloc(sk->max_entities));
+		sk->d_lod = std::move(lod); sk->d_pose_frame = std::move(pose_frame);
 	}
 	ent_unpack_state_kernel<<<(sk->max_entities + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, sk->d_lod, sk->d_pose_frame);
 	LB200_CHECK_LAUNCH(ctx);
@@ -1065,12 +1043,14 @@ int lb200_sortkeys_move_device(lb200_sortkeys* sk, const int32_t* dev_entities, 
 	if (!n) return LB200_OK;
 	lb200_ctx* ctx = sk->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!sk->d_moved_list) {
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_moved_list, sizeof(uint32_t) * (size_t)sk->max_entities));
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_moved_count, sizeof(uint32_t)));
-		LB200_CUDA(ctx, cudaMemsetAsync(sk->d_moved_count, 0, sizeof(uint32_t), ctx->stream));
-		LB200_CUDA(ctx, cudaMalloc(&sk->d_prev, sizeof(lb200_transform) * (size_t)sk->max_entities));
-		LB200_CUDA(ctx, cudaMemsetAsync(sk->d_prev, 0, sizeof(lb200_transform) * (size_t)sk->max_entities, ctx->stream));
+	if (!sk->d_moved_list || !sk->d_moved_count || !sk->d_prev) { // end_frame tests d_moved_list alone: all three or none
+		DeviceArray<uint32_t> moved_list, moved_count; DeviceArray<lb200_transform> prev;
+		LB200_CUDA(ctx, moved_list.alloc(sk->max_entities));
+		LB200_CUDA(ctx, moved_count.alloc(1));
+		LB200_CUDA(ctx, cudaMemsetAsync(moved_count, 0, sizeof(uint32_t), ctx->stream));
+		LB200_CUDA(ctx, prev.alloc(sk->max_entities));
+		LB200_CUDA(ctx, cudaMemsetAsync(prev, 0, sizeof(lb200_transform) * (size_t)sk->max_entities, ctx->stream));
+		sk->d_moved_list = std::move(moved_list); sk->d_moved_count = std::move(moved_count); sk->d_prev = std::move(prev);
 	}
 	ent_move_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, dev_entities, dev_transforms, n, dev_bounding_radius, dev_out_pos3, dev_out_radius, sk->d_moved_list, sk->d_moved_count);
 	LB200_CHECK_LAUNCH(ctx);

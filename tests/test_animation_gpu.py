@@ -147,17 +147,19 @@ def test_blend_layers_match_oracle(ctx, oracle):
     lw[::7, 1] = 1.0       # replacement instead of blending
     lw[::11, 0] = 0.99995  # just above the switch
     lw[::13, 2] = 0.0
-    anim.setLayers(lci, ltt, lw)
-    anim.update(0.0, lb.PALETTE_DUAL_QUAT | lb.PALETTE_MATRIX | lb.PALETTE_POSE)
-    pos, rot = anim.getPose()
-    dq, mtx = anim.getDualQuats(), anim.getMatrices()
-    for i in list(range(0, n_inst, 7)) + [1, 2, n_inst - 1]:
-        p, r = oracle.pose_evaluate(sk, clips[ci[i]], tt[i], compute_absolute=False)
-        for k in range(n_layers):
-            p, r = oracle.pose_evaluate(sk, clips[lci[i, k]], ltt[i, k], weight=float(lw[i, k]), start_from_bind=False, compute_absolute=False, pos=p, rot=r)
-        p, r = oracle.pose_compute_absolute(sk, p, r)
-        edq, emtx = oracle.palettes(sk, p, r)
-        _close(pos[i], p, "layered pose.pos"); _close(rot[i], r, "layered pose.rot"); _close(dq[i], edq, "layered dq"); _close(mtx[i], emtx, "layered mtx")
+    # one layer first, then all of them: the second call replaces the layer tables with larger ones
+    for k_used in (1, n_layers):
+        anim.setLayers(lci[:, :k_used], ltt[:, :k_used], lw[:, :k_used])
+        anim.update(0.0, lb.PALETTE_DUAL_QUAT | lb.PALETTE_MATRIX | lb.PALETTE_POSE)
+        pos, rot = anim.getPose()
+        dq, mtx = anim.getDualQuats(), anim.getMatrices()
+        for i in list(range(0, n_inst, 7)) + [1, 2, n_inst - 1]:
+            p, r = oracle.pose_evaluate(sk, clips[ci[i]], tt[i], compute_absolute=False)
+            for k in range(k_used):
+                p, r = oracle.pose_evaluate(sk, clips[lci[i, k]], ltt[i, k], weight=float(lw[i, k]), start_from_bind=False, compute_absolute=False, pos=p, rot=r)
+            p, r = oracle.pose_compute_absolute(sk, p, r)
+            edq, emtx = oracle.palettes(sk, p, r)
+            _close(pos[i], p, "layered pose.pos"); _close(rot[i], r, "layered pose.rot"); _close(dq[i], edq, "layered dq"); _close(mtx[i], emtx, "layered mtx")
     # removing the layers gives the plain single-clip result again
     anim.setLayers(None, None, None)
     anim.update(0.0, lb.PALETTE_POSE)

@@ -418,3 +418,54 @@ def test_device_rebinning_equals_host_set(ctx, oracle):
                 alive[gone] = False
             assert np.array_equal(seen, alive)
     cs.close()
+
+
+def test_buffers_grow_after_first_use(ctx, oracle):
+    """Every buffer that grows on demand is re-allocated after its first use, and the results stay equal to the oracle's: more entities
+    than the page arrays and the output ids were sized for, a sparse upload of more pages than the first one staged, and a device
+    re-binning batch with more movers, entities and pages than the first batch."""
+    rng = np.random.default_rng(44)
+    n, n0 = 200_000, 20_000
+    scene = scenes.cull_scene(n, (30000.0, 300.0, 30000.0), seed=61, type_probs=(0.7, 0.2, 0.1))
+    pos, rad = scene["pos"].copy(), scene["radius"].copy()
+    cs = lb.CullingSystem(ctx)
+    oc = oracle.OracleCulling()
+    a = scenes.c1_frustum_args()
+    views = [lb.frustum_perspective(**dict(a, far=20000.0)), lb.frustum_ortho((0.0, 0.0, 40000.0), (0.0, 0.0, 1.0), (0.0, 1.0, 0.0), 40000.0, 40000.0, 0.0, 80000.0)]
+
+    def check(step):
+        for f in views:
+            res = cs.cull(f)
+            oi, ot, _ = oc.cull(lb.culling.frustum_bytes(f))
+            assert res.total == len(oi) and np.array_equal(_canon(res), np.sort(oi.astype(np.int64) * 256 + ot)), step
+
+    def move(ids, sigma):
+        pos[ids] += rng.normal(size=(len(ids), 3)) * np.array([sigma, 1.0, sigma])
+        cs.setPosition(ids, pos[ids]); oc.set_position(ids, pos[ids])
+
+    def rebin(ids, max_entity):
+        pos[ids] += rng.normal(size=(len(ids), 3)) * np.array([400.0, 10.0, 400.0])
+        d_ents, d_pos, d_rad = ctx.to_device(ids), ctx.to_device(pos[ids]), ctx.to_device(rad[ids])
+        cs.set_many_device(d_pos, d_rad, len(ids), dev_entities=d_ents, max_entity=max_entity)
+        for p in (d_ents, d_pos, d_rad):
+            ctx.free_device(p)
+        oc.set(ids, pos[ids], rad[ids])
+
+    def add(lo, hi):
+        s = slice(lo, hi)
+        cs.add(scene["entities"][s], scene["types"][s], pos[s], rad[s]); oc.add(scene["entities"][s], scene["types"][s], pos[s], rad[s])
+
+    add(0, n0)
+    check("first upload")
+    move(rng.choice(n0, 10, replace=False).astype(np.int32), 50.0)  # a sparse upload of a few pages
+    check("small sparse upload")
+    rebin(rng.choice(n0, 1000, replace=False).astype(np.int32), n0 - 1)
+    check("small re-binning batch")
+    add(n0, n)  # ten times the entities: the page arrays and output ids grow
+    check("grown scene")
+    assert cs.page_count() > 8 * 2 * 800
+    move(rng.choice(n, 800, replace=False).astype(np.int32), 50.0)  # still a sparse upload, of more pages than the first one
+    check("large sparse upload")
+    rebin(rng.permutation(n).astype(np.int32), n - 1)  # more movers, entities and pages than the first batch
+    check("large re-binning batch")
+    cs.close()

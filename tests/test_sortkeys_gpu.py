@@ -46,6 +46,7 @@ def test_sort_keys_match_oracle_over_frames(ctx, oracle, n, seed, is_shadow, key
     oc = oracle.OracleCulling()
     oc.add(scene["entities"], scene["types"], scene["pos"], scene["radius"])
     S = lb.SortKeys(ctx, n, sk["max_sort_key"] + 1, max_keys=4 * n, max_instances=4 * n)
+    S.setModels(sk["models"][:1], sk["meshes"][:1])  # replaced by the larger tables below: the second call re-allocates both
     S.setModels(sk["models"], sk["meshes"])
     S.setInstances(sk["model_of"], sk["lod"], sk["flags"], sk["pose_frame"], sk["decal_sort_key"], sk["decal_layer"])
     S.setTransforms(sk["transforms"])
