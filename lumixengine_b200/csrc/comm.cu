@@ -58,7 +58,7 @@ static int loadNccl(lb200_ctx* ctx) {
 		}                                                                                                      \
 	} while (0)
 
-// used by culling.cu: all-gather `words` u32 per rank on the context stream (asynchronous)
+// used by culling_exchange.cu: all-gather `words` u32 per rank on the context stream (asynchronous)
 int lb200_comm_allgather_u32(lb200_ctx* ctx, const uint32_t* send, uint32_t* recv, size_t words) {
 	if (!ctx->nccl_comm) { lb200_set_error(ctx, "lb200_comm_init has not been called"); return LB200_ERR_STATE; }
 	LB200_NCCL(ctx, p_ncclAllGather(send, recv, words, ncclUint32_dt, (ncclComm_t)ctx->nccl_comm, ctx->stream));

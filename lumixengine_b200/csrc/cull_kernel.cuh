@@ -25,6 +25,7 @@
 // HBM-bound: 32 B descriptor per page + 16 B per tested sphere + 4 B read + 4 B write per visible id + 32 B mask row per page.
 #pragma once
 
+#include "culling_internal.h" // counter and slab layout
 #include "lb200_internal.h"
 #include "lb200_math.cuh"
 
@@ -33,11 +34,6 @@ namespace lbcull {
 using namespace lb;
 
 constexpr int ROWS = 7;                 // ceil(200 / 32)
-constexpr int N_STATS = 8;
-enum { ST_PAGES_TESTED = 0, ST_PAGES_INSIDE, ST_PAGES_OUTSIDE, ST_PAGES_FILTERED, ST_ENT_TESTED, ST_ENT_INSIDE, ST_ENT_STREAMED };
-// counters of one cull: [0,256) visible per type, [256,264) statistics, [264] exchange records written
-constexpr int CNT_N_REC = 256 + N_STATS;
-constexpr int COUNTER_WORDS = 256 + N_STATS + 8;
 constexpr int CULL_THREADS = 256;       // 4 blocks/SM at 64 registers; pages per block per round <= one classify thread each
 constexpr int CULL_WARPS = CULL_THREADS / 32;
 constexpr int MAX_CHUNK = CULL_THREADS;
@@ -63,8 +59,6 @@ struct CullParams {
 	uint32_t* xflags[LB200_MAX_RANKS]; // rank r's flag block: [n_buffers][LB200_MAX_RANKS]
 	uint32_t type_base[256];
 };
-// exchange slab = [256 per-type counts][n_pages, n_records, 0, item_cap, 0, 0, 0, 0][page ids: item_cap][rows: item_cap x 8]
-constexpr uint32_t XHEADER_WORDS = 264;
 
 __device__ __forceinline__ int ldg_stream_i32(const int* p) {
 	int r;
@@ -479,7 +473,7 @@ __global__ void __launch_bounds__(CULL_THREADS, 4) cull_pages_kernel(const __gri
 	if (blockIdx.x == 0) {
 		for (int i = tid; i < COUNTER_WORDS; i += CULL_THREADS) next_counters[i] = 0;
 	}
-	// exchange mode: nothing more to do here.  The records were stored without a fence; publish_wait_kernel (culling.cu), which runs
+	// exchange mode: nothing more to do here.  The records were stored without a fence; publish_wait_kernel (culling_exchange.cu), which runs
 	// after this grid has completed, sends the header, fences once at system scope and raises the epoch flags.
 }
 

@@ -71,7 +71,7 @@ struct CullingHost {
 	AllocFn alloc_fn;
 	FreeFn free_fn;
 
-	uint64_t edit_gen = 0; // bumped by every edit: the device-side re-binning tables (culling.cu) are rebuilt when it moved
+	uint64_t edit_gen = 0; // bumped by every edit: the device-side re-binning tables (culling_rebin.cu) are rebuilt when it moved
 
 	void markDirty(uint32_t page) {
 		++edit_gen;

@@ -154,6 +154,7 @@ size_t lb200_radix_sort_state_bytes();
 int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t stream, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
 	void* state, uint32_t* block_hist, uint32_t blocks, bool force_tiled, uint32_t* out_grid);
 int lb200_comm_check(lb200_ctx* ctx); // comm.cu: LB200_ERR_NCCL (and reset) if a peer wait timed out since the last check
+int lb200_comm_allgather_u32(lb200_ctx* ctx, const uint32_t* send, uint32_t* recv, size_t words); // comm.cu, asynchronous on the context stream
 uint32_t lb200_cull_lanes(); // LB200_CULL_LANES, default 2, 1..LB200_MAX_LANES (context.cu)
 
 #define LB200_CUDA(ctx, expr)                                                                        \

@@ -730,7 +730,7 @@ int coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem
 // Stable LSD radix sort of n = min(*count_dev, cap) (key, value) pairs of 64 bits, one cooperative launch on `stream`, n read on the device.
 // The sorted pairs end in buffer 0.  state: lb200_radix_sort_state_bytes() bytes, block_hist: 256 x blocks words; at most `blocks` blocks
 // are launched.  force_tiled: the tiled path at any n.  *out_grid (may be null): the blocks launched.  (Also used by the device re-binning
-// of the culling structure, culling.cu, and by lb200_radix_sort_device.)
+// of the culling structure, culling_rebin.cu, and by lb200_radix_sort_device.)
 size_t lb200_radix_sort_state_bytes() { return sizeof(SortState); }
 
 static int radix_sort_grid_limit(lb200_ctx* ctx, uint32_t* out) {

@@ -1,7 +1,8 @@
-"""The C-ABI library loads without a GPU and exports every symbol include/lumix_b200.h declares."""
+"""The C-ABI library loads without a GPU and exports every symbol include/lumix_b200.h declares, and none of its own besides."""
 import ctypes
 import os
 import re
+import subprocess
 
 import lumixengine_b200 as lb
 from lumixengine_b200 import _lib
@@ -21,6 +22,18 @@ def test_header_symbols_are_exported():
     missing = [s for s in syms if not hasattr(L, s)]
     assert not missing, missing
     assert sorted(_lib.SYMBOLS) == syms
+
+
+def test_exports_are_declared_in_header():
+    """The other direction: the .so exports nothing of its own beyond the header.  Helpers shared between sources have external
+    linkage and stay internal only through -fvisibility=hidden; an exported one would become ABI nobody declared."""
+    out = subprocess.run(["nm", "-D", "--defined-only", _lib.SO_PATH], capture_output=True, text=True, check=True).stdout
+    exported = [line.split()[-1] for line in out.splitlines() if line.strip()]
+    # C symbols lb200_*, C++ functions named lb200_* in the global namespace, anything in the library's namespaces lb / lbcull
+    own = [s for s in exported if re.match(r"lb200_|_Z\d+lb200_|_ZN(K|L)?\d+(lb|lbcull)\d", s)]
+    assert len(own) > 50
+    declared = set(_header_symbols())
+    assert sorted(s for s in own if s not in declared) == []
 
 
 def test_no_cpu_fallback_without_device():

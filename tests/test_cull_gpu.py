@@ -420,6 +420,74 @@ def test_device_rebinning_equals_host_set(ctx, oracle):
     cs.close()
 
 
+def test_const_getters_pull_back_the_device_state(ctx, oracle):
+    """The four const getters of the C API read the host mirror.  Each one, called first after a device re-binning batch (no
+    sync_host), pulls the device state back itself: it answers for the batch, and the mirror it leaves agrees entity by entity."""
+    import ctypes as C
+    from lumixengine_b200 import _lib
+    rng = np.random.default_rng(77)
+    n = 30_000
+    scene = scenes.cull_scene(n, (2000.0, 300.0, 2000.0), seed=17, big_fraction=0.01, type_probs=(0.7, 0.2, 0.1))
+    cs, _ = _both(ctx, oracle, scene)
+    pos, rad = scene["pos"].copy(), scene["radius"].copy()
+
+    def batch(crowd=0):  # every entity moves, some change their radius (and big-ness); the device is ahead of the mirror afterwards
+        nonlocal pos, rad
+        pos = pos + rng.normal(size=pos.shape) * np.array([60.0, 3.0, 60.0])
+        c = rng.choice(n, crowd, replace=False)  # teleported into an empty cell far outside the scene: new pages
+        pos[c] = np.array([6100.0, 10.0, 6100.0]) + rng.random((crowd, 3)) * 40.0
+        changed = rng.random(n) < 0.05
+        rad = np.where(changed, (rng.random(n) * 650).astype(np.float32), rad).astype(np.float32)
+        d_pos, d_rad = ctx.to_device(pos), ctx.to_device(rad)
+        assert cs.set_many_device(d_pos, d_rad, n) > 100
+        ctx.free_device(d_pos); ctx.free_device(d_rad)
+        return np.nonzero(changed)[0]
+
+    def check_page(origin, indices, is_big, spheres, e):
+        key = (pos[e] * np.float32(1 / 300.0)).astype(np.int64)  # trunc toward zero like IVec3(DVec3)
+        assert np.all(key == np.asarray(indices)[None, :]) and np.all((rad[e] > 300.0) == bool(is_big))
+        assert np.array_equal(spheres[:, :3], (pos[e] - np.asarray(origin)).astype(np.float32)) and np.array_equal(spheres[:, 3], rad[e])
+
+    def check_mirror():
+        seen = np.zeros(n, bool)
+        for pg in cs.pages():
+            e = pg["entities"]
+            assert pg["count"] == len(e) <= 200 and not seen[e].any()
+            seen[e] = True
+            check_page(pg["origin"], pg["indices"], pg["is_big"], pg["spheres"], e)
+        assert seen.all()
+        return len(cs.pages())
+
+    changed = batch()
+    radii = [cs.L.lb200_culling_get_radius(cs.h, C.c_int32(int(e))) for e in changed[:50]]
+    assert np.array_equal(np.array(radii, np.float32), rad[changed[:50]])
+    before = check_mirror()
+
+    batch(crowd=6000)
+    count = int(cs.L.lb200_culling_page_count(cs.h))
+    cs.sync_host()  # a no-op unless page_count left the device ahead: the references below do not go through page_count's pull-back
+    assert count > before and count == int(cs.L.lb200_culling_page_count(cs.h)) == check_mirror()
+
+    batch()
+    o, ind = (C.c_double * 3)(), (C.c_int32 * 3)()
+    ty, big, cnt = C.c_uint8(), C.c_uint8(), C.c_uint32()
+    sph = np.empty((_lib.PAGE_SLOTS, 4), np.float32)
+    ent = np.empty(_lib.PAGE_SLOTS, np.int32)
+    ptr = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    rc = cs.L.lb200_culling_get_page(cs.h, C.c_uint32(0), o, ind, C.byref(ty), C.byref(big), C.byref(cnt), ptr(sph), ptr(ent))
+    assert rc == 0 and cnt.value > 0
+    check_page(tuple(o), tuple(ind), big.value, sph[:cnt.value], ent[:cnt.value])
+    check_mirror()
+
+    batch()
+    ids = []
+    while (p := int(cs.L.lb200_culling_page_id(cs.h, C.c_uint32(len(ids))))) >= 0:
+        ids.append(p)
+    assert np.array_equal(np.array(ids, np.int64), cs.page_ids())
+    check_mirror()
+    cs.close()
+
+
 def test_buffers_grow_after_first_use(ctx, oracle):
     """Every buffer that grows on demand is re-allocated after its first use, and the results stay equal to the oracle's: more entities
     than the page arrays and the output ids were sized for, a sparse upload of more pages than the first one staged, and a device
