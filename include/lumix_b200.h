@@ -268,6 +268,9 @@ typedef struct lb200_sk_outputs { /* device pointers, valid until the next creat
 #define LB200_SK_DIRTY 2u /* ModelInstance::dirty */
 LB200_API int lb200_sortkeys_create(lb200_ctx* ctx, uint32_t max_entities, uint32_t max_groups, uint32_t max_keys, uint32_t max_instances, lb200_sortkeys** out);
 LB200_API void lb200_sortkeys_destroy(lb200_sortkeys* sk);
+/* Replaces both tables.  LB200_ERR_INVALID for a mesh sort key >= max_groups or a non-empty LOD range outside [0, mesh_count) of its model.
+ * A model whose meshes [mesh_base, mesh_base + mesh_count) leave the mesh table is stored, but create_keys refuses to launch
+ * (LB200_ERR_INVALID) until set_models is called with tables that fit. */
 LB200_API int lb200_sortkeys_set_models(lb200_sortkeys* sk, const lb200_sk_model* models, uint32_t n_models, const lb200_sk_mesh* meshes, uint32_t n_meshes);
 /* Per-entity state, arrays indexed by entity id; a null pointer leaves that array as it is. */
 LB200_API int lb200_sortkeys_set_instances(lb200_sortkeys* sk, uint32_t n, const uint32_t* model_of, const float* lod, const uint8_t* flags, const uint32_t* pose_frame,
@@ -278,6 +281,13 @@ LB200_API int lb200_sortkeys_set_transforms(lb200_sortkeys* sk, const lb200_tran
 LB200_API int lb200_sortkeys_set_transforms_device(lb200_sortkeys* sk, const lb200_transform* dev_transforms, uint32_t n);
 /* createSortKeys (+ radixSort if `sort`) for the last cull of `cs` on the context stream.  Asynchronous unless `want_counts`. */
 LB200_API int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb200_sk_view* view, int sort, int want_counts, lb200_sk_result* result);
+/* Launch shape of later create_keys calls.  blocks: 0 = the default (LB200_SK_BLOCKS_PER_SM per SM, else 2, and at most one block per 256
+ * renderables the cull can emit), -1 = every block that is co-resident, n > 0 = min(n, co-resident blocks); only 0 caps the grid by the
+ * work.  prefetch_ahead: 0..4 grid strides of L2 prefetch, -1 = the default (LB200_SK_PREFETCH, else 0).  Any other value is
+ * LB200_ERR_INVALID.  get_launch reports the last create_keys launch: blocks, whether the group counters lived in shared memory
+ * (max_sort_key < 8192) and the prefetch distance (all 0 before the first). */
+LB200_API int lb200_sortkeys_set_launch(lb200_sortkeys* sk, int blocks, int prefetch_ahead);
+LB200_API int lb200_sortkeys_get_launch(lb200_sortkeys* sk, uint32_t* grid, int* groups_in_smem, uint32_t* prefetch_ahead);
 LB200_API int lb200_sortkeys_device_outputs(lb200_sortkeys* sk, lb200_sk_outputs* out);
 /* RenderModuleImpl::onModelInstanceMoved (src/renderer/render_module.cpp:1544-1554) for n instances whose new transforms lie in device memory:
  * the transforms go into the entity records, ModelInstance::MOVED is set (createSortKeys then draws the instance as DRAW_MESH, pipeline.cpp

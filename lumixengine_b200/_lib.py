@@ -97,7 +97,7 @@ SYMBOLS = [
     "lb200_comm_get_unique_id", "lb200_comm_init", "lb200_comm_destroy", "lb200_comm_enable_p2p", "lb200_comm_status", "lb200_culling_gather_stride_words", "lb200_culling_allgather", "lb200_culling_cull_gather",
     "lb200_culling_cull_exchange", "lb200_culling_cull_exchange_n", "lb200_culling_exchange_slab_words", "lb200_culling_page_id",
     "lb200_sortkeys_create", "lb200_sortkeys_destroy", "lb200_sortkeys_set_models", "lb200_sortkeys_set_instances", "lb200_sortkeys_set_transforms",
-    "lb200_sortkeys_set_transforms_device", "lb200_sortkeys_create_keys", "lb200_sortkeys_device_outputs",
+    "lb200_sortkeys_set_transforms_device", "lb200_sortkeys_create_keys", "lb200_sortkeys_set_launch", "lb200_sortkeys_get_launch", "lb200_sortkeys_device_outputs",
     "lb200_sortkeys_move_device", "lb200_sortkeys_end_frame", "lb200_sortkeys_prev_transforms", "lb200_radix_sort_device", "lb200_animation_bone_attachments_device",
     "lb200_hierarchy_create", "lb200_hierarchy_destroy", "lb200_hierarchy_depth", "lb200_hierarchy_set_locals", "lb200_hierarchy_set_root_globals", "lb200_hierarchy_set_subset",
     "lb200_hierarchy_propagate", "lb200_hierarchy_get_globals", "lb200_hierarchy_get_spheres", "lb200_hierarchy_refresh_spheres", "lb200_hierarchy_get_relative_matrices", "lb200_hierarchy_set_globals", "lb200_hierarchy_compute_locals", "lb200_hierarchy_get_locals", "lb200_hierarchy_algorithmic_bytes",

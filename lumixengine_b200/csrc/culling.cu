@@ -424,6 +424,9 @@ int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, con
 	return LB200_OK;
 }
 
+// the device re-binning only moves entities the host mirror added, so its entity -> slot table spans every id a cull can emit
+uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs) { return (uint32_t)cs->host.entity_to_slot.size(); }
+
 extern "C" {
 
 int lb200_culling_create(lb200_ctx* ctx, lb200_culling** out) {

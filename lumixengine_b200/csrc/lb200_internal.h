@@ -148,6 +148,8 @@ struct lb200_range {
 };
 // culling.cu: where the last cull left its result (device: ids, counters; host: per-type segment bases and entity counts, 256 each)
 int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, const uint32_t** counters, const uint32_t** type_base, const uint32_t** type_counts);
+// culling.cu: 1 + the largest entity id ever added (0 if none): every id a cull of cs can emit is below it
+uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs);
 // sortkeys.cu: stable LSD radix sort of (u64 key, u64 value) pairs, count read on the device; the result ends in buffer 0.
 // force_tiled: the tiled path at any n (the register path is taken iff !force_tiled && n <= grid * 512 * 16); *out_grid (may be null) = blocks launched
 size_t lb200_radix_sort_state_bytes();

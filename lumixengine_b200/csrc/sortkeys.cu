@@ -32,6 +32,7 @@
 
 #include <algorithm>
 #include <memory>
+#include <stdio.h>
 #include <stdlib.h>
 #include <new>
 
@@ -796,6 +797,8 @@ extern "C" int lb200_radix_sort_device(lb200_ctx* ctx, uint64_t* dev_keys, uint6
 	return LB200_OK;
 }
 
+constexpr uint32_t NO_MODEL = 0xffffffffu;
+
 struct lb200_sortkeys {
 	lb200_ctx* ctx = nullptr;
 	uint32_t max_entities = 0, max_groups = 0;
@@ -818,7 +821,15 @@ struct lb200_sortkeys {
 	DeviceArray<SortState> d_sort_state; DeviceArray<uint32_t> d_block_hist;
 	uint32_t sort_blocks = 0;
 	uint32_t last_groups = 0;
+	uint32_t max_mesh_sort_key = 0; // largest sort key of the mesh table: every view's max_sort_key must reach it
+	uint32_t model_past_table = NO_MODEL; // first model whose meshes leave the mesh table (create_keys refuses to launch), NO_MODEL if none
+	char past_table_text[128] = {};
 	uint32_t keys_grid_limit[2] = {0, 0}; // co-resident blocks of create_keys_kernel: group counters in shared memory / in HBM
+	// lb200_sortkeys_set_launch (blocks 0 = environment switch, else 2 per SM; -1 = all co-resident; prefetch -1 = environment switch) and
+	// what the last create_keys launched
+	int launch_blocks = 0, launch_prefetch = -1;
+	uint32_t last_grid = 0, last_prefetch = 0;
+	int last_in_smem = 0;
 };
 
 namespace {
@@ -888,7 +899,26 @@ int lb200_sortkeys_set_models(lb200_sortkeys* sk, const lb200_sk_model* models, 
 	if (!sk || !models || !meshes || !n_models || !n_meshes) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = sk->ctx;
 	if (n_models > CODE_MODEL_MASK + 1u) { lb200_set_error(ctx, "%u models: the entity record keeps 24 bits of model index", n_models); return LB200_ERR_INVALID; }
-	for (uint32_t i = 0; i < n_meshes; ++i) if (meshes[i].sort_key >= sk->max_groups) { lb200_set_error(ctx, "mesh %u: sort key %u >= max_groups %u", i, meshes[i].sort_key, sk->max_groups); return LB200_ERR_INVALID; }
+	uint32_t max_key = 0;
+	for (uint32_t i = 0; i < n_meshes; ++i) {
+		if (meshes[i].sort_key >= sk->max_groups) { lb200_set_error(ctx, "mesh %u: sort key %u >= max_groups %u", i, meshes[i].sort_key, sk->max_groups); return LB200_ERR_INVALID; }
+		max_key = std::max(max_key, meshes[i].sort_key);
+	}
+	// the kernel reads meshes[mesh_base + j] for every j of the drawn LOD ranges without a bounds check: a LOD range has to stay inside its
+	// model's meshes (refused here), and the model's meshes inside the mesh table (create_keys refuses to launch until they do, so that a
+	// table can be set ahead of the meshes it will be paired with)
+	uint32_t model_past_table = NO_MODEL;
+	for (uint32_t m = 0; m < n_models; ++m) {
+		const lb200_sk_model& md = models[m];
+		if (model_past_table == NO_MODEL && (md.mesh_base > n_meshes || md.mesh_count > n_meshes - md.mesh_base)) model_past_table = m;
+		for (int l = 0; l < 5; ++l) {
+			if (md.lod_from[l] > md.lod_to[l]) continue; // empty LOD: nothing drawn
+			if (md.lod_from[l] < 0 || (uint32_t)md.lod_to[l] >= md.mesh_count) {
+				lb200_set_error(ctx, "model %u: LOD %d meshes [%d, %d] leave the model's %u meshes", m, l, md.lod_from[l], md.lod_to[l], md.mesh_count);
+				return LB200_ERR_INVALID;
+			}
+		}
+	}
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	sk->d_models.reset(); sk->d_meshes.reset(); // both go before either is allocated again
 	DeviceArray<lb200_sk_model> d_models; DeviceArray<lb200_sk_mesh> d_meshes;
@@ -907,6 +937,13 @@ int lb200_sortkeys_set_models(lb200_sortkeys* sk, const lb200_sk_model* models, 
 	cudaStreamSynchronize(ctx->stream);
 	delete[] layer;
 	LB200_CUDA(ctx, e);
+	sk->max_mesh_sort_key = max_key;
+	sk->model_past_table = model_past_table;
+	if (model_past_table != NO_MODEL) {
+		const lb200_sk_model& md = models[model_past_table];
+		snprintf(sk->past_table_text, sizeof(sk->past_table_text), "model %u: meshes [%u, %u + %u) leave the %u-mesh table", model_past_table, md.mesh_base, md.mesh_base,
+			md.mesh_count, n_meshes);
+	}
 	return LB200_OK;
 }
 
@@ -967,9 +1004,14 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	lb200_range range("create keys"); // pipeline.cpp:3818
 	if (!sk->have_transforms || !sk->d_models) { lb200_set_error(ctx, "create_keys needs set_models and set_transforms first"); return LB200_ERR_STATE; }
 	if (view->max_sort_key >= sk->max_groups) { lb200_set_error(ctx, "view.max_sort_key %u >= max_groups %u", view->max_sort_key, sk->max_groups); return LB200_ERR_INVALID; }
+	if (sk->model_past_table != NO_MODEL) { lb200_set_error(ctx, "create_keys: %s", sk->past_table_text); return LB200_ERR_INVALID; }
+	if (view->max_sort_key < sk->max_mesh_sort_key) { lb200_set_error(ctx, "view.max_sort_key %u < sort key %u of the mesh table", view->max_sort_key, sk->max_mesh_sort_key); return LB200_ERR_INVALID; }
 	const uint32_t *visible = nullptr, *cull_counters = nullptr, *type_base = nullptr, *type_counts = nullptr;
 	int rc = lb200_culling_internal_last(cs, &visible, &cull_counters, &type_base, &type_counts);
 	if (rc) return rc;
+	// the kernel indexes the entity records, the decal arrays and the stash by the culled ids without a bounds check
+	const uint32_t entity_range = lb200_culling_internal_entity_range(cs);
+	if (entity_range > sk->max_entities) { lb200_set_error(ctx, "the culling system holds entity ids up to %u, max_entities is %u", entity_range - 1, sk->max_entities); return LB200_ERR_INVALID; }
 	cudaStream_t s = ctx->stream;
 	uint32_t n_groups = view->max_sort_key + 1;
 	sk->last_groups = n_groups;
@@ -981,7 +1023,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	for (int t = 0; t < 4; ++t) EP.type_base[t] = type_base[t];
 	EP.cap_keys = sk->cap_keys; EP.cap_recs = sk->cap_recs; EP.cap_pose = sk->max_entities; EP.cap_dirty = sk->max_entities;
 	static const uint32_t prefetch_ahead = [] { const char* e = getenv("LB200_SK_PREFETCH"); const int v = e ? atoi(e) : 0; return (uint32_t)std::max(0, std::min(v, 4)); }(); // off: on H100 the prefetch slows the pass (DESIGN.md 4.5)
-	EP.prefetch_ahead = prefetch_ahead;
+	EP.prefetch_ahead = sk->launch_prefetch >= 0 ? (uint32_t)sk->launch_prefetch : prefetch_ahead;
 	const bool in_smem = n_groups <= SK_SMEM_GROUPS;
 	size_t smem = in_smem ? sizeof(uint32_t) * n_groups : 0;
 	uint32_t& limit = sk->keys_grid_limit[in_smem ? 0 : 1];
@@ -992,11 +1034,14 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	const uint32_t work = type_counts[RT_MESH] + type_counts[RT_DECAL] + type_counts[RT_CURVE_DECAL]; // upper bound of visible renderables
 	static const uint32_t blocks_per_sm = [] { const char* e = getenv("LB200_SK_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 2; return (uint32_t)std::max(0, v); }(); // fewer resident blocks than fit (0 = all): 2 is fastest on H100
 	uint32_t grid = std::max(1u, std::min(blocks_per_sm ? std::min(limit, blocks_per_sm * (uint32_t)ctx->sm_count) : limit, (work + SK_THREADS - 1) / SK_THREADS));
+	if (sk->launch_blocks < 0) grid = limit; // lb200_sortkeys_set_launch: not capped by the work, so that threads with nothing to do still take part
+	else if (sk->launch_blocks > 0) grid = std::min((uint32_t)sk->launch_blocks, limit);
 	EmitArgs EA = {sk->d_ent, sk->d_decal_sort_key, sk->d_decal_layer, sk->d_models, sk->d_meshes, sk->d_keys[0], sk->d_values[0], sk->d_counts,
 		sk->d_group_count, sk->d_group_offset, sk->d_group_cursor, sk->d_group_layer, sk->d_group_renderables, sk->d_instance_data, sk->d_pose_list, sk->d_dirty_list, sk->d_stash, sk->d_stash4, sk->max_entities, sk->d_bar};
 	void* args[] = {&EP, &visible, &cull_counters, &EA, &n_groups};
 	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)create_keys_kernel, dim3(grid), dim3(SK_THREADS), args, smem, s));
 	LB200_CHECK_LAUNCH(ctx);
+	sk->last_grid = grid; sk->last_in_smem = in_smem ? 1 : 0; sk->last_prefetch = EP.prefetch_ahead;
 	if (sort) {
 		lb200_range r2("radixSort"); // pipeline.cpp:4101
 		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->d_sort_state, sk->d_block_hist, sk->sort_blocks, false, nullptr);
@@ -1010,6 +1055,23 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 		result->n_dirty = sk->h_counts[CNT_DIRTY]; result->n_groups = n_groups;
 		if (result->n_keys > sk->cap_keys || sk->h_counts[CNT_RECS] > sk->cap_recs) { lb200_set_error(ctx, "create_keys: %u keys / %u instances exceed the capacities %u / %u", result->n_keys, sk->h_counts[CNT_RECS], sk->cap_keys, sk->cap_recs); return LB200_ERR_CAPACITY; }
 	}
+	return LB200_OK;
+}
+
+int lb200_sortkeys_set_launch(lb200_sortkeys* sk, int blocks, int prefetch_ahead) {
+	if (!sk) return LB200_ERR_INVALID;
+	if (blocks < -1) { lb200_set_error(sk->ctx, "set_launch: blocks %d is not -1, 0 or a block count", blocks); return LB200_ERR_INVALID; }
+	if (prefetch_ahead < -1 || prefetch_ahead > 4) { lb200_set_error(sk->ctx, "set_launch: prefetch_ahead %d is not -1 or 0..4", prefetch_ahead); return LB200_ERR_INVALID; }
+	sk->launch_blocks = blocks;
+	sk->launch_prefetch = prefetch_ahead;
+	return LB200_OK;
+}
+
+int lb200_sortkeys_get_launch(lb200_sortkeys* sk, uint32_t* grid, int* groups_in_smem, uint32_t* prefetch_ahead) {
+	if (!sk) return LB200_ERR_INVALID;
+	if (grid) *grid = sk->last_grid;
+	if (groups_in_smem) *groups_in_smem = sk->last_in_smem;
+	if (prefetch_ahead) *prefetch_ahead = sk->last_prefetch;
 	return LB200_OK;
 }
 

@@ -104,6 +104,17 @@ class SortKeys:
         self._err(self.L.lb200_sortkeys_create_keys(self.h, culling.h, ptr(view), C.c_int(1 if sort else 0), C.c_int(1 if want_counts else 0), C.byref(res)))
         return res if want_counts else None
 
+    def setLaunch(self, blocks=0, prefetch_ahead=-1):
+        """Launch shape of later createSortKeys calls: blocks 0 = the default (environment switch, else 2 per SM, at most one per 256
+        renderables), -1 = all co-resident, n > 0 = min(n, co-resident); prefetch_ahead 0..4 grid strides, -1 = the default."""
+        self._err(self.L.lb200_sortkeys_set_launch(self.h, C.c_int(blocks), C.c_int(prefetch_ahead)))
+
+    def lastLaunch(self):
+        """(grid, group counters in shared memory, prefetch distance) of the last createSortKeys; zeros before the first."""
+        g, s, p = C.c_uint32(), C.c_int(), C.c_uint32()
+        self._err(self.L.lb200_sortkeys_get_launch(self.h, C.byref(g), C.byref(s), C.byref(p)))
+        return int(g.value), bool(s.value), int(p.value)
+
     def moveDevice(self, dev_entities, dev_transforms, n, dev_bounding_radius=None, dev_out_pos3=None, dev_out_radius=None):
         """RenderModule::onModelInstanceMoved for n instances whose transforms lie in device memory (pointers as ints): records updated, MOVED set;
         with bounding radii also the spheres for CullingSystem.set_many_device."""
