@@ -214,6 +214,17 @@ LB200_API uint32_t lb200_culling_last_rebin_changers(const lb200_culling* cs);
  * the two event records, 2 = one empty kernel of the cull's grid (the fixed costs the first number contains). */
 LB200_API int lb200_culling_time_lone_cull(lb200_culling* cs, const lb200_shifted_frustum* frustum, uint8_t type, uint32_t iters, int mode, float* out_ms);
 LB200_API uint64_t lb200_culling_last_algorithmic_bytes(const lb200_culling* cs);
+/* Launch shape of later culls of this object, every entry point (cull, begin / end, cull_device[_n], cull_gather, cull_exchange[_n]).
+ * blocks: 0 = the default rule (every co-resident block, LB200_CULL_BLOCKS_PER_SM per SM on the internal lanes, at most one block per
+ * chunk of pages), -1 = every block that is co-resident when the cull has the device to itself (on the lanes too), 1..LB200_CULL_MAX_BLOCKS
+ * = exactly that many, whatever fits and whatever the work (the cap keeps the kernel's 32-bit page index from overflowing).  chunk: pages per block per round, 0 = the default (ceil(pages / blocks) within
+ * 32..256), 1..256 = exactly that many.  plane_masking: -1 = automatic (on unless some radius is negative or NaN), 0 = off.  Any other
+ * value is LB200_ERR_INVALID.  The visible sets, statistics and mask rows do not depend on the shape.  get_launch reports the last cull:
+ * blocks, chunk, rounds = ceil(pages / (blocks x chunk)), whether it was launched with programmatic dependent launch (no upload since the
+ * cull before it) and whether plane masking was on (all 0 before the first cull; for a batch, its last cull). */
+#define LB200_CULL_MAX_BLOCKS (1 << 20)
+LB200_API int lb200_culling_set_launch(lb200_culling* cs, int blocks, int chunk, int plane_masking);
+LB200_API int lb200_culling_get_launch(lb200_culling* cs, uint32_t* blocks, uint32_t* chunk, uint32_t* rounds, int* pdl, int* plane_masking);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Sort keys — the consumer of the visible list (SURVEY.md 8f N1): PipelineImpl::createSortKeys (src/renderer/pipeline.cpp:3789-4018:

@@ -284,7 +284,7 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 		if (xchg->pub_epoch) for (int r = 0; r < ctx->n_ranks; ++r) P.xprev[r] = peerSlab(ctx, xchg->pub_epoch, r);
 	}
 	static const bool no_mask = getenv("LB200_NO_PLANE_MASKING") != nullptr;
-	P.plane_masking = (h.n_bad_radius == 0 && !no_mask) ? 1u : 0u;
+	P.plane_masking = (h.n_bad_radius == 0 && !no_mask && cs->launch_plane_masking != 0) ? 1u : 0u;
 	// Programmatic stream serialization: the kernel's prologue (up to cudaGridDependencySynchronize: descriptor reads, classification, the
 	// sphere tests of round 0, whose results sit in shared memory) only READS scene data.  Those arrays are written by flushPages alone, so
 	// unless something was uploaded since the last cull the prologue may overlap the tail of whatever kernel precedes it on the stream —
@@ -293,11 +293,15 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 	static const bool no_pdl = getenv("LB200_NO_PDL") != nullptr;
 	const bool pdl = !no_pdl && !cs->uploaded_since_last_cull;
 	cs->uploaded_since_last_cull = false;
-	// chunk = pages per block per round: spread the pages over every resident block, at most one classify thread per page
+	// chunk = pages per block per round: spread the pages over every resident block, at most one classify thread per page.
+	// lb200_culling_set_launch may force either: the kernel is correct for any grid (no co-residency, no grid barrier) and any chunk in
+	// 1..MAX_CHUNK, so a forced block count is capped by neither residency nor the work; the floor of 32 pages is a speed choice.
 	const uint32_t resident = (uint32_t)(stream || xchg ? cs->grid_lanes : cs->grid);
-	uint32_t chunk = (n_pages + resident - 1) / resident;
+	const uint32_t spread = cs->launch_blocks > 0 ? (uint32_t)cs->launch_blocks : cs->launch_blocks < 0 ? (uint32_t)cs->grid : resident;
+	uint32_t chunk = (n_pages + spread - 1) / spread;
 	chunk = std::max(32u, std::min((uint32_t)MAX_CHUNK, chunk));
-	const uint32_t blocks = std::max(1u, std::min(resident, (n_pages + chunk - 1) / chunk));
+	if (cs->launch_chunk) chunk = (uint32_t)cs->launch_chunk;
+	const uint32_t blocks = cs->launch_blocks ? spread : std::max(1u, std::min(resident, (n_pages + chunk - 1) / chunk));
 	P.chunk = chunk;
 	cudaLaunchAttribute attr;
 	const cudaLaunchConfig_t cfg = launchConfig(blocks, CULL_THREADS, stream ? stream : ctx->stream, &attr, pdl);
@@ -309,6 +313,8 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 	cs->lane_parity[lane] ^= 1u;
 	if (!xchg) ++cs->seq;
 	cs->last_pages = n_pages;
+	cs->last_blocks = blocks; cs->last_chunk = chunk; cs->last_rounds = (uint32_t)((n_pages + (uint64_t)blocks * chunk - 1) / ((uint64_t)blocks * chunk));
+	cs->last_pdl = pdl ? 1 : 0; cs->last_plane_masking = (int)P.plane_masking;
 	return LB200_OK;
 }
 
@@ -745,5 +751,26 @@ int lb200_culling_time_lone_cull(lb200_culling* cs, const lb200_shifted_frustum*
 }
 
 uint64_t lb200_culling_last_algorithmic_bytes(const lb200_culling* cs) { return cs && cs->has_last ? cs->last_bytes : 0; }
+
+int lb200_culling_set_launch(lb200_culling* cs, int blocks, int chunk, int plane_masking) {
+	if (!cs) return LB200_ERR_INVALID;
+	if (blocks < -1 || blocks > LB200_CULL_MAX_BLOCKS) { lb200_set_error(cs->ctx, "set_launch: blocks %d is not -1, 0 or a block count up to %d", blocks, LB200_CULL_MAX_BLOCKS); return LB200_ERR_INVALID; }
+	if (chunk < 0 || chunk > MAX_CHUNK) { lb200_set_error(cs->ctx, "set_launch: chunk %d is not 0 or 1..%d", chunk, MAX_CHUNK); return LB200_ERR_INVALID; }
+	if (plane_masking != -1 && plane_masking != 0) { lb200_set_error(cs->ctx, "set_launch: plane_masking %d is not -1 or 0", plane_masking); return LB200_ERR_INVALID; }
+	cs->launch_blocks = blocks;
+	cs->launch_chunk = chunk;
+	cs->launch_plane_masking = plane_masking;
+	return LB200_OK;
+}
+
+int lb200_culling_get_launch(lb200_culling* cs, uint32_t* blocks, uint32_t* chunk, uint32_t* rounds, int* pdl, int* plane_masking) {
+	if (!cs) return LB200_ERR_INVALID;
+	if (blocks) *blocks = cs->last_blocks;
+	if (chunk) *chunk = cs->last_chunk;
+	if (rounds) *rounds = cs->last_rounds;
+	if (pdl) *pdl = cs->last_pdl;
+	if (plane_masking) *plane_masking = cs->last_plane_masking;
+	return LB200_OK;
+}
 
 } // extern "C"

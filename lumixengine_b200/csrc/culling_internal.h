@@ -84,6 +84,10 @@ struct lb200_culling {
 	uint32_t* h_counters_dev = nullptr; // the same memory as the device addresses it (null: no direct host writes)
 	int grid = 0;       // resident blocks of a cull that has the device to itself
 	int grid_lanes = 0; // resident blocks of a cull issued by cull_device_n (runs next to its neighbours)
+	// lb200_culling_set_launch (0, 0, -1: the default rule) and what the last cull launched (lb200_culling_get_launch)
+	int launch_blocks = 0, launch_chunk = 0, launch_plane_masking = -1;
+	uint32_t last_blocks = 0, last_chunk = 0, last_rounds = 0;
+	int last_pdl = 0, last_plane_masking = 0;
 	// staging for sparse dirty uploads, the same size on both sides, allocated and released together
 	PinnedArray<uint8_t> h_stage;
 	DeviceArray<uint8_t> d_stage;

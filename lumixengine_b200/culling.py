@@ -269,6 +269,17 @@ class CullingSystem:
     def last_algorithmic_bytes(self):
         return int(self.L.lb200_culling_last_algorithmic_bytes(self.h))
 
+    def setLaunch(self, blocks=0, chunk=0, plane_masking=-1):
+        """Launch shape of later culls on this object (lb200_culling_set_launch): blocks 0 = the default rule, -1 = every co-resident
+        block, n > 0 = exactly n; chunk 0 = the default, 1..256 pages per block per round; plane_masking -1 = automatic, 0 = off."""
+        self._err(self.L.lb200_culling_set_launch(self.h, C.c_int(blocks), C.c_int(chunk), C.c_int(plane_masking)))
+
+    def lastLaunch(self):
+        """dict(blocks, chunk, rounds, pdl, plane_masking) of the last cull (the last of a batch); zeros before the first."""
+        b, c, r, p, m = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_int(), C.c_int()
+        self._err(self.L.lb200_culling_get_launch(self.h, C.byref(b), C.byref(c), C.byref(r), C.byref(p), C.byref(m)))
+        return dict(blocks=int(b.value), chunk=int(c.value), rounds=int(r.value), pdl=bool(p.value), plane_masking=bool(m.value))
+
     def allgather(self, slab_ids, n_ranks):
         """Exchange of the cull just issued: returns (device pointer of the gathered slabs, counts[n_ranks, 256])."""
         counts = np.zeros(n_ranks * 256, np.uint32)
