@@ -22,6 +22,14 @@ void lb200_set_error(lb200_ctx* ctx, const char* fmt, ...) {
 	va_end(args);
 }
 
+int lb200_coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out) {
+	int per_sm = 0;
+	LB200_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+	if (per_sm < 1) { lb200_set_error(ctx, "cooperative kernel does not fit on an SM (%zu B of shared memory)", smem); return LB200_ERR_CUDA; }
+	*out = (uint32_t)per_sm * (uint32_t)ctx->sm_count;
+	return LB200_OK;
+}
+
 extern "C" {
 
 int lb200_device_count(void) {

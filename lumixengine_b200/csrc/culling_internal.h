@@ -109,7 +109,7 @@ struct lb200_culling {
 	DeviceArray<uint32_t> d_page_dirty, d_dirty_pages;
 	DeviceArray<unsigned long long> d_hash_keys; DeviceArray<uint32_t> d_hash_vals; // packed cell key -> open page of its chain
 	DeviceArray<uint32_t> d_rebin_counters; PinnedArray<uint32_t> h_rebin_counters; // RB_* (culling_rebin.cu); pinned mirror
-	DeviceArray<uint8_t> d_rb_sort_state; DeviceArray<uint32_t> d_rb_block_hist; uint32_t rb_sort_blocks = 0;
+	RadixSortScratch rb_radix_scratch; // the changer sort, with d_rb_keys[1] / d_rb_vals[1] as its alternate buffers
 	// per changer slot
 	DeviceArray<uint32_t> d_changers;       // mover indices that change cell / chain
 	DeviceArray<uint4> d_rb_plans;          // one RunPlan per changer slot (used at the first index of every run)

@@ -249,15 +249,13 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	if (cs->replicas != 1) { lb200_set_error(ctx, "device re-binning works on the live page arrays: set_replicas(1)"); return LB200_ERR_STATE; }
 	int rc = flushPages(cs);
 	if (rc) return rc;
-	if (!cs->d_rebin_counters || !cs->h_rebin_counters || !cs->d_rb_sort_state || !cs->d_rb_block_hist) {
-		cs->rb_sort_blocks = (uint32_t)ctx->sm_count * 2;
-		DeviceArray<uint32_t> d_counters; PinnedArray<uint32_t> h_counters; DeviceArray<uint8_t> sort_state; DeviceArray<uint32_t> block_hist;
+	if (!cs->d_rebin_counters || !cs->h_rebin_counters || !cs->rb_radix_scratch.state) {
+		DeviceArray<uint32_t> d_counters; PinnedArray<uint32_t> h_counters; RadixSortScratch sort;
 		LB200_CUDA(ctx, d_counters.alloc(RB_WORDS));
 		LB200_CUDA(ctx, h_counters.alloc(RB_WORDS));
-		LB200_CUDA(ctx, sort_state.alloc(lb200_radix_sort_state_bytes()));
-		LB200_CUDA(ctx, block_hist.alloc(256 * (size_t)cs->rb_sort_blocks));
-		cs->d_rebin_counters = std::move(d_counters); cs->h_rebin_counters = std::move(h_counters);
-		cs->d_rb_sort_state = std::move(sort_state); cs->d_rb_block_hist = std::move(block_hist);
+		rc = lb200_radix_sort_alloc_scratch(ctx, (uint32_t)ctx->sm_count * 2, sort);
+		if (rc) return rc;
+		cs->d_rebin_counters = std::move(d_counters); cs->h_rebin_counters = std::move(h_counters); cs->rb_radix_scratch = std::move(sort);
 	}
 	if (!cs->d_page_cell) { // the per-page side arrays: none yet, or released by a discarding resizePages, which also reset rebin_built_gen
 		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -427,8 +425,8 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 		rebin_compact_kernel<<<grid, 256, 0, s>>>(cs->d_dirty_pages, C, cs->d_desc, cs->d_page_cell, cs->d_spheres, cs->d_entities, cs->d_entity_to_slot, cs->d_page_dirty,
 			cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, hash_cap);
 		LB200_CHECK_LAUNCH(ctx);
-		rc = lb200_radix_sort_pairs(ctx, s, cs->d_rb_keys[0], cs->d_rb_keys[1], cs->d_rb_vals[0], cs->d_rb_vals[1], C + RB_N_CHANGERS, changers_cap, cs->d_rb_sort_state,
-			cs->d_rb_block_hist, cs->rb_sort_blocks, false, nullptr);
+		rc = lb200_radix_sort_pairs(ctx, s, cs->d_rb_keys[0], cs->d_rb_keys[1], cs->d_rb_vals[0], cs->d_rb_vals[1], C + RB_N_CHANGERS, changers_cap, cs->rb_radix_scratch,
+			0, false, nullptr);
 		if (rc) return rc;
 		LB200_CUDA(ctx, cudaMemsetAsync(C + RB_WORDS - 1, 0, sizeof(uint32_t), s)); // the new-page cursor of this batch
 		rebin_plan_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 8u, (n_changers + 127) / 128)), 128, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, dev_pos3, cs->d_desc,

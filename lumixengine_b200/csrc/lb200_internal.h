@@ -91,6 +91,15 @@ private:
 using Event = lb200_handle<cudaEvent_t, cudaEventDestroy>;
 using Stream = lb200_handle<cudaStream_t, cudaStreamDestroy>;
 
+// Scratch of one caller of the device radix sort (radix_sort.cu): the sort's state, a type private to radix_sort.cu, and one 256-digit
+// histogram row per block a sort with it may launch.  lb200_radix_sort_alloc_scratch sizes it; the alternate key / value buffers stay
+// with the caller.
+struct RadixSortScratch {
+	DeviceArray<uint8_t> state;
+	DeviceArray<uint32_t> block_hist; // [blocks()][256]
+	uint32_t blocks() const { return (uint32_t)(block_hist.size() / 256); }
+};
+
 #define LB200_MAX_RANKS 8
 #define LB200_MAX_LANES 8  // concurrent culls (streams / output lanes); exchange buffers = 3 x lanes
 
@@ -99,11 +108,13 @@ struct lb200_ctx {
 	Stream stream;
 	Stream copy_stream;
 	int sm_count = 0;
+	uint32_t radix_sort_grid = 0; // blocks of radix_sort_kernel that can be co-resident (radix_sort.cu), 0 until the first scratch is sized
 	std::atomic<uint64_t> launches{0};
 	char error[512] = {0};
-	// scratch of lb200_radix_sort_device (sortkeys.cu); its size in bytes follows the pair capacity sort_scratch_cap
-	DeviceArray<uint8_t> sort_scratch;
-	uint32_t sort_scratch_cap = 0;
+	// scratch of lb200_radix_sort_device (radix_sort.cu): the alternate key / value buffers, grown to the largest cap asked for (their size is
+	// the capacity), and the sort's own scratch for every co-resident block
+	DeviceArray<uint64_t> radix_keys1, radix_values1;
+	RadixSortScratch radix_scratch;
 	// NCCL (dlopen) state, see comm.cu
 	void* nccl_lib = nullptr;
 	void* nccl_comm = nullptr;
@@ -150,11 +161,15 @@ struct lb200_range {
 int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, const uint32_t** counters, const uint32_t** type_base, const uint32_t** type_counts);
 // culling.cu: 1 + the largest entity id ever added (0 if none): every id a cull of cs can emit is below it
 uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs);
-// sortkeys.cu: stable LSD radix sort of (u64 key, u64 value) pairs, count read on the device; the result ends in buffer 0.
+// context.cu: *out = blocks of a cooperative kernel that can be co-resident on the context's device (threads per block, dynamic smem)
+int lb200_coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out);
+// radix_sort.cu: scratch for sorts of up to min(blocks, co-resident blocks) blocks; on failure `out` is left as it was
+int lb200_radix_sort_alloc_scratch(lb200_ctx* ctx, uint32_t blocks, RadixSortScratch& out);
+// radix_sort.cu: stable LSD radix sort of n = min(*count_dev, cap) (u64 key, u64 value) pairs, one cooperative launch on `stream`, n read on
+// the device; the result ends in buffer 0.  Launches max(1, min(scratch.blocks(), max_blocks unless 0, ceil(cap / 2048))) blocks.
 // force_tiled: the tiled path at any n (the register path is taken iff !force_tiled && n <= grid * 512 * 16); *out_grid (may be null) = blocks launched
-size_t lb200_radix_sort_state_bytes();
 int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t stream, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
-	void* state, uint32_t* block_hist, uint32_t blocks, bool force_tiled, uint32_t* out_grid);
+	const RadixSortScratch& scratch, uint32_t max_blocks, bool force_tiled, uint32_t* out_grid);
 int lb200_comm_check(lb200_ctx* ctx); // comm.cu: LB200_ERR_NCCL (and reset) if a peer wait timed out since the last check
 int lb200_comm_allgather_u32(lb200_ctx* ctx, const uint32_t* send, uint32_t* recv, size_t words); // comm.cu, asynchronous on the context stream
 uint32_t lb200_cull_lanes(); // LB200_CULL_LANES, default 2, 1..LB200_MAX_LANES (context.cu)

@@ -1,6 +1,6 @@
 // Consumer of the visible list on the device (SURVEY.md 8f N1): PipelineImpl::createSortKeys (src/renderer/pipeline.cpp:3789-4018) —
 // LOD selection with its smoothing state, sort keys / sort values (:53-143), auto-instancing groups + their instance data (:452-523,
-// :3958-4016) — and PipelineImpl::radixSort (:4020-4144).  The ids the cull kernel compacted never leave HBM: this stage reads them
+// :3958-4016) — followed by PipelineImpl::radixSort (:4020-4144, radix_sort.cu).  The ids the cull kernel compacted never leave HBM: this stage reads them
 // where they lie (lb200_culling's per-type segments + counters) and leaves sorted keys / values and per-group instance data in HBM; the
 // host reads back a handful of counters.
 //
@@ -20,13 +20,10 @@
 //             block 0 also writes group_offset and one key/value per non-empty group (:3958-3969).
 //     pass 2  the stashed decisions are replayed: keys / values (:53-143) at the claimed slots, pose / dirty lists, and for every
 //             auto-instanced mesh the 48 bytes of instance data (:3990-4008) straight at group_offset + the block's slice + rank.
-//   radix_sort_kernel  LSD, 8 bits per pass over the 64-bit keys, stable, hand-written, ONE cooperative launch for all passes: only bits that
-//             differ between keys are sorted on (OR of all keys / of all complements; the reference skips the all-in-bin-0 case, :4120);
-//             per pass block histograms -> grid barrier -> every block sums the histograms of the blocks before it -> stable scatter
-//             (warp match + per-warp digit counters) -> grid barrier.  No library sort.
 // The reference runs createSortKeys on every job worker with one AutoInstancer per worker; this is the one-instancer form (instancer
 // index 0 in the group values), every mesh's instances in one group.  Order inside a group and among equal keys is unspecified in the
 // reference too (it depends on the workers' race for result pages).
+#include "grid_barrier.cuh"
 #include "lb200_internal.h"
 #include "lb200_math.cuh"
 
@@ -60,28 +57,6 @@ struct alignas(64) SkEntity {
 	uint32_t pose_frame;  // Pose::frame (0xffffffff = never)
 };
 static_assert(sizeof(SkEntity) == 64, "one burst per entity");
-
-// ---- grid-wide barrier of a cooperative launch (every block of the grid is resident) ----
-// One word that only counts up (zeroed before the launch): barrier number k of the launch is complete when it reads k * gridDim.  Per block:
-// one release-add by thread 0 after the block barrier, then acquire-polls — no generation word, no reset by a last arriver.
-struct GridBar { uint32_t count, pad; };
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
-	uint32_t v;
-	asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-	return v;
-}
-__device__ __forceinline__ void grid_barrier(GridBar* b, uint32_t& passed /* barriers this block has been through; starts at 0 */) {
-	__syncthreads();
-	++passed;
-	if (threadIdx.x == 0) {
-		__threadfence(); // the block's writes (ordered before this by the block barrier) before the arrival
-		atomicAdd(&b->count, 1u);
-		const uint32_t target = passed * gridDim.x;
-		while (ld_acquire_gpu(&b->count) < target) {}
-		__threadfence(); // gpu-scope fence: also drops this SM's L1 lines, the block's plain loads behind the barrier see the other blocks' writes
-	}
-	__syncthreads();
-}
 
 struct EmitParams {
 	lb200_sk_view view;
@@ -479,323 +454,7 @@ __global__ void __launch_bounds__(256) ent_end_frame_kernel(SkEntity* ent, const
 }
 __global__ void reset_word_kernel(uint32_t* w) { *w = 0; }
 
-// ---------------------------------------------------------------- radix sort ----------------------------------------------------------------
-constexpr int RS_THREADS = 512;
-constexpr int RS_WARPS = RS_THREADS / 32;
-constexpr int RS_ITEMS = 4;                         // keys per thread and tile
-constexpr int RS_TILE = RS_THREADS * RS_ITEMS;      // 2048 keys
-constexpr int RS_PASSES = 8;
-struct SortState { // zero-initialised before every launch
-	GridBar bar; uint32_t pad[2];
-	unsigned long long key_or, key_or_not; // OR of all keys, OR of all complements
-	uint32_t digit_total[RS_PASSES][256];    // per digit window: keys of every digit, summed by the blocks with one atomic each
-};
-
-constexpr int RS_REG_ITEMS = 16;                    // keys a thread can keep in registers over all passes
-
-// Where this block's keys of digit d start: all keys of smaller digits + the keys of digit d in the blocks before this one.
-// In: block_hist[b][d] of every block and digit_total[d] = their column sums (behind a grid barrier).  Out: s_hist[d].  All RS_THREADS threads.
-// A block in the first half of the grid sums the rows before it, one in the second half subtracts the rows from itself on from the total:
-// nobody reads more than half of the rows.
-__device__ __forceinline__ void digit_starts(const uint32_t* block_hist, const uint32_t* digit_total, uint32_t* s_hist, uint32_t (*s_part)[256], uint32_t* s_wsum) {
-	const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-	const uint32_t d = tid & 255u, part = tid >> 8;
-	const bool front = 2u * blockIdx.x <= gridDim.x;
-	const uint32_t row_begin = front ? 0u : blockIdx.x, row_end = front ? blockIdx.x : gridDim.x;
-	uint32_t sum = 0;
-	// 8 rows in flight per thread: the rows come from L2 and a row-at-a-time loop would pay one L2 round trip per row
-	for (uint32_t b0 = row_begin + part; b0 < row_end; b0 += 8 * (RS_THREADS / 256)) {
-		uint32_t c[8];
-#pragma unroll
-		for (int u = 0; u < 8; ++u) {
-			const uint32_t b = b0 + u * (RS_THREADS / 256);
-			c[u] = b < row_end ? __ldcg(block_hist + b * 256 + d) : 0u;
-		}
-#pragma unroll
-		for (int u = 0; u < 8; ++u) sum += c[u];
-	}
-	s_part[part][d] = sum;
-	__syncthreads();
-	uint32_t x = 0, mine = 0, before = 0;
-	if (tid < 256) { // exclusive scan of the 256 digit totals by the first 8 warps
-		mine = __ldcg(digit_total + tid);
-		const uint32_t rows = s_part[0][tid] + s_part[1][tid];
-		before = front ? rows : mine - rows;
-		x = mine;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= (uint32_t)o) x += y; }
-		if (lane == 31) s_wsum[warp] = x;
-	}
-	__syncthreads();
-	if (tid < 256) {
-		uint32_t start = x - mine;
-		for (uint32_t w = 0; w < warp; ++w) start += s_wsum[w];
-		s_hist[tid] = start + before;
-	}
-	__syncthreads();
-}
-
-// All passes in one cooperative launch, stable: the key order is "block, then position inside the block's contiguous run".
-//   n <= gridDim * RS_THREADS * RS_REG_ITEMS (a frame's worth of draw keys): every block owns ONE run of `items` keys per thread that stays in
-//   registers from the pass's ranking to its scatter — a pass reads every pair once and writes it once;
-//   larger n: tiles of RS_TILE keys, dealt to the blocks in contiguous runs (block b: tiles [b*T/G, (b+1)*T/G)), counted, then re-read and scattered.
-__global__ void __launch_bounds__(RS_THREADS, 1) radix_sort_kernel(uint64_t* kbuf0, uint64_t* kbuf1, uint64_t* vbuf0, uint64_t* vbuf1, const uint32_t* __restrict__ counts, uint32_t cap,
-	SortState* st, uint32_t* block_hist /* [gridDim][256] */, uint32_t reg_items /* RS_REG_ITEMS; 0 forces the tiled path (tests) */)
-{
-	__shared__ uint32_t s_hist[256];              // count phase: this block's digit histogram; scatter phase: the block's running digit cursors
-	__shared__ uint32_t s_part[2][256], s_wsum[8];
-	__shared__ uint32_t s_wcnt[RS_WARPS][256];    // per warp: keys of digit d in the warp's part of the tile, then the warp's first destination of digit d
-	__shared__ unsigned long long s_red[2][RS_WARPS];
-	const uint32_t n = min(counts[0], cap);
-	if (n < 2) return; // uniform over the grid: nothing to sort (buffer 0 already holds the result)
-	uint32_t barriers_passed = 0;
-	const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-	const bool in_regs = n <= gridDim.x * (uint32_t)RS_THREADS * reg_items;
-	uint32_t key_begin, key_end, tile_begin = 0, tile_end = 0, items = 0;
-	if (in_regs) {
-		items = (n + gridDim.x * RS_THREADS - 1) / (gridDim.x * RS_THREADS); // 1..RS_REG_ITEMS keys per thread
-		key_begin = min(n, blockIdx.x * items * RS_THREADS);
-		key_end = min(n, key_begin + items * RS_THREADS);
-	}
-	else {
-		const uint32_t n_tiles = (n + RS_TILE - 1) / RS_TILE;
-		tile_begin = (uint32_t)(((unsigned long long)blockIdx.x * n_tiles) / gridDim.x);
-		tile_end = (uint32_t)(((unsigned long long)(blockIdx.x + 1) * n_tiles) / gridDim.x);
-		key_begin = tile_begin * RS_TILE;
-		key_end = min(n, tile_end * RS_TILE);
-	}
-
-	// which bits differ at all: OR of every key and OR of every complement
-	{
-		unsigned long long o = 0ull, a = 0ull;
-		for (uint32_t i = key_begin + tid; i < key_end; i += RS_THREADS) { const unsigned long long k = kbuf0[i]; o |= k; a |= ~k; }
-#pragma unroll
-		for (int d = 16; d > 0; d >>= 1) { o |= __shfl_xor_sync(0xffffffffu, o, d); a |= __shfl_xor_sync(0xffffffffu, a, d); }
-		if (lane == 0) { s_red[0][warp] = o; s_red[1][warp] = a; }
-		__syncthreads();
-		if (tid == 0) {
-			for (int w = 1; w < RS_WARPS; ++w) { o |= s_red[0][w]; a |= s_red[1][w]; }
-			if (key_begin < key_end) { atomicOr(&st->key_or, o); atomicOr(&st->key_or_not, a); }
-		}
-	}
-	grid_barrier(&st->bar, barriers_passed);
-	const unsigned long long varying = __ldcg(&st->key_or) & __ldcg(&st->key_or_not); // bits that are 1 in some key and 0 in another
-
-	uint32_t cur = 0;
-	int window = 0; // at most RS_PASSES digit windows: each takes at least one differing bit out of 64 and 8 bits wide windows cover them all
-	if (in_regs) {
-		// the warp's run: [key_begin + warp * items * 32, + items * 32); item j of lane l = run + j * 32 + l, so (j, lane) is the key order
-		const uint32_t wbase = key_begin + warp * items * 32u;
-		uint64_t k[RS_REG_ITEMS], v[RS_REG_ITEMS];
-		uint16_t rk[RS_REG_ITEMS];
-		// digit windows: 8 bits from the lowest bit that still differs between keys, then from the next such bit above the window, ...
-		// (bytes in which every key agrees cost nothing, and a group of differing bits that straddles a byte border is one pass, not two)
-#pragma unroll 1
-		for (unsigned long long left = varying; left != 0ull; ++window) {
-			const int shift = __ffsll((long long)left) - 1;
-			left &= ~(0xffull << shift);
-			const uint64_t* ksrc = cur ? kbuf1 : kbuf0;
-			const uint64_t* vsrc = cur ? vbuf1 : vbuf0;
-			uint64_t* kdst = cur ? kbuf0 : kbuf1;
-			uint64_t* vdst = cur ? vbuf0 : vbuf1;
-#pragma unroll
-			for (int j = 0; j < RS_REG_ITEMS; ++j) {
-				const uint32_t i = wbase + j * 32 + lane;
-				const bool has = (uint32_t)j < items && i < key_end;
-				k[j] = has ? __ldcg(ksrc + i) : 0;
-				v[j] = has ? __ldcg(vsrc + i) : 0;
-			}
-			for (int d = lane; d < 256; d += 32) s_wcnt[warp][d] = 0;
-			__syncwarp();
-#pragma unroll
-			for (int j = 0; j < RS_REG_ITEMS; ++j) {
-				if ((uint32_t)j < items) { // uniform
-					const bool has = wbase + j * 32 + lane < key_end;
-					const uint32_t dg = has ? (uint32_t)(k[j] >> shift) & 0xffu : 0x100u; // lanes past the end match only each other
-					const uint32_t peers = __match_any_sync(0xffffffffu, dg);
-					const uint32_t below = __popc(peers & ((1u << lane) - 1u));
-					uint32_t seen = 0;
-					if (has) seen = s_wcnt[warp][dg];
-					__syncwarp();
-					if (has && below == 0) s_wcnt[warp][dg] = seen + __popc(peers);
-					__syncwarp();
-					rk[j] = (uint16_t)(seen + below);
-				}
-			}
-			__syncthreads();
-			if (tid < 256) { // digit tid: the warps' counts -> each warp's offset inside the block's slice; the sum is the block's histogram entry
-				uint32_t acc = 0;
-#pragma unroll
-				for (int w = 0; w < RS_WARPS; ++w) { const uint32_t t = s_wcnt[w][tid]; s_wcnt[w][tid] = acc; acc += t; }
-				block_hist[blockIdx.x * 256 + tid] = acc;
-				if (acc) atomicAdd(&st->digit_total[window][tid], acc);
-			}
-			grid_barrier(&st->bar, barriers_passed);
-			digit_starts(block_hist, st->digit_total[window], s_hist, s_part, s_wsum);
-#pragma unroll
-			for (int j = 0; j < RS_REG_ITEMS; ++j) {
-				if ((uint32_t)j < items && wbase + j * 32 + lane < key_end) {
-					const uint32_t dg = (uint32_t)(k[j] >> shift) & 0xffu;
-					const uint32_t dest = s_hist[dg] + s_wcnt[warp][dg] + rk[j];
-					kdst[dest] = k[j];
-					vdst[dest] = v[j];
-				}
-			}
-			grid_barrier(&st->bar, barriers_passed);
-			cur ^= 1u;
-		}
-	}
-	else {
-#pragma unroll 1
-		for (unsigned long long left = varying; left != 0ull; ++window) {
-			const int shift = __ffsll((long long)left) - 1;
-			left &= ~(0xffull << shift);
-			const uint64_t* ksrc = cur ? kbuf1 : kbuf0;
-			const uint64_t* vsrc = cur ? vbuf1 : vbuf0;
-			uint64_t* kdst = cur ? kbuf0 : kbuf1;
-			uint64_t* vdst = cur ? vbuf0 : vbuf1;
-			// count
-			if (tid < 256) s_hist[tid] = 0;
-			__syncthreads();
-			for (uint32_t i = key_begin + tid; i < key_end; i += RS_THREADS) atomicAdd(&s_hist[(uint32_t)(__ldcg(ksrc + i) >> shift) & 0xffu], 1u);
-			__syncthreads();
-			if (tid < 256) {
-				block_hist[blockIdx.x * 256 + tid] = s_hist[tid];
-				if (s_hist[tid]) atomicAdd(&st->digit_total[window][tid], s_hist[tid]);
-			}
-			grid_barrier(&st->bar, barriers_passed);
-			digit_starts(block_hist, st->digit_total[window], s_hist, s_part, s_wsum);
-			// stable scatter, tile by tile
-			for (uint32_t tile = tile_begin; tile < tile_end; ++tile) {
-				const uint32_t wbase = tile * RS_TILE + warp * (32 * RS_ITEMS);
-				uint64_t k[RS_ITEMS], v[RS_ITEMS];
-				uint32_t dg[RS_ITEMS], rk[RS_ITEMS];
-#pragma unroll
-				for (int j = 0; j < RS_ITEMS; ++j) {
-					const uint32_t i = wbase + j * 32 + lane;
-					const bool has = i < n;
-					k[j] = has ? __ldcg(ksrc + i) : 0;
-					v[j] = has ? __ldcg(vsrc + i) : 0;
-					dg[j] = has ? (uint32_t)(k[j] >> shift) & 0xffu : 0x100u; // keys past the end match only each other
-				}
-				for (int d = lane; d < 256; d += 32) s_wcnt[warp][d] = 0;
-				__syncwarp();
-#pragma unroll
-				for (int j = 0; j < RS_ITEMS; ++j) {
-					const uint32_t peers = __match_any_sync(0xffffffffu, dg[j]);
-					const uint32_t below = __popc(peers & ((1u << lane) - 1u));
-					uint32_t seen = 0;
-					if (dg[j] < 256) seen = s_wcnt[warp][dg[j]];
-					__syncwarp();
-					if (dg[j] < 256 && below == 0) s_wcnt[warp][dg[j]] = seen + __popc(peers);
-					__syncwarp();
-					rk[j] = seen + below;
-				}
-				__syncthreads();
-				if (tid < 256) { // digit tid: the warps' slices in warp order, then advance the block's cursor past the tile
-					uint32_t acc = s_hist[tid];
-#pragma unroll
-					for (int w = 0; w < RS_WARPS; ++w) { const uint32_t t = s_wcnt[w][tid]; s_wcnt[w][tid] = acc; acc += t; }
-					s_hist[tid] = acc;
-				}
-				__syncthreads();
-#pragma unroll
-				for (int j = 0; j < RS_ITEMS; ++j) {
-					if (dg[j] < 256) {
-						const uint32_t dest = s_wcnt[warp][dg[j]] + rk[j];
-						kdst[dest] = k[j];
-						vdst[dest] = v[j];
-					}
-				}
-				__syncthreads();
-			}
-			grid_barrier(&st->bar, barriers_passed);
-			cur ^= 1u;
-		}
-	}
-	if (cur) { // sorted data to buffer 0 if it ended up in buffer 1
-		for (uint32_t i = key_begin + tid; i < key_end; i += RS_THREADS) { kbuf0[i] = __ldcg(kbuf1 + i); vbuf0[i] = __ldcg(vbuf1 + i); }
-	}
-}
-
-int coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out) {
-	int per_sm = 0;
-	LB200_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-	if (per_sm < 1) { lb200_set_error(ctx, "cooperative kernel does not fit on an SM (%zu B of shared memory)", smem); return LB200_ERR_CUDA; }
-	*out = (uint32_t)per_sm * (uint32_t)ctx->sm_count;
-	return LB200_OK;
-}
-
 } // namespace
-
-// Stable LSD radix sort of n = min(*count_dev, cap) (key, value) pairs of 64 bits, one cooperative launch on `stream`, n read on the device.
-// The sorted pairs end in buffer 0.  state: lb200_radix_sort_state_bytes() bytes, block_hist: 256 x blocks words; at most `blocks` blocks
-// are launched.  force_tiled: the tiled path at any n.  *out_grid (may be null): the blocks launched.  (Also used by the device re-binning
-// of the culling structure, culling_rebin.cu, and by lb200_radix_sort_device.)
-size_t lb200_radix_sort_state_bytes() { return sizeof(SortState); }
-
-static int radix_sort_grid_limit(lb200_ctx* ctx, uint32_t* out) {
-	static uint32_t limit = 0; // blocks of radix_sort_kernel that are co-resident (one device kind per process)
-	if (!limit) { const int rc = coop_grid_limit(ctx, (const void*)radix_sort_kernel, RS_THREADS, 0, &limit); if (rc) return rc; }
-	*out = limit;
-	return LB200_OK;
-}
-
-int lb200_radix_sort_pairs(lb200_ctx* ctx, cudaStream_t s, uint64_t* keys0, uint64_t* keys1, uint64_t* values0, uint64_t* values1, const uint32_t* count_dev, uint32_t cap,
-	void* state, uint32_t* block_hist, uint32_t blocks, bool force_tiled, uint32_t* out_grid)
-{
-	uint32_t limit = 0;
-	const int rc = radix_sort_grid_limit(ctx, &limit);
-	if (rc) return rc;
-	SortState* st = (SortState*)state;
-	LB200_CUDA(ctx, cudaMemsetAsync(st, 0, sizeof(SortState), s));
-	uint32_t grid = std::max(1u, std::min(std::min(limit, blocks), (cap + RS_TILE - 1) / RS_TILE));
-	uint32_t reg_items = force_tiled ? 0u : (uint32_t)RS_REG_ITEMS;
-	void* args[] = {&keys0, &keys1, &values0, &values1, &count_dev, &cap, &st, &block_hist, &reg_items};
-	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)radix_sort_kernel, dim3(grid), dim3(RS_THREADS), args, 0, s));
-	LB200_CHECK_LAUNCH(ctx);
-	if (out_grid) *out_grid = grid;
-	return LB200_OK;
-}
-
-// Scratch of lb200_radix_sort_device, kept in the context and grown to the largest cap asked for: the second key / value buffers,
-// then the SortState and the block histograms of the largest grid.
-struct SortScratch { uint64_t* keys1; uint64_t* values1; SortState* state; uint32_t* block_hist; };
-static size_t sort_scratch_bytes(uint32_t cap, uint32_t blocks) { return 2 * sizeof(uint64_t) * (size_t)cap + sizeof(SortState) + sizeof(uint32_t) * 256 * (size_t)blocks; }
-static SortScratch sort_scratch_at(void* base, uint32_t cap) {
-	char* p = (char*)base;
-	SortScratch s;
-	s.keys1 = (uint64_t*)p;
-	s.values1 = (uint64_t*)(p + sizeof(uint64_t) * (size_t)cap);
-	s.state = (SortState*)(p + 2 * sizeof(uint64_t) * (size_t)cap);
-	s.block_hist = (uint32_t*)(s.state + 1);
-	return s;
-}
-
-extern "C" int lb200_radix_sort_device(lb200_ctx* ctx, uint64_t* dev_keys, uint64_t* dev_values, const uint32_t* dev_count, uint32_t cap, uint32_t max_blocks, int force_tiled,
-	uint32_t* out_grid)
-{
-	if (!ctx || !dev_keys || !dev_values || !dev_count) return LB200_ERR_INVALID;
-	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	uint32_t limit = 0;
-	int rc = radix_sort_grid_limit(ctx, &limit);
-	if (rc) return rc;
-	const uint32_t scratch_cap = std::max(cap, 1u);
-	if (scratch_cap > ctx->sort_scratch_cap) { // the stream may still use the old scratch
-		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		ctx->sort_scratch.reset();
-		ctx->sort_scratch_cap = 0;
-		LB200_CUDA(ctx, ctx->sort_scratch.alloc(sort_scratch_bytes(scratch_cap, limit)));
-		ctx->sort_scratch_cap = scratch_cap;
-	}
-	const SortScratch sc = sort_scratch_at(ctx->sort_scratch, ctx->sort_scratch_cap);
-	uint32_t grid = 0;
-	rc = lb200_radix_sort_pairs(ctx, ctx->stream, dev_keys, sc.keys1, dev_values, sc.values1, dev_count, cap, sc.state, sc.block_hist, max_blocks ? max_blocks : limit,
-		force_tiled != 0, &grid);
-	if (rc) return rc;
-	if (out_grid) *out_grid = grid;
-	return LB200_OK;
-}
 
 constexpr uint32_t NO_MODEL = 0xffffffffu;
 
@@ -818,8 +477,7 @@ struct lb200_sortkeys {
 	DeviceArray<float> d_lod; DeviceArray<uint32_t> d_pose_frame; // unpacked on request (lb200_sortkeys_device_outputs)
 	DeviceArray<uint32_t> d_moved_list, d_moved_count; DeviceArray<lb200_transform> d_prev; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move onwards)
 	DeviceArray<GridBar> d_bar;
-	DeviceArray<SortState> d_sort_state; DeviceArray<uint32_t> d_block_hist;
-	uint32_t sort_blocks = 0;
+	RadixSortScratch radix_scratch; // the sort of d_keys / d_values, with d_keys[1] / d_values[1] as its alternate buffers
 	uint32_t last_groups = 0;
 	uint32_t max_mesh_sort_key = 0; // largest sort key of the mesh table: every view's max_sort_key must reach it
 	uint32_t model_past_table = NO_MODEL; // first model whose meshes leave the mesh table (create_keys refuses to launch), NO_MODEL if none
@@ -880,9 +538,8 @@ int lb200_sortkeys_create(lb200_ctx* ctx, uint32_t max_entities, uint32_t max_gr
 	LB200_CUDA(ctx, sk->d_stash4.alloc(3 * E));
 	LB200_CUDA(ctx, sk->d_bar.alloc(1));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_bar, 0, sizeof(GridBar), ctx->stream));
-	LB200_CUDA(ctx, sk->d_sort_state.alloc(1));
-	sk->sort_blocks = (uint32_t)ctx->sm_count * 2;
-	LB200_CUDA(ctx, sk->d_block_hist.alloc(256 * (size_t)sk->sort_blocks));
+	const int rc = lb200_radix_sort_alloc_scratch(ctx, (uint32_t)ctx->sm_count * 2, sk->radix_scratch);
+	if (rc) return rc;
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	*out = sk.release();
 	return LB200_OK;
@@ -1028,7 +685,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	size_t smem = in_smem ? sizeof(uint32_t) * n_groups : 0;
 	uint32_t& limit = sk->keys_grid_limit[in_smem ? 0 : 1];
 	if (!limit) { // co-resident blocks with the largest group table this path can ask for, so that the number holds for every view
-		rc = coop_grid_limit(ctx, (const void*)create_keys_kernel, SK_THREADS, in_smem ? sizeof(uint32_t) * SK_SMEM_GROUPS : 0, &limit);
+		rc = lb200_coop_grid_limit(ctx,(const void*)create_keys_kernel, SK_THREADS, in_smem ? sizeof(uint32_t) * SK_SMEM_GROUPS : 0, &limit);
 		if (rc) return rc;
 	}
 	const uint32_t work = type_counts[RT_MESH] + type_counts[RT_DECAL] + type_counts[RT_CURVE_DECAL]; // upper bound of visible renderables
@@ -1044,7 +701,7 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	sk->last_grid = grid; sk->last_in_smem = in_smem ? 1 : 0; sk->last_prefetch = EP.prefetch_ahead;
 	if (sort) {
 		lb200_range r2("radixSort"); // pipeline.cpp:4101
-		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->d_sort_state, sk->d_block_hist, sk->sort_blocks, false, nullptr);
+		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->radix_scratch, 0, false, nullptr);
 		if (rc) return rc;
 	}
 	if (want_counts) {

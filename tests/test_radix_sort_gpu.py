@@ -1,4 +1,4 @@
-"""The device radix sort on its own (radix_sort_kernel, csrc/sortkeys.cu, through lb200_radix_sort_device), held to its contract: a stable
+"""The device radix sort on its own (radix_sort_kernel, csrc/radix_sort.cu, through lb200_radix_sort_device), held to its contract: a stable
 sort of (u64 key, u64 value) pairs by key.  The reference is np.argsort(kind="stable"), and for up to a few thousand pairs also the oracle's
 restatement of the reference's own PipelineImpl::radixSort; the device result must equal it element for element.  Values are mostly the
 input positions, so that any pair of equal keys that changes order shows.

@@ -1,4 +1,4 @@
-"""GPU parity of the stage behind the cull — createSortKeys + radixSort on the device (csrc/sortkeys.cu) — against the oracle:
+"""GPU parity of the stage behind the cull — createSortKeys + radixSort on the device (csrc/sortkeys.cu, csrc/radix_sort.cu) — against the oracle:
 sorted (key, value) pairs as a multiset, auto-instancing groups as sets with their 48-byte instance data matched by renderable, lod state,
 pose and dirty lists, bit for bit."""
 import numpy as np
