@@ -209,6 +209,16 @@ LB200_API int lb200_culling_set_replicas(lb200_culling* cs, uint32_t replicas);
 LB200_API int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities, const double* dev_pos3, const float* dev_radius, uint32_t n, uint32_t max_entity);
 LB200_API int lb200_culling_sync_host(lb200_culling* cs);
 LB200_API uint32_t lb200_culling_last_rebin_changers(const lb200_culling* cs);
+/* CullingSystem::add (culling_system.cpp:131-157) for n entities whose spheres and types lie in device memory (spawn lists built on the
+ * device).  dev_entities NULL = identity.  Every id must be in [0, max_entity], not added yet, listed once, and have a type other than
+ * LB200_TYPE_ALL; otherwise the call returns LB200_ERR_INVALID and changes nothing.  Like lb200_culling_set_many_device the device stays
+ * authoritative (the host mirror follows lazily), two synchronisations per call, and slots / pages may differ from a sequential replay
+ * while visible sets do not.  Needs set_replicas(1). */
+LB200_API int lb200_culling_add_many_device(lb200_culling* cs, const int32_t* dev_entities, const uint8_t* dev_types, const double* dev_pos3,
+                                            const float* dev_radius, uint32_t n, uint32_t max_entity);
+/* CullingSystem::remove (culling_system.cpp:160-187) for n entity ids in device memory.  Ids that are not added are skipped, as in the
+ * reference; an id listed twice is removed once.  One synchronisation per call.  Needs set_replicas(1). */
+LB200_API int lb200_culling_remove_many_device(lb200_culling* cs, const int32_t* dev_entities, uint32_t n);
 /* Measurement helper: device time (ms) of `iters` single culls, each with the device to itself and its launch already queued when the
  * device reaches it (no host launch latency inside the interval, nothing overlapping the cull).  mode 0 = the cull, 1 = nothing between
  * the two event records, 2 = one empty kernel of the cull's grid (the fixed costs the first number contains). */

@@ -173,7 +173,7 @@ int prepareExchange(lb200_culling* cs, const lb200_shifted_frustum* frustum) {
 	lb200_ctx* ctx = cs->ctx;
 	lb200_ctx::Peer& peer = ctx->peer;
 	if (!peer.ready) { lb200_set_error(ctx, "cull_exchange needs lb200_comm_enable_p2p"); return LB200_ERR_STATE; }
-	if (cs->host.cells.empty()) { lb200_set_error(ctx, "cull_exchange on an empty culling system"); return LB200_ERR_STATE; }
+	if (noEntities(cs)) { lb200_set_error(ctx, "cull_exchange on an empty culling system"); return LB200_ERR_STATE; }
 	int rc = flushPages(cs); // uploads (if any) go to the context stream, before any lane forks from it
 	if (rc) return rc;
 	if (peer.lanes != cs->lanes) { lb200_set_error(ctx, "exchange lanes (%u) differ from cull lanes (%u)", peer.lanes, cs->lanes); return LB200_ERR_STATE; }
@@ -241,7 +241,7 @@ int lb200_culling_cull_gather(lb200_culling* cs, const lb200_shifted_frustum* fr
 	if (!cs || !frustum) return LB200_ERR_INVALID;
 	if (!cs->ctx) return LB200_ERR_NO_DEVICE;
 	lb200_ctx* ctx = cs->ctx;
-	if (cs->host.cells.empty()) { lb200_set_error(ctx, "cull_gather on an empty culling system"); return LB200_ERR_STATE; }
+	if (noEntities(cs)) { lb200_set_error(ctx, "cull_gather on an empty culling system"); return LB200_ERR_STATE; }
 	int rc = lb200_comm_check(ctx);
 	if (rc) return rc;
 	rc = launchCull(cs, frustum, type);

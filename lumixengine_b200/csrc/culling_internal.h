@@ -99,6 +99,9 @@ struct lb200_culling {
 	// While `device_authoritative`, the page arrays in HBM are ahead of the host mirror (entities were re-binned by kernels); any host-side
 	// accessor or mutator first pulls the device state back (syncHostFromDevice).
 	bool device_authoritative = false;
+	// Device adds / removes (lb200_culling_add_many_device, _remove_many_device) changed which entities are added since the last pull-back:
+	// is_added has to pull back first.  Type counts, entity count and bad-radius count stay current on the host either way.
+	bool membership_on_device = false;
 	uint64_t rebin_built_gen = ~0ull;   // host.edit_gen the device-side tables were built from
 	// Each group below is allocated and released as a whole (ensureRebinState, lb200_culling_set_many_device).
 	DeviceArray<uint32_t> d_entity_to_slot;
@@ -108,7 +111,7 @@ struct lb200_culling {
 	DeviceArray<uint32_t> d_free_pages;     // stack of free page ids
 	DeviceArray<uint32_t> d_page_dirty, d_dirty_pages;
 	DeviceArray<unsigned long long> d_hash_keys; DeviceArray<uint32_t> d_hash_vals; // packed cell key -> open page of its chain
-	DeviceArray<uint32_t> d_rebin_counters; PinnedArray<uint32_t> h_rebin_counters; // RB_* (culling_rebin.cu); pinned mirror
+	DeviceArray<uint32_t> d_rebin_counters; PinnedArray<uint32_t> h_rebin_counters; // RB_* and per-type deltas (culling_rebin.cu); pinned mirror
 	RadixSortScratch rb_radix_scratch; // the changer sort, with d_rb_keys[1] / d_rb_vals[1] as its alternate buffers
 	// per changer slot
 	DeviceArray<uint32_t> d_changers;       // mover indices that change cell / chain
@@ -142,6 +145,9 @@ int syncHostFromDevice(lb200_culling* cs);
 
 // pages the kernels have to look at: the host's high-water mark, or the device's own while it is ahead of the host mirror
 inline uint32_t livePages(const lb200_culling* cs) { return cs->device_authoritative ? cs->dev_high_water : cs->host.high_water; }
+// no entity is added (the reference's empty m_cells, culling_system.cpp:322): the host's chains are stale after device adds / removes,
+// its entity count is not
+inline bool noEntities(const lb200_culling* cs) { return cs->device_authoritative ? cs->host.n_entities == 0 : cs->host.cells.empty(); }
 
 // the host mirror made current before it is read or edited, by const accessors too: LB200_OK or the error of the pull-back
 inline int hostView(const lb200_culling* cs) { return cs && cs->device_authoritative ? syncHostFromDevice(const_cast<lb200_culling*>(cs)) : LB200_OK; }

@@ -13,6 +13,12 @@
 // origin computed exactly as culling_system.cpp:100 does, pages hold <= 200 spheres, empty pages are skipped.  Which slot / which page of
 // its chain an entity occupies differs from the sequential host order (as it does between two edit orders on the host); the per-page
 // statistics of a cull can therefore differ from a host-side replay, visible sets cannot.
+// Device adds and removes (CullingSystem::add / remove, culling_system.cpp:131-187, for batches whose data lies in HBM) use the same steps:
+//   add      one thread per new entity claims its id in entity -> slot (a refused batch releases its claims and changes nothing else) and
+//            builds its chain key; after one read-back the keys go through step 3 exactly as re-binned changers do;
+//   remove   one thread per id takes the entity's slot out of entity -> slot and tombstones it; step 2's compaction follows.
+// Both keep per-type count deltas, which the batch's last read-back applies to the host's type counts (the cull's output layout).
+// The chain hash map counts its keys and is rehashed on the device into a larger table before a batch could fill it past half.
 // The pull-back of the host mirror (syncHostFromDevice) lives here too: it undoes what these kernels leave ahead of the host.
 // =====================================================================================================================================
 #include "culling_internal.h"
@@ -24,9 +30,16 @@ using namespace lbcull;
 
 namespace {
 
-enum { RB_HIGH_WATER = 0, RB_N_FREE, RB_N_CHANGERS, RB_N_DIRTY, RB_OVERFLOW, RB_BAD_RADIUS, RB_WORDS = 8 };
+// counter words: [0, RB_WORDS) the state every batch reads back (RB_OVERFLOW holds OVERFLOW_PAGES | OVERFLOW_HASH), then the words of an
+// add batch's first read-back, then RB_TYPE_DELTA: 256 per-type count deltas of an add / remove batch (two's complement).  The batch
+// words are zeroed by the batch that uses them.
+enum { RB_HIGH_WATER = 0, RB_N_FREE, RB_N_CHANGERS, RB_N_DIRTY, RB_OVERFLOW, RB_BAD_RADIUS, RB_N_KEYS, RB_NEW_PAGES, RB_WORDS,
+	RB_REFUSED = RB_WORDS, RB_MAX_ID, RB_ADD_WORDS = RB_WORDS + 8 };
+constexpr uint32_t RB_TYPE_DELTA = RB_ADD_WORDS, RB_ALL_WORDS = RB_ADD_WORDS + 256;
+constexpr uint32_t OVERFLOW_PAGES = 1u, OVERFLOW_HASH = 2u;
 constexpr unsigned long long HASH_EMPTY = ~0ull;
 constexpr uint32_t NO_OPEN_PAGE = 0xffffffffu;
+constexpr uint32_t CLAIMED = 0xfffffffeu; // entity -> slot of an id an add batch has claimed and not placed yet (no page reaches it)
 
 __host__ __device__ __forceinline__ unsigned long long packCellKey(int x, int y, int z, uint32_t type, uint32_t is_big) {
 	// 18 bits per axis (+-131 071 cells of 300 m), 8 bits type, 1 bit is_big
@@ -40,12 +53,33 @@ __host__ __device__ __forceinline__ uint32_t hashCellKey(unsigned long long k) {
 
 __device__ __forceinline__ uint32_t hashFind(const unsigned long long* keys, const uint32_t* vals, uint32_t cap, unsigned long long key, uint32_t* slot_out) {
 	uint32_t i = hashCellKey(key) & (cap - 1);
-	for (;;) {
+	for (uint32_t probe = 0; probe < cap; ++probe) {
 		const unsigned long long k = keys[i];
 		if (k == key) { *slot_out = i; return vals[i]; }
 		if (k == HASH_EMPTY) { *slot_out = i; return NO_OPEN_PAGE; }
 		i = (i + 1) & (cap - 1);
 	}
+	*slot_out = 0; // a full table without the key: the key has no open page
+	return NO_OPEN_PAGE;
+}
+
+// find or claim `key`'s slot (linear probing, at most `cap` probes); false: the table is full
+__device__ __forceinline__ bool hashClaim(unsigned long long* keys, uint32_t cap, unsigned long long key, uint32_t* slot_out, bool* inserted) {
+	uint32_t i = hashCellKey(key) & (cap - 1);
+	for (uint32_t probe = 0; probe < cap; ++probe) {
+		const unsigned long long prev = atomicCAS(&keys[i], HASH_EMPTY, key);
+		if (prev == HASH_EMPTY || prev == key) { *slot_out = i; *inserted = prev == HASH_EMPTY; return true; }
+		i = (i + 1) & (cap - 1);
+	}
+	return false;
+}
+
+// chain of an entity: cell = IVec3(pos * (1 / 300.f)) (culling_system.cpp:25-31), is_big = radius > 300
+__device__ __forceinline__ unsigned long long chainKey(const double* __restrict__ pos3, uint32_t i, uint32_t type, float radius, int* ix_out) {
+	const double inv = (double)(1 / LB200_CELL_SIZE);
+	const int ix = (int)__dmul_rn(pos3[3 * (size_t)i], inv), iy = (int)__dmul_rn(pos3[3 * (size_t)i + 1], inv), iz = (int)__dmul_rn(pos3[3 * (size_t)i + 2], inv);
+	*ix_out = ix;
+	return packCellKey(ix, iy, iz, type, radius > LB200_CELL_SIZE ? 1u : 0u);
 }
 
 // 1. classify + in-place overwrite
@@ -101,10 +135,9 @@ __global__ void __launch_bounds__(256) rebin_remove_kernel(const uint32_t* __res
 		if (!(old_r >= 0.0f)) atomicAdd(&wcounters[RB_BAD_RADIUS], 0xffffffffu);
 		entities[slot] = -1 - e; // tombstone
 		if (atomicExch(&page_dirty[page], 1u) == 0u) dirty_pages[atomicAdd(&wcounters[RB_N_DIRTY], 1u)] = page;
-		const double inv = (double)(1 / LB200_CELL_SIZE);
-		const int ix = (int)__dmul_rn(pos3[3 * (size_t)i], inv), iy = (int)__dmul_rn(pos3[3 * (size_t)i + 1], inv), iz = (int)__dmul_rn(pos3[3 * (size_t)i + 2], inv);
+		int ix;
 		const uint32_t type = (uint32_t)page_cell[page].w & 0xffu; // set() keeps the renderable type (:236-239)
-		keys[k] = packCellKey(ix, iy, iz, type, radius[i] > LB200_CELL_SIZE ? 1u : 0u);
+		keys[k] = chainKey(pos3, i, type, radius[i], &ix);
 		vals[k] = ((uint64_t)(uint32_t)ix) | ((uint64_t)i << 32); // mover index; the cell indices are recomputed by the add kernel
 		if (!(radius[i] >= 0.0f)) atomicAdd(&wcounters[RB_BAD_RADIUS], 1u);
 	}
@@ -155,6 +188,90 @@ __global__ void __launch_bounds__(256) rebin_compact_kernel(const uint32_t* __re
 	}
 }
 
+// Device add, before step 3: every id is claimed (atomicCAS NO_SLOT -> CLAIMED, so an added id or one listed twice fails), ids outside
+// [0, max_entity] and the reserved type are refused, the batch's types and its largest id are counted, and every entity's chain key is
+// built for step 3.  Nothing but this batch's claims and its zeroed batch words is written: rebin_add_release_kernel undoes a refusal.
+__global__ void __launch_bounds__(256) rebin_add_claim_kernel(uint32_t n, const int32_t* __restrict__ ents, const uint8_t* __restrict__ types,
+	const double* __restrict__ pos3, const float* __restrict__ radius, uint32_t max_entity, uint32_t* __restrict__ entity_to_slot, uint32_t* __restrict__ counters,
+	uint64_t* __restrict__ keys, uint64_t* __restrict__ vals)
+{
+	__shared__ uint32_t s_types[256];
+	__shared__ uint32_t s_max, s_refused;
+	s_types[threadIdx.x] = 0;
+	if (threadIdx.x == 0) { s_max = 0; s_refused = 0; }
+	__syncthreads();
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) {
+		const int32_t e = ents ? ents[i] : (int32_t)i;
+		const uint32_t type = types[i];
+		bool ok = e >= 0 && (uint32_t)e <= max_entity && type != LB200_TYPE_ALL;
+		if (ok) ok = atomicCAS(&entity_to_slot[e], NO_SLOT, CLAIMED) == NO_SLOT;
+		if (ok) { atomicAdd(&s_types[type], 1u); atomicMax(&s_max, (uint32_t)e); }
+		else atomicAdd(&s_refused, 1u);
+		int ix;
+		keys[i] = chainKey(pos3, i, type, radius[i], &ix);
+		vals[i] = ((uint64_t)(uint32_t)ix) | ((uint64_t)i << 32);
+	}
+	if (i == 0) counters[RB_N_CHANGERS] = n; // step 3 places every entity of an accepted batch
+	__syncthreads();
+	if (s_types[threadIdx.x]) atomicAdd(&counters[RB_TYPE_DELTA + threadIdx.x], s_types[threadIdx.x]);
+	if (threadIdx.x == 0) {
+		if (s_refused) atomicAdd(&counters[RB_REFUSED], s_refused);
+		atomicMax(&counters[RB_MAX_ID], s_max);
+	}
+}
+
+// a refused add batch: the ids it claimed go back to NO_SLOT
+__global__ void __launch_bounds__(256) rebin_add_release_kernel(uint32_t n, const int32_t* __restrict__ ents, uint32_t max_entity, uint32_t* __restrict__ entity_to_slot) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const int32_t e = ents ? ents[i] : (int32_t)i;
+	if (e >= 0 && (uint32_t)e <= max_entity && entity_to_slot[e] == CLAIMED) entity_to_slot[e] = NO_SLOT;
+}
+
+// Device remove: each id takes its slot out of entity -> slot (atomicExch, so an id listed twice finds NO_SLOT the second time; ids that
+// are not added are skipped, culling_system.cpp:160-163) and tombstones it as step 2a does; rebin_compact_kernel then compacts the pages.
+__global__ void __launch_bounds__(256) rebin_remove_ids_kernel(uint32_t n, const int32_t* __restrict__ ents, uint32_t* __restrict__ entity_to_slot, uint32_t entity_cap,
+	const int4* __restrict__ page_cell, const float4* __restrict__ spheres, int* __restrict__ entities, uint32_t* __restrict__ page_dirty, uint32_t* __restrict__ dirty_pages,
+	uint32_t* __restrict__ counters)
+{
+	__shared__ uint32_t s_types[256];
+	__shared__ uint32_t s_bad;
+	s_types[threadIdx.x] = 0;
+	if (threadIdx.x == 0) s_bad = 0;
+	__syncthreads();
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) {
+		const int32_t e = ents[i];
+		const uint32_t slot = e >= 0 && (uint32_t)e < entity_cap ? atomicExch(&entity_to_slot[e], NO_SLOT) : NO_SLOT;
+		if (slot != NO_SLOT) {
+			const uint32_t page = slot / PAGE_SLOTS;
+			atomicAdd(&s_types[(uint32_t)page_cell[page].w & 0xffu], 1u);
+			if (!(spheres[slot].w >= 0.0f)) atomicAdd(&s_bad, 1u);
+			entities[slot] = -1 - e; // tombstone
+			if (atomicExch(&page_dirty[page], 1u) == 0u) dirty_pages[atomicAdd(&counters[RB_N_DIRTY], 1u)] = page;
+		}
+	}
+	__syncthreads();
+	if (s_types[threadIdx.x]) atomicSub(&counters[RB_TYPE_DELTA + threadIdx.x], s_types[threadIdx.x]);
+	if (threadIdx.x == 0 && s_bad) atomicSub(&counters[RB_BAD_RADIUS], s_bad);
+}
+
+// the chain hash map moved into a larger, emptied table; entries without an open page are dropped (a missing key reads the same)
+__global__ void __launch_bounds__(256) rebin_rehash_kernel(const unsigned long long* __restrict__ old_keys, const uint32_t* __restrict__ old_vals, uint32_t old_cap,
+	unsigned long long* __restrict__ keys, uint32_t* __restrict__ vals, uint32_t cap, uint32_t* __restrict__ counters)
+{
+	for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < old_cap; j += gridDim.x * blockDim.x) {
+		const unsigned long long k = old_keys[j];
+		const uint32_t v = old_vals[j];
+		if (k == HASH_EMPTY || v == NO_OPEN_PAGE) continue;
+		uint32_t slot; bool inserted;
+		if (!hashClaim(keys, cap, k, &slot, &inserted)) { atomicOr(&counters[RB_OVERFLOW], OVERFLOW_HASH); continue; }
+		vals[slot] = v;
+		atomicAdd(&counters[RB_N_KEYS], 1u);
+	}
+}
+
 // 3a. adds, sorted by chain: the head of every run of equal keys plans the run — how many go into the chain's open page, how many new
 // pages the rest needs (taken from the free list / the high-water mark), the pages' descriptors and final counts, the chain's new open
 // page.  Work per run is proportional to its PAGES, not its entities: a crowd that moves into one cell is placed in parallel by 3b.
@@ -171,14 +288,15 @@ __global__ void __launch_bounds__(128) rebin_plan_kernel(const uint64_t* __restr
 		uint32_t lo = k, hi = n; // end of the run: first index whose key differs (the keys are sorted)
 		while (hi - lo > 1) { const uint32_t mid = lo + (hi - lo) / 2; if (keys[mid] == key) lo = mid; else hi = mid; }
 		const uint32_t run = hi - k;
-		uint32_t hslot = hashCellKey(key) & (hash_cap - 1);
+		// find or claim the key's hash slot (runs have distinct keys: no two threads insert the same one); the host keeps the table at most
+		// half full before a batch, so a full one is an error, not a wait
+		uint32_t hslot = 0;
+		bool inserted = false;
 		uint32_t page = NO_OPEN_PAGE;
-		for (;;) { // find or claim the key's hash slot (runs have distinct keys: no two threads insert the same one)
-			const unsigned long long prev = atomicCAS(&hash_keys[hslot], HASH_EMPTY, (unsigned long long)key);
-			if (prev == HASH_EMPTY) { hash_vals[hslot] = NO_OPEN_PAGE; break; }
-			if (prev == key) { page = hash_vals[hslot]; break; }
-			hslot = (hslot + 1) & (hash_cap - 1);
-		}
+		const bool have_slot = hashClaim(hash_keys, hash_cap, key, &hslot, &inserted);
+		if (!have_slot) atomicOr(&counters[RB_OVERFLOW], OVERFLOW_HASH);
+		else if (inserted) { hash_vals[hslot] = NO_OPEN_PAGE; atomicAdd(&counters[RB_N_KEYS], 1u); }
+		else page = hash_vals[hslot];
 		RunPlan plan;
 		plan.open_page = page;
 		plan.open_count = page != NO_OPEN_PAGE ? desc[page].count : PAGE_SLOTS;
@@ -203,7 +321,7 @@ __global__ void __launch_bounds__(128) rebin_plan_kernel(const uint64_t* __restr
 				const uint32_t nf = atomicSub(&counters[RB_N_FREE], 1u);
 				if (nf != 0u && nf < 0x80000000u) np = free_pages[nf - 1];
 				else { atomicAdd(&counters[RB_N_FREE], 1u); np = atomicAdd(&counters[RB_HIGH_WATER], 1u); }
-				if (np >= page_cap) { atomicExch(&counters[RB_OVERFLOW], 1u); np = 0; }
+				if (np >= page_cap) { atomicOr(&counters[RB_OVERFLOW], OVERFLOW_PAGES); np = 0; }
 				d.count = q + 1 < m ? PAGE_SLOTS : rest - q * PAGE_SLOTS;
 				desc[np] = d;
 				page_cell[np] = make_int4(ix, iy, iz, (int)(type | (is_big << 8)));
@@ -212,14 +330,16 @@ __global__ void __launch_bounds__(128) rebin_plan_kernel(const uint64_t* __restr
 			}
 		}
 		plans[k] = plan;
-		if (page != NO_OPEN_PAGE) hash_vals[hslot] = page; // the last page opened (or the old open page) takes the chain's next adds
+		if (have_slot && page != NO_OPEN_PAGE) hash_vals[hslot] = page; // the last page opened (or the old open page) takes the chain's next adds
 	}
 }
 
-// 3b. every changer finds its run (binary search on the sorted keys), its rank in it, and from the run's plan its page and slot
-__global__ void __launch_bounds__(256) rebin_place_kernel(const uint64_t* __restrict__ keys, const uint64_t* __restrict__ vals, const uint32_t* __restrict__ counters,
+// 3b. every changer finds its run (binary search on the sorted keys), its rank in it, and from the run's plan its page and slot.
+// bad_radius: the counter new spheres with radius < 0 or NaN are counted into (device adds; re-binned changers were counted by step 2a)
+__global__ void __launch_bounds__(256) rebin_place_kernel(const uint64_t* __restrict__ keys, const uint64_t* __restrict__ vals, const uint32_t* counters,
 	const int32_t* __restrict__ ents, const double* __restrict__ pos3, const float* __restrict__ radius, uint32_t* __restrict__ entity_to_slot,
-	const lb200_page_desc* __restrict__ desc, float4* __restrict__ spheres, int* __restrict__ entities, const RunPlan* __restrict__ plans, const uint32_t* __restrict__ new_pages)
+	const lb200_page_desc* __restrict__ desc, float4* __restrict__ spheres, int* __restrict__ entities, const RunPlan* __restrict__ plans, const uint32_t* __restrict__ new_pages,
+	uint32_t* bad_radius)
 {
 	const uint32_t n = counters[RB_N_CHANGERS];
 	for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
@@ -239,6 +359,7 @@ __global__ void __launch_bounds__(256) rebin_place_kernel(const uint64_t* __rest
 			(float)__dsub_rn(pos3[3 * (size_t)i + 2], d.origin[2]), radius[i]); // :100
 		entities[slot] = e;
 		entity_to_slot[e] = slot;
+		if (bad_radius && !(radius[i] >= 0.0f)) atomicAdd(bad_radius, 1u);
 	}
 }
 
@@ -251,8 +372,8 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	if (rc) return rc;
 	if (!cs->d_rebin_counters || !cs->h_rebin_counters || !cs->rb_radix_scratch.state) {
 		DeviceArray<uint32_t> d_counters; PinnedArray<uint32_t> h_counters; RadixSortScratch sort;
-		LB200_CUDA(ctx, d_counters.alloc(RB_WORDS));
-		LB200_CUDA(ctx, h_counters.alloc(RB_WORDS));
+		LB200_CUDA(ctx, d_counters.alloc(RB_ALL_WORDS));
+		LB200_CUDA(ctx, h_counters.alloc(RB_ALL_WORDS));
 		rc = lb200_radix_sort_alloc_scratch(ctx, (uint32_t)ctx->sm_count * 2, sort);
 		if (rc) return rc;
 		cs->d_rebin_counters = std::move(d_counters); cs->h_rebin_counters = std::move(h_counters); cs->rb_radix_scratch = std::move(sort);
@@ -270,11 +391,15 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	}
 	const uint32_t need_entities = std::max((uint32_t)h.entity_to_slot.size(), max_entity + 1);
 	if (cs->d_entity_to_slot.size() < need_entities) {
+		// grown with its contents: while the device is authoritative the table is live and nothing rebuilds it from the host
+		const size_t old = cs->d_entity_to_slot.size();
+		const size_t cap = grownCapacity(old, 4096, need_entities);
+		DeviceArray<uint32_t> grown;
+		LB200_CUDA(ctx, grown.alloc(cap));
+		if (old) LB200_CUDA(ctx, cudaMemcpyAsync(grown, cs->d_entity_to_slot, sizeof(uint32_t) * old, cudaMemcpyDeviceToDevice, ctx->stream));
+		LB200_CUDA(ctx, cudaMemsetAsync(grown + old, 0xff, sizeof(uint32_t) * (cap - old), ctx->stream)); // NO_SLOT
 		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		const size_t cap = grownCapacity(cs->d_entity_to_slot.size(), 4096, need_entities);
-		cs->d_entity_to_slot.reset();
-		cs->rebin_built_gen = ~0ull;
-		LB200_CUDA(ctx, cs->d_entity_to_slot.alloc(cap));
+		cs->d_entity_to_slot = std::move(grown);
 	}
 	if (cs->rebin_built_gen == h.edit_gen && !cs->device_authoritative) return LB200_OK;
 	if (cs->device_authoritative) return LB200_OK; // the tables are live on the device
@@ -307,6 +432,7 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	counters[RB_HIGH_WATER] = n_pages;
 	counters[RB_N_FREE] = (uint32_t)h.free_pages.size();
 	counters[RB_BAD_RADIUS] = h.n_bad_radius;
+	counters[RB_N_KEYS] = (uint32_t)h.cell_map.size();
 	LB200_CUDA(ctx, cudaMemcpyAsync(cs->d_page_cell, cells.data(), sizeof(int4) * n_pages, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaMemcpyAsync(cs->d_hash_keys, hk.data(), sizeof(unsigned long long) * hcap, cudaMemcpyHostToDevice, ctx->stream));
 	LB200_CUDA(ctx, cudaMemcpyAsync(cs->d_hash_vals, hv.data(), sizeof(uint32_t) * hcap, cudaMemcpyHostToDevice, ctx->stream));
@@ -317,6 +443,91 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	cs->dev_high_water = n_pages;
 	cs->rebin_built_gen = h.edit_gen;
 	return LB200_OK;
+}
+
+// the per-changer buffers (changer list, run plans, sort keys / values and their alternates) for n changers
+int ensureChangerBuffers(lb200_culling* cs, uint32_t n) {
+	lb200_ctx* ctx = cs->ctx;
+	if (cs->d_changers.size() >= n) return LB200_OK;
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	const size_t cap = grownCapacity(cs->d_changers.size(), 4096, n);
+	// the old buffers go before the new ones are allocated
+	cs->d_changers.reset(); cs->d_rb_plans.reset();
+	for (int b = 0; b < 2; ++b) { cs->d_rb_keys[b].reset(); cs->d_rb_vals[b].reset(); }
+	DeviceArray<uint32_t> changers; DeviceArray<uint4> plans; DeviceArray<uint64_t> keys[2], vals[2];
+	LB200_CUDA(ctx, changers.alloc(cap));
+	LB200_CUDA(ctx, plans.alloc(cap));
+	for (int b = 0; b < 2; ++b) {
+		LB200_CUDA(ctx, keys[b].alloc(cap));
+		LB200_CUDA(ctx, vals[b].alloc(cap));
+	}
+	cs->d_changers = std::move(changers); cs->d_rb_plans = std::move(plans);
+	for (int b = 0; b < 2; ++b) { cs->d_rb_keys[b] = std::move(keys[b]); cs->d_rb_vals[b] = std::move(vals[b]); }
+	return LB200_OK;
+}
+
+// Keys are never removed from the chain hash map, so before a batch that may insert `adding` keys into a table holding `keys` (RB_N_KEYS
+// of the last read-back) the table is rehashed on the device into one at least twice that size: it stays at most half full.
+int growCellMap(lb200_culling* cs, uint32_t keys, uint32_t adding) {
+	lb200_ctx* ctx = cs->ctx;
+	const uint32_t old_cap = (uint32_t)cs->d_hash_keys.size();
+	const uint64_t need = 2 * ((uint64_t)keys + adding);
+	if (need <= old_cap) return LB200_OK;
+	uint64_t cap = old_cap;
+	while (cap < need) cap *= 2;
+	if (cap > 0x80000000ull) { lb200_set_error(ctx, "the chain hash map would need %llu slots", (unsigned long long)cap); return LB200_ERR_CAPACITY; }
+	cudaStream_t s = ctx->stream;
+	DeviceArray<unsigned long long> hk; DeviceArray<uint32_t> hv;
+	LB200_CUDA(ctx, hk.alloc(cap));
+	LB200_CUDA(ctx, hv.alloc(cap));
+	LB200_CUDA(ctx, cudaMemsetAsync(hk, 0xff, sizeof(unsigned long long) * cap, s)); // HASH_EMPTY
+	LB200_CUDA(ctx, cudaMemsetAsync(hv, 0xff, sizeof(uint32_t) * cap, s));           // NO_OPEN_PAGE
+	LB200_CUDA(ctx, cudaMemsetAsync(cs->d_rebin_counters + RB_N_KEYS, 0, sizeof(uint32_t), s));
+	rebin_rehash_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 4u, (old_cap + 255) / 256)), 256, 0, s>>>(cs->d_hash_keys, cs->d_hash_vals, old_cap, hk, hv,
+		(uint32_t)cap, cs->d_rebin_counters);
+	LB200_CHECK_LAUNCH(ctx);
+	LB200_CUDA(ctx, cudaStreamSynchronize(s)); // the old table is read up to here
+	cs->d_hash_keys = std::move(hk); cs->d_hash_vals = std::move(hv);
+	return LB200_OK;
+}
+
+// step 3 for the n_changers keys / values in d_rb_keys[0] / d_rb_vals[0] (their count in RB_N_CHANGERS): sort by chain, plan every
+// run, place every changer.  count_bad: the new spheres' bad radii are counted here (device adds) rather than by step 2a.
+int placeChangers(lb200_culling* cs, const int32_t* ents, const double* pos3, const float* radius, uint32_t n_changers, bool count_bad) {
+	lb200_ctx* ctx = cs->ctx;
+	cudaStream_t s = ctx->stream;
+	uint32_t* C = cs->d_rebin_counters;
+	int rc = lb200_radix_sort_pairs(ctx, s, cs->d_rb_keys[0], cs->d_rb_keys[1], cs->d_rb_vals[0], cs->d_rb_vals[1], C + RB_N_CHANGERS, (uint32_t)cs->d_changers.size(),
+		cs->rb_radix_scratch, 0, false, nullptr);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_NEW_PAGES, 0, sizeof(uint32_t), s)); // the new-page cursor of this batch
+	rebin_plan_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 8u, (n_changers + 127) / 128)), 128, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, pos3, cs->d_desc,
+		cs->d_page_cell, cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, (uint32_t)cs->d_hash_keys.size(), cs->dev_cap, (RunPlan*)cs->d_rb_plans.get(),
+		(uint32_t*)cs->d_rb_vals[1].get(), C + RB_NEW_PAGES);
+	LB200_CHECK_LAUNCH(ctx);
+	rebin_place_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 4u, (n_changers + 255) / 256)), 256, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, ents, pos3,
+		radius, cs->d_entity_to_slot, cs->d_desc, cs->d_spheres, cs->d_entities, (const RunPlan*)cs->d_rb_plans.get(), (const uint32_t*)cs->d_rb_vals[1].get(),
+		count_bad ? C + RB_BAD_RADIUS : nullptr);
+	LB200_CHECK_LAUNCH(ctx);
+	return LB200_OK;
+}
+
+// the read-back of a batch's end, in h_rebin_counters: the error of a full page array or hash map, if any
+int checkOverflow(lb200_culling* cs) {
+	const uint32_t of = cs->h_rebin_counters[RB_OVERFLOW];
+	if (of & OVERFLOW_PAGES) { lb200_set_error(cs->ctx, "device re-binning ran out of pages (capacity %u)", cs->dev_cap); return LB200_ERR_CAPACITY; }
+	if (of & OVERFLOW_HASH) { lb200_set_error(cs->ctx, "device re-binning found the chain hash map full (%zu slots)", cs->d_hash_keys.size()); return LB200_ERR_CAPACITY; }
+	return LB200_OK;
+}
+
+// the read-back of an add / remove batch's end (RB_ALL_WORDS) -> the host's counts, which the cull's output layout, its output capacity
+// and its plane-masking switch come from
+void applyBatchCounts(lb200_culling* cs) {
+	lb::CullingHost& h = cs->host;
+	const uint32_t* delta = cs->h_rebin_counters + RB_TYPE_DELTA;
+	for (int t = 0; t < 256; ++t) { h.type_counts[t] += delta[t]; h.n_entities += delta[t]; } // two's complement: removals wrap back
+	h.n_bad_radius = cs->h_rebin_counters[RB_BAD_RADIUS];
+	cs->dev_high_water = cs->h_rebin_counters[RB_HIGH_WATER];
 }
 
 } // namespace
@@ -373,6 +584,7 @@ int lbcull::syncHostFromDevice(lb200_culling* cs) {
 	h.clearDirty();
 	++h.edit_gen;
 	cs->device_authoritative = false;
+	cs->membership_on_device = false;
 	cs->rebin_built_gen = ~0ull;
 	return LB200_OK;
 }
@@ -387,24 +599,9 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 	lb200_range range("culling set many");
 	int rc = ensureRebinState(cs, max_entity);
 	if (rc) return rc;
+	rc = ensureChangerBuffers(cs, n);
+	if (rc) return rc;
 	cudaStream_t s = ctx->stream;
-	if (cs->d_changers.size() < n) {
-		LB200_CUDA(ctx, cudaStreamSynchronize(s));
-		const size_t cap = grownCapacity(cs->d_changers.size(), 4096, n);
-		// the old buffers go before the new ones are allocated
-		cs->d_changers.reset(); cs->d_rb_plans.reset();
-		for (int b = 0; b < 2; ++b) { cs->d_rb_keys[b].reset(); cs->d_rb_vals[b].reset(); }
-		DeviceArray<uint32_t> changers; DeviceArray<uint4> plans; DeviceArray<uint64_t> keys[2], vals[2];
-		LB200_CUDA(ctx, changers.alloc(cap));
-		LB200_CUDA(ctx, plans.alloc(cap));
-		for (int b = 0; b < 2; ++b) {
-			LB200_CUDA(ctx, keys[b].alloc(cap));
-			LB200_CUDA(ctx, vals[b].alloc(cap));
-		}
-		cs->d_changers = std::move(changers); cs->d_rb_plans = std::move(plans);
-		for (int b = 0; b < 2; ++b) { cs->d_rb_keys[b] = std::move(keys[b]); cs->d_rb_vals[b] = std::move(vals[b]); }
-	}
-	const uint32_t changers_cap = (uint32_t)cs->d_changers.size(), hash_cap = (uint32_t)cs->d_hash_keys.size();
 	uint32_t* C = cs->d_rebin_counters;
 	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_N_CHANGERS, 0, sizeof(uint32_t) * 2, s)); // changers, dirty pages
 	rebin_classify_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, dev_entities, dev_pos3, dev_radius, cs->d_entity_to_slot, (uint32_t)cs->d_entity_to_slot.size(), cs->d_desc, cs->d_page_cell, cs->d_spheres, cs->d_changers, C);
@@ -418,29 +615,106 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 	if (n_changers) {
 		rc = resizePages(cs, cs->h_rebin_counters[RB_HIGH_WATER] + n_changers, true); // worst case: every changer opens a page
 		if (rc) return rc;
+		rc = growCellMap(cs, cs->h_rebin_counters[RB_N_KEYS], n_changers); // worst case: every changer starts a chain
+		if (rc) return rc;
 		const uint32_t grid = std::max(1u, std::min((uint32_t)ctx->sm_count * 4u, (n_changers + 255) / 256));
 		rebin_remove_kernel<<<grid, 256, 0, s>>>(cs->d_changers, dev_entities, dev_pos3, dev_radius, cs->d_entity_to_slot, cs->d_page_cell, cs->d_spheres, cs->d_entities,
 			cs->d_page_dirty, cs->d_dirty_pages, C, cs->d_rb_keys[0], cs->d_rb_vals[0]);
 		LB200_CHECK_LAUNCH(ctx);
 		rebin_compact_kernel<<<grid, 256, 0, s>>>(cs->d_dirty_pages, C, cs->d_desc, cs->d_page_cell, cs->d_spheres, cs->d_entities, cs->d_entity_to_slot, cs->d_page_dirty,
-			cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, hash_cap);
+			cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, (uint32_t)cs->d_hash_keys.size());
 		LB200_CHECK_LAUNCH(ctx);
-		rc = lb200_radix_sort_pairs(ctx, s, cs->d_rb_keys[0], cs->d_rb_keys[1], cs->d_rb_vals[0], cs->d_rb_vals[1], C + RB_N_CHANGERS, changers_cap, cs->rb_radix_scratch,
-			0, false, nullptr);
+		rc = placeChangers(cs, dev_entities, dev_pos3, dev_radius, n_changers, false);
 		if (rc) return rc;
-		LB200_CUDA(ctx, cudaMemsetAsync(C + RB_WORDS - 1, 0, sizeof(uint32_t), s)); // the new-page cursor of this batch
-		rebin_plan_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 8u, (n_changers + 127) / 128)), 128, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, dev_pos3, cs->d_desc,
-			cs->d_page_cell, cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, hash_cap, cs->dev_cap, (RunPlan*)cs->d_rb_plans.get(), (uint32_t*)cs->d_rb_vals[1].get(), C + RB_WORDS - 1);
-		LB200_CHECK_LAUNCH(ctx);
-		rebin_place_kernel<<<grid, 256, 0, s>>>(cs->d_rb_keys[0], cs->d_rb_vals[0], C, dev_entities, dev_pos3, dev_radius, cs->d_entity_to_slot, cs->d_desc, cs->d_spheres,
-			cs->d_entities, (const RunPlan*)cs->d_rb_plans.get(), (const uint32_t*)cs->d_rb_vals[1].get());
-		LB200_CHECK_LAUNCH(ctx);
 		LB200_CUDA(ctx, cudaMemcpyAsync(cs->h_rebin_counters, C, sizeof(uint32_t) * RB_WORDS, cudaMemcpyDeviceToHost, s));
 		LB200_CUDA(ctx, cudaStreamSynchronize(s));
-		if (cs->h_rebin_counters[RB_OVERFLOW]) { lb200_set_error(ctx, "device re-binning ran out of pages (capacity %u)", cs->dev_cap); return LB200_ERR_CAPACITY; }
+		rc = checkOverflow(cs);
+		if (rc) return rc;
 	}
 	cs->dev_high_water = cs->h_rebin_counters[RB_HIGH_WATER];
 	cs->host.n_bad_radius = cs->h_rebin_counters[RB_BAD_RADIUS]; // plane masking of the cull kernel needs radius >= 0 everywhere
+	return LB200_OK;
+}
+
+int lb200_culling_add_many_device(lb200_culling* cs, const int32_t* dev_entities, const uint8_t* dev_types, const double* dev_pos3, const float* dev_radius,
+	uint32_t n, uint32_t max_entity)
+{
+	if (!cs || !dev_types || !dev_pos3 || !dev_radius) return LB200_ERR_INVALID;
+	if (!cs->ctx) return LB200_ERR_NO_DEVICE;
+	if (n == 0) return LB200_OK;
+	lb200_ctx* ctx = cs->ctx;
+	if (max_entity > (uint32_t)INT32_MAX) { lb200_set_error(ctx, "add_many_device: max_entity %u is not an entity id", max_entity); return LB200_ERR_INVALID; }
+	lb200_range range("culling add many");
+	int rc = ensureRebinState(cs, max_entity);
+	if (rc) return rc;
+	rc = ensureChangerBuffers(cs, n);
+	if (rc) return rc;
+	cudaStream_t s = ctx->stream;
+	uint32_t* C = cs->d_rebin_counters;
+	const uint32_t blocks = (n + 255) / 256;
+	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_REFUSED, 0, sizeof(uint32_t) * 2, s)); // refused, largest id
+	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_TYPE_DELTA, 0, sizeof(uint32_t) * 256, s));
+	rebin_add_claim_kernel<<<blocks, 256, 0, s>>>(n, dev_entities, dev_types, dev_pos3, dev_radius, max_entity, cs->d_entity_to_slot, C, cs->d_rb_keys[0], cs->d_rb_vals[0]);
+	LB200_CHECK_LAUNCH(ctx);
+	// the one read-back before placement: whether the batch is refused, and the page and key counts its placement is sized by
+	LB200_CUDA(ctx, cudaMemcpyAsync(cs->h_rebin_counters, C, sizeof(uint32_t) * RB_ADD_WORDS, cudaMemcpyDeviceToHost, s));
+	LB200_CUDA(ctx, cudaStreamSynchronize(s));
+	const uint32_t refused = cs->h_rebin_counters[RB_REFUSED];
+	if (!refused) {
+		rc = resizePages(cs, cs->h_rebin_counters[RB_HIGH_WATER] + n, true); // worst case: every entity opens a page
+		if (!rc) rc = growCellMap(cs, cs->h_rebin_counters[RB_N_KEYS], n); // worst case: every entity starts a chain
+	}
+	if (refused || rc) { // the batch changes nothing: its claims are released
+		rebin_add_release_kernel<<<blocks, 256, 0, s>>>(n, dev_entities, max_entity, cs->d_entity_to_slot);
+		LB200_CHECK_LAUNCH(ctx);
+		if (rc) return rc;
+		lb200_set_error(ctx, "add_many_device: %u of %u entities refused (an id added already, listed twice or outside [0, %u], or type 0xff)", refused, n, max_entity);
+		return LB200_ERR_INVALID;
+	}
+	cs->device_authoritative = true;
+	cs->membership_on_device = true;
+	cs->uploaded_since_last_cull = true; // the page arrays change: the next cull must not overlap these kernels
+	rc = placeChangers(cs, dev_entities, dev_pos3, dev_radius, n, true);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaMemcpyAsync(cs->h_rebin_counters, C, sizeof(uint32_t) * RB_ALL_WORDS, cudaMemcpyDeviceToHost, s));
+	LB200_CUDA(ctx, cudaStreamSynchronize(s));
+	rc = checkOverflow(cs);
+	if (rc) return rc;
+	lb::CullingHost& h = cs->host;
+	const uint32_t max_id = cs->h_rebin_counters[RB_MAX_ID];
+	// the pull-back brings the new ids home, and the ids a cull can emit stay inside entity_range (createSortKeys checks it)
+	if (h.entity_to_slot.size() <= max_id) h.entity_to_slot.resize((size_t)max_id + 1, NO_SLOT);
+	applyBatchCounts(cs);
+	return LB200_OK;
+}
+
+int lb200_culling_remove_many_device(lb200_culling* cs, const int32_t* dev_entities, uint32_t n) {
+	if (!cs || !dev_entities) return LB200_ERR_INVALID;
+	if (!cs->ctx) return LB200_ERR_NO_DEVICE;
+	if (n == 0) return LB200_OK;
+	lb200_ctx* ctx = cs->ctx;
+	lb200_range range("culling remove many");
+	int rc = ensureRebinState(cs, 0);
+	if (rc) return rc;
+	cudaStream_t s = ctx->stream;
+	uint32_t* C = cs->d_rebin_counters;
+	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_N_DIRTY, 0, sizeof(uint32_t), s));
+	LB200_CUDA(ctx, cudaMemsetAsync(C + RB_TYPE_DELTA, 0, sizeof(uint32_t) * 256, s));
+	rebin_remove_ids_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, dev_entities, cs->d_entity_to_slot, (uint32_t)cs->d_entity_to_slot.size(), cs->d_page_cell, cs->d_spheres,
+		cs->d_entities, cs->d_page_dirty, cs->d_dirty_pages, C);
+	LB200_CHECK_LAUNCH(ctx);
+	rebin_compact_kernel<<<std::max(1u, std::min((uint32_t)ctx->sm_count * 4u, (n + 255) / 256)), 256, 0, s>>>(cs->d_dirty_pages, C, cs->d_desc, cs->d_page_cell, cs->d_spheres,
+		cs->d_entities, cs->d_entity_to_slot, cs->d_page_dirty, cs->d_free_pages, cs->d_hash_keys, cs->d_hash_vals, (uint32_t)cs->d_hash_keys.size());
+	LB200_CHECK_LAUNCH(ctx);
+	LB200_CUDA(ctx, cudaMemcpyAsync(cs->h_rebin_counters, C, sizeof(uint32_t) * RB_ALL_WORDS, cudaMemcpyDeviceToHost, s));
+	LB200_CUDA(ctx, cudaStreamSynchronize(s));
+	const uint32_t before = cs->host.n_entities;
+	applyBatchCounts(cs);
+	if (cs->host.n_entities != before) { // something was removed: the pages in HBM are ahead of the mirror now
+		cs->device_authoritative = true;
+		cs->membership_on_device = true;
+		cs->uploaded_since_last_cull = true;
+	}
 	return LB200_OK;
 }
 

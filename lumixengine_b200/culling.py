@@ -256,6 +256,16 @@ class CullingSystem:
                                                         C.c_uint32(n - 1 if max_entity is None else max_entity)))
         return int(self.L.lb200_culling_last_rebin_changers(self.h))
 
+    def add_many_device(self, dev_pos3, dev_radius, dev_types, n, dev_entities=None, max_entity=None):
+        """CullingSystem::add for n entities whose spheres (f64[n, 3], f32[n]) and types (u8[n]) lie in device memory (pointers as ints).
+        Ids must lie in [0, max_entity], be new and distinct, types below 0xff; otherwise nothing changes and LumixB200Error is raised."""
+        self._err(self.L.lb200_culling_add_many_device(self.h, vp(dev_entities) if dev_entities else None, vp(dev_types), vp(dev_pos3), vp(dev_radius),
+                                                        C.c_uint32(n), C.c_uint32(n - 1 if max_entity is None else max_entity)))
+
+    def remove_many_device(self, dev_entities, n):
+        """CullingSystem::remove for n entity ids (i32[n]) in device memory; ids that are not added are skipped, duplicates removed once."""
+        self._err(self.L.lb200_culling_remove_many_device(self.h, vp(dev_entities), C.c_uint32(n)))
+
     def sync_host(self):
         self._err(self.L.lb200_culling_sync_host(self.h))
 
