@@ -387,6 +387,20 @@ typedef struct lb200_hierarchy lb200_hierarchy;
 LB200_API int lb200_hierarchy_create(lb200_ctx* ctx, const int32_t* parents, uint32_t n, lb200_hierarchy** out);
 LB200_API void lb200_hierarchy_destroy(lb200_hierarchy* h);
 LB200_API uint32_t lb200_hierarchy_depth(const lb200_hierarchy* h);
+/* World::setParent (world.cpp:619-701) for any number of nodes at once, and nodes entering / leaving: replace the whole parent array.
+ * parents[i] = parent node index, negative = root (as lb200_hierarchy_create); n may differ from the current node count.  The hierarchy then
+ * holds exactly the level order lb200_hierarchy_create(parents, n) builds (roots in ascending index, then level by level each node's
+ * children in ascending index).  Node i < min(old n, n) keeps its local and global transform; nodes >= old n start as the identity.  Locals
+ * are not recomputed: for setParent's keep-the-global behaviour call set_subset, or set_globals + compute_locals, afterwards.  When n changes
+ * the bounding radii are released (the next get_spheres / refresh_spheres must pass them) and the sphere pointers may change.
+ * A parent >= n, a cycle or n = 0 returns LB200_ERR_INVALID (create's error texts) and leaves the hierarchy as it was.
+ * The device form reads the parents from device memory and reads back only the build's counters and the depth + 1 level starts;
+ * max_blocks caps the grid of the cooperative kernels (0 = as many as are co-resident).  Both launch the same kernels at any depth. */
+LB200_API int lb200_hierarchy_set_parents(lb200_hierarchy* h, const int32_t* parents, uint32_t n);
+LB200_API int lb200_hierarchy_set_parents_device(lb200_hierarchy* h, const int32_t* dev_parents, uint32_t n, uint32_t max_blocks);
+/* Introspection: order[k] = node at level position k (n), parent_pos[k] = its parent's level position (n, -1 for roots),
+ * level_start = the first position of every level and n (depth + 1). */
+LB200_API int lb200_hierarchy_get_level_order(lb200_hierarchy* h, uint32_t* order, int32_t* parent_pos, uint32_t* level_start);
 /* World::setLocalTransform for all nodes (world.h:98-123): upload locals (n Transforms, caller's node order). */
 LB200_API int lb200_hierarchy_set_locals(lb200_hierarchy* h, const lb200_transform* locals);
 /* Root world transforms (entries of non-root nodes are ignored). */

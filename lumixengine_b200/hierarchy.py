@@ -43,6 +43,28 @@ class Hierarchy:
     def depth(self):
         return int(self.L.lb200_hierarchy_depth(self.h))
 
+    def setParents(self, parents):
+        """World::setParent for any number of nodes, and nodes entering or leaving: the whole parent array again (len may differ from n).
+        The level order is rebuilt on the device as the constructor builds it; node i < min(old n, new n) keeps its transforms, new nodes
+        start as the identity.  A parent >= n or a cycle raises and leaves the hierarchy as it was."""
+        p = np.ascontiguousarray(parents, np.int32)
+        check(self.L.lb200_hierarchy_set_parents(self.h, ptr(p), C.c_uint32(len(p))), self.ctx.h)
+        self.n = len(p)
+
+    def setParentsDevice(self, dev_parents, n, max_blocks=0):
+        """setParents from n int32 parents in device memory (a device pointer); max_blocks caps the builder's cooperative grid (0 = all
+        co-resident blocks)."""
+        check(self.L.lb200_hierarchy_set_parents_device(self.h, vp(dev_parents), C.c_uint32(n), C.c_uint32(max_blocks)), self.ctx.h)
+        self.n = int(n)
+
+    def levelOrder(self):
+        """(order u32[n]: level position -> node, parent_pos i32[n]: -> the parent's level position or -1, level_start u32[depth + 1])."""
+        order = np.empty(self.n, np.uint32)
+        parent_pos = np.empty(self.n, np.int32)
+        level_start = np.empty(self.depth + 1, np.uint32)
+        check(self.L.lb200_hierarchy_get_level_order(self.h, ptr(order), ptr(parent_pos), ptr(level_start)), self.ctx.h)
+        return order, parent_pos, level_start
+
     def setLocalTransforms(self, locals_):
         a = np.ascontiguousarray(locals_, TRANSFORM_DTYPE)
         assert len(a) == self.n
