@@ -236,6 +236,26 @@ LB200_API uint64_t lb200_culling_last_algorithmic_bytes(const lb200_culling* cs)
 LB200_API int lb200_culling_set_launch(lb200_culling* cs, int blocks, int chunk, int plane_masking);
 LB200_API int lb200_culling_get_launch(lb200_culling* cs, uint32_t* blocks, uint32_t* chunk, uint32_t* rounds, int* pdl, int* plane_masking);
 
+/* Several views of one frame in one pass over the pages (the main camera and the shadow cascades, pipeline.cpp:734-827,1254-1258).
+ * n_views culls of the same scene (1 <= n_views <= LB200_CULL_MAX_VIEWS): view v = frusta[v] with type filter types[v] (types may be
+ * NULL = LB200_TYPE_ALL for every view).  Each view's visible set per type, statistics and mask rows equal those of a lone
+ * lb200_culling_cull_device(frusta[v], types[v]).  Results stay in HBM, one id buffer / counter set / mask per view, owned by the culling
+ * system apart from the output lanes; dev_ids (may be NULL) receives each view's id pointer (per-type segments as in
+ * lb200_culling_cull_device).  want_counts != 0: results[v] filled (may be NULL; one read-back, one synchronisation) and
+ * lb200_culling_last_algorithmic_bytes reports the whole call; 0: fully asynchronous, results may be NULL.
+ * The view buffers stay valid until the next cull_views call; plain culls neither touch them nor are touched by them.  n_views = 1 runs
+ * the single cull kernel; two or more run one fused kernel, whose pages per block per round are at most
+ * min(256, 512 / n_views) (a larger chunk forced by lb200_culling_set_launch is capped; lb200_culling_get_launch reports the launch).
+ * With no entity added every result is zero and nothing is launched.  Exchange mode is not part of this call. */
+#define LB200_CULL_MAX_VIEWS 8
+LB200_API int lb200_culling_cull_views(lb200_culling* cs, const lb200_shifted_frustum* frusta, const uint8_t* types, uint32_t n_views,
+                                       const uint32_t** dev_ids, lb200_cull_result* results, int want_counts);
+/* Make view k of the latest cull_views call "the last cull" for lb200_culling_last_result, lb200_culling_read_bitmask and
+ * lb200_sortkeys_create_keys, with the per-type segment bases that view was culled with.  Any time after that call, plain culls in between
+ * included.  LB200_ERR_INVALID for k >= its n_views; LB200_ERR_STATE if no cull_views was issued, if it culled an empty system, or if the
+ * view buffers were released since (a growth of the page arrays, lb200_culling_set_replicas). */
+LB200_API int lb200_culling_select_view(lb200_culling* cs, uint32_t k);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Sort keys — the consumer of the visible list (SURVEY.md 8f N1): PipelineImpl::createSortKeys (src/renderer/pipeline.cpp:3789-4018:
  * LOD selection + smoothing, sort keys / values :53-143, auto-instancing :452-523 and its instance data :3958-4016) and

@@ -94,7 +94,7 @@ SYMBOLS = [
     "lb200_culling_page_count", "lb200_culling_entity_count", "lb200_culling_get_page",
     "lb200_culling_cull", "lb200_culling_cull_begin", "lb200_culling_cull_poll", "lb200_culling_cull_end", "lb200_culling_cull_device", "lb200_culling_cull_device_n", "lb200_culling_last_result", "lb200_culling_flush", "lb200_culling_read_bitmask", "lb200_culling_set_replicas",
     "lb200_culling_last_algorithmic_bytes", "lb200_culling_time_lone_cull", "lb200_culling_set_launch", "lb200_culling_get_launch", "lb200_culling_set_many_device", "lb200_culling_sync_host", "lb200_culling_last_rebin_changers",
-    "lb200_culling_add_many_device", "lb200_culling_remove_many_device",
+    "lb200_culling_add_many_device", "lb200_culling_remove_many_device", "lb200_culling_cull_views", "lb200_culling_select_view",
     "lb200_comm_get_unique_id", "lb200_comm_init", "lb200_comm_destroy", "lb200_comm_enable_p2p", "lb200_comm_status", "lb200_culling_gather_stride_words", "lb200_culling_allgather", "lb200_culling_cull_gather",
     "lb200_culling_cull_exchange", "lb200_culling_cull_exchange_n", "lb200_culling_exchange_slab_words", "lb200_culling_page_id",
     "lb200_sortkeys_create", "lb200_sortkeys_destroy", "lb200_sortkeys_set_models", "lb200_sortkeys_set_instances", "lb200_sortkeys_set_transforms",

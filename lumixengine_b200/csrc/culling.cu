@@ -7,7 +7,8 @@
 //   culling_exchange.cu  the multi-GPU exchange: all-gather of visible ids, NVLink push, bitmask exchange steps
 //   culling_rebin.cu     device re-binning (set_many_device), device adds / removes (add_many_device, remove_many_device) and the
 //                        pull-back of the host mirror
-//   culling_internal.h   struct lb200_culling, the counter and slab layout, and the functions the three share
+//   culling_views.cu     several views in one pass (cull_views, select_view): cull_views_kernel.cuh, or this file's launchCull for one view
+//   culling_internal.h   struct lb200_culling, the counter and slab layout, and the functions the four share
 #include "cull_kernel.cuh"
 #include "culling_internal.h"
 #include "lb200_math.cuh"
@@ -134,6 +135,7 @@ int resizePages(lb200_culling* cs, uint32_t min_pages, bool keep) {
 	if (min_pages <= cs->dev_cap) return LB200_OK;
 	const uint32_t cap = (uint32_t)grownCapacity(cs->dev_cap, 1024, min_pages);
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	releaseViews(cs);
 	if (!keep) {
 		cs->d_spheres.reset(); cs->d_entities.reset(); cs->d_desc.reset(); cs->d_mask.reset(); // before the new ones are allocated
 		cs->d_page_cell.reset(); cs->d_free_pages.reset(); cs->d_page_dirty.reset(); cs->d_dirty_pages.reset();
@@ -245,7 +247,7 @@ int flushPages(lb200_culling* cs) {
 	return LB200_OK;
 }
 
-int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg, cudaStream_t stream) {
+int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg, cudaStream_t stream, const CullOutput* dest) {
 	lb200_range range("culling"); // culling_system.cpp:330
 	lb200_ctx* ctx = cs->ctx;
 	lb::CullingHost& h = cs->host;
@@ -267,7 +269,7 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 	P.item_cap = cs->item_cap;
 	uint32_t acc = 0;
 	for (int t = 0; t < 256; ++t) { P.type_base[t] = acc; acc += h.type_counts[t]; }
-	memcpy(cs->last_type_base, P.type_base, sizeof(P.type_base));
+	memcpy(dest ? dest->type_base : cs->last_type_base, P.type_base, sizeof(P.type_base));
 
 	const uint32_t r = cs->next_replica;
 	cs->next_replica = (cs->next_replica + 1) % cs->replicas;
@@ -277,6 +279,7 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 	uint32_t* nxt = cs->d_counters + ((size_t)lane * 2 + (cs->lane_parity[lane] ^ 1u)) * COUNTER_WORDS;
 	uint32_t* out = cs->d_out_ids + (size_t)lane * (cs->d_out_ids.size() / cs->lanes);
 	uint32_t* mask = cs->d_mask + (size_t)lane * (cs->d_mask.size() / cs->lanes);
+	if (dest) { cur = dest->counters; nxt = dest->next_counters; out = dest->ids; mask = dest->mask; }
 	P.n_buffers = 1;
 	if (xchg) {
 		P.n_ranks = (uint32_t)ctx->n_ranks;
@@ -310,10 +313,13 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 	LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, cull_pages_kernel, P, (const lb200_page_desc*)(cs->d_desc + off), (const float4*)(cs->d_spheres + off * PAGE_SLOTS),
 		(const int*)(cs->d_entities + off * PAGE_SLOTS), out, cur, nxt, mask_arg));
 	LB200_CHECK_LAUNCH(ctx);
-	cs->last_counters = cur; cs->last_out = out; cs->last_mask = mask_arg; // exchange culls keep their rows in the slabs
-	cs->lane_parity[lane] ^= 1u;
-	if (!xchg) ++cs->seq;
-	cs->last_pages = n_pages;
+	if (!dest) {
+		cs->last_counters = cur; cs->last_out = out; cs->last_mask = mask_arg; // exchange culls keep their rows in the slabs
+		cs->last_is_view = false;
+		cs->lane_parity[lane] ^= 1u;
+		if (!xchg) ++cs->seq;
+		cs->last_pages = n_pages;
+	}
 	cs->last_blocks = blocks; cs->last_chunk = chunk; cs->last_rounds = (uint32_t)((n_pages + (uint64_t)blocks * chunk - 1) / ((uint64_t)blocks * chunk));
 	cs->last_pdl = pdl ? 1 : 0; cs->last_plane_masking = (int)P.plane_masking;
 	return LB200_OK;
@@ -345,6 +351,22 @@ int joinLanes(lb200_culling* cs) {
 	return LB200_OK;
 }
 
+void fillResult(const lb200_culling* cs, const uint32_t* counters, const uint32_t* type_base, lb200_cull_result* res) {
+	memset(res, 0, sizeof(*res));
+	for (int t = 0; t < 256; ++t) {
+		res->type_count[t] = counters[t];
+		res->type_offset[t] = type_base[t];
+		res->total += res->type_count[t];
+		if (cs->host.type_counts[t]) res->n_types = t + 1;
+	}
+	res->pages_tested = counters[256 + ST_PAGES_TESTED];
+	res->pages_inside = counters[256 + ST_PAGES_INSIDE];
+	res->pages_outside = counters[256 + ST_PAGES_OUTSIDE];
+	res->pages_filtered = counters[256 + ST_PAGES_FILTERED];
+	res->entities_tested = counters[256 + ST_ENT_TESTED];
+	res->entities_inside = counters[256 + ST_ENT_INSIDE];
+}
+
 int launchPack(lb200_culling* cs, const uint32_t* counters, uint32_t capacity, uint32_t* ids_dst, uint32_t* counters_dst, uint32_t counter_words, int blocks) {
 	lb200_ctx* ctx = cs->ctx;
 	PackParams PP;
@@ -362,19 +384,7 @@ namespace {
 // h_counters (already on the host) -> cs->last / *result
 void parseCounts(lb200_culling* cs, lb200_cull_result* result) {
 	lb200_cull_result& res = cs->last;
-	memset(&res, 0, sizeof(res));
-	for (int t = 0; t < 256; ++t) {
-		res.type_count[t] = cs->h_counters[t];
-		res.type_offset[t] = cs->last_type_base[t];
-		res.total += res.type_count[t];
-		if (cs->host.type_counts[t]) res.n_types = t + 1;
-	}
-	res.pages_tested = cs->h_counters[256 + ST_PAGES_TESTED];
-	res.pages_inside = cs->h_counters[256 + ST_PAGES_INSIDE];
-	res.pages_outside = cs->h_counters[256 + ST_PAGES_OUTSIDE];
-	res.pages_filtered = cs->h_counters[256 + ST_PAGES_FILTERED];
-	res.entities_tested = cs->h_counters[256 + ST_ENT_TESTED];
-	res.entities_inside = cs->h_counters[256 + ST_ENT_INSIDE];
+	fillResult(cs, cs->h_counters, cs->last_type_base, &res);
 	cs->has_last = true;
 	// DESIGN.md §4.1: descriptor per page + 16 B per sphere the kernel reads (pages left to test after plane masking) + (4 B id read +
 	// 4 B id write) per visible + 32 B mask per page
@@ -564,6 +574,7 @@ int lb200_culling_set_replicas(lb200_culling* cs, uint32_t replicas) {
 	if (!cs->ctx) return LB200_ERR_NO_DEVICE;
 	if (replicas == cs->replicas) return LB200_OK;
 	LB200_CUDA(cs->ctx, cudaStreamSynchronize(cs->ctx->stream));
+	releaseViews(cs);
 	cs->replicas = replicas;
 	cs->next_replica = 0;
 	cs->dev_cap = 0; // forces reallocation + full upload at the next flush (resizePages, discarding)

@@ -119,6 +119,23 @@ struct lb200_culling {
 	DeviceArray<uint64_t> d_rb_keys[2], d_rb_vals[2];
 	uint32_t dev_high_water = 0;        // pages [0, dev_high_water) may be in use on the device
 
+	// ---- several views in one pass (lb200_culling_cull_views, culling_views.cu) ----
+	// The latest call's results: view v's ids at d_view_ids + v * view_id_cap, its rows at d_view_mask + v * 8 * dev_cap, its counters in
+	// one of two counter blocks (a call zeroes the other one for the next call).  The fused kernel and the single kernel (n_views = 1)
+	// keep separate counter blocks, each with its own parity, because each zeroes only the layout it writes.
+	DeviceArray<uint32_t> d_view_ids;
+	DeviceArray<uint32_t> d_view_mask;       // released with the page arrays (resizePages) and by set_replicas
+	DeviceArray<uint32_t> d_view_counters;   // [2][CALL_COUNTER_WORDS] for the fused kernel, then [2][COUNTER_WORDS] for n_views = 1
+	PinnedArray<uint32_t> h_view_counters;   // CALL_COUNTER_WORDS
+	uint32_t view_id_cap = 0;
+	uint8_t view_parity[2] = {};             // fused, single
+	uint32_t views_n = 0;                    // n_views of the latest call, 0 = none issued
+	bool views_live = false;                 // the view buffers hold that call's results
+	uint32_t* views_counters = nullptr;      // counters of that call's view 0; view v's at + v * COUNTER_WORDS
+	uint32_t views_pages = 0;
+	uint32_t views_type_base[256];
+	bool last_is_view = false;               // the "last cull" below is a view selected by lb200_culling_select_view
+
 	uint32_t last_type_base[256];
 	lb200_cull_result last = {};
 	bool has_last = false;
@@ -131,11 +148,19 @@ namespace lbcull {
 // non-null: store {page, row} records + counts into every rank's slab (peer memory); lane = epoch % lanes; pub / wait: fused steps (cull_kernel.cuh)
 struct Exchange { uint32_t epoch; uint32_t pub_epoch = 0, wait_epoch = 0; };
 
+// non-null: the cull writes here instead of into a lane, and leaves the lanes, the sequence and "the last cull" as they are
+struct CullOutput { uint32_t* ids; uint32_t* counters; uint32_t* next_counters; uint32_t* mask; uint32_t* type_base; };
+
 // culling.cu
 int ensureDevice(lb200_culling* cs);
 int flushPages(lb200_culling* cs);
 int resizePages(lb200_culling* cs, uint32_t min_pages, bool keep); // the one owner of the page arrays' size
-int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg = nullptr, cudaStream_t stream = nullptr);
+int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg = nullptr, cudaStream_t stream = nullptr,
+	const CullOutput* out = nullptr);
+// counters of one cull (on the host) and the type bases it was culled with -> *res
+void fillResult(const lb200_culling* cs, const uint32_t* counters, const uint32_t* type_base, lb200_cull_result* res);
+// culling_views.cu: drop the results of the latest cull_views call (their masks are sized by the page arrays); the stream is idle
+void releaseViews(lb200_culling* cs);
 int forkLanes(lb200_culling* cs);
 int joinLanes(lb200_culling* cs);
 // pack_kernel on the context stream: ids of the cull with these counters into ids_dst (at most `capacity`), counters[0, counter_words) into counters_dst

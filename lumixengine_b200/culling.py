@@ -231,6 +231,29 @@ class CullingSystem:
         """n independent asynchronous culls issued from C: consecutive ones run on different streams / output lanes and overlap."""
         self._err(self.L.lb200_culling_cull_device_n(self.h, C.byref(frustum), C.c_uint8(type), C.c_uint32(n)))
 
+    def cull_views(self, frusta, types=None, want_counts=True):
+        """Several views of the same scene culled in one pass over the pages (lb200_culling_cull_views): a frame's main camera and its shadow
+        cascades.  frusta: 1..8 ShiftedFrustum; types: None (every view culls all types) or one type filter per view (0xff = all).  Returns
+        [(device ids pointer, lb200_cull_result or None)] per view, each equal to a lone cull_device of that view.  The results stay valid
+        until the next cull_views call; select_view(k) makes view k the last cull."""
+        frusta = list(frusta)
+        n = len(frusta)
+        arr = (ShiftedFrustum * max(n, 1))(*frusta)
+        ty = None
+        if types is not None:
+            ty = np.ascontiguousarray(types, np.uint8)
+            if len(ty) != n:
+                raise ValueError(f"{len(ty)} type filters for {n} views")
+        dev = (vp * max(n, 1))()
+        res = (_lib.CullResult * max(n, 1))()
+        self._err(self.L.lb200_culling_cull_views(self.h, arr if n else None, ptr(ty), C.c_uint32(n), dev, res if want_counts else None,
+                                                  C.c_int(1 if want_counts else 0)))
+        return [((dev[v] or 0), (res[v] if want_counts else None)) for v in range(n)]
+
+    def select_view(self, k):
+        """Make view k of the latest cull_views call the last cull (last_result, read_bitmask, SortKeys.createSortKeys)."""
+        self._err(self.L.lb200_culling_select_view(self.h, C.c_uint32(k)))
+
     def last_result(self):
         """(device ids pointer, lb200_cull_result) of the cull issued last (e.g. the last one of cull_device_n)."""
         dev = vp()

@@ -46,6 +46,45 @@ def c2_frustum_args():
     return a
 
 
+SHADOW_CAM_FAR = 500.0  # pipeline.cpp:270
+DEFAULT_CASCADES = (3.0, 10.0, 60.0, 150.0)  # pipeline.cpp:741, without an environment light
+
+
+def shadow_cascade_args(camera, light_dir, cascades=DEFAULT_CASCADES):
+    """Ortho frustum arguments (lb200_frustum_ortho) of the four shadow cascades PipelineImpl::prepareShadowCameras derives for a
+    perspective camera given as c1_frustum_args() (pipeline.cpp:734-827): slice i covers the camera's depth range between split
+    distances i and i + 1 of (0.1, *cascades); its bounding sphere (Frustum::computeBoundingSphere, geometry.cpp:231-249) sets the size
+    bb; the slice's corners projected on xvec / yvec set the ortho size and centre; the camera sits SHADOW_CAM_FAR - 2 bb back along
+    the light and sees 0 .. SHADOW_CAM_FAR + 2 bb.  A numpy restatement in float64, for test and timing inputs."""
+    unit = lambda v: np.asarray(v, np.float64) / np.linalg.norm(v)  # noqa: E731
+    pos = np.asarray(camera["position"], np.float64)
+    view_dir, up = unit(camera["direction"]), unit(camera["up"])
+    right = unit(np.cross(view_dir, up))
+    up = np.cross(right, view_dir)
+    light = unit(light_dir)
+    xvec = unit(np.cross(light, view_dir))
+    yvec = unit(np.cross(light, xvec))
+    splits = (0.1,) + tuple(float(c) for c in cascades)
+    tan_half = np.tan(camera["fov"] * 0.5)
+    out = []
+    for s in range(4):
+        pts = []
+        for dist in (splits[s], splits[s + 1]):
+            hh = tan_half * dist
+            hw = hh * camera["ratio"]
+            for sx in (-1.0, 1.0):
+                for sy in (-1.0, 1.0):
+                    pts.append(view_dir * dist + right * sx * hw + up * sy * hh)
+        pts = np.array(pts)
+        bb = float(np.linalg.norm(pts - pts.mean(0), axis=1).max())
+        px, py = pts @ xvec, pts @ yvec
+        ortho = max(px.max() - px.min(), py.max() - py.min()) * 0.5
+        cam = xvec * (px.max() + px.min()) * 0.5 + yvec * (py.max() + py.min()) * 0.5 - light * (SHADOW_CAM_FAR - 2.0 * bb)
+        out.append(dict(position=tuple(pos + cam), direction=tuple(light), up=tuple(yvec), width=float(ortho), height=float(ortho), near=0.0,
+                        far=SHADOW_CAM_FAR + 2.0 * bb))
+    return out
+
+
 def random_unit_quats(rng, n):
     q = rng.normal(size=(n, 4)).astype(np.float32)
     q /= np.linalg.norm(q, axis=1, keepdims=True).astype(np.float32)
