@@ -205,7 +205,12 @@ LB200_API int lb200_culling_set_replicas(lb200_culling* cs, uint32_t replicas);
  * dev_entities: n entity ids in device memory, or NULL for the identity (mover i = entity i); max_entity: largest entity id that can appear.
  * The host mirror is refreshed lazily: the next host-side accessor / mutator (add, remove, set*, get_page, ...) pulls the device state back
  * first (or call lb200_culling_sync_host).  Visible sets of later culls are the reference's; slots / pages inside a chain may differ from
- * a sequential replay of the same edits (as they do between two edit orders).  Needs set_replicas(1). */
+ * a sequential replay of the same edits (as they do between two edit orders).  Needs set_replicas(1).
+ * Cell range: the device keys a chain by 18 bits per cell axis, so it holds cells [-131072, 131071] on every axis (about +-39 321 km).  A
+ * batch that computes a cell outside that range, and every device edit while the host holds such a chain, is applied by the host
+ * bookkeeping instead (device state pulled back, batch copied to the host): same results, host speed.  The same holds for
+ * lb200_culling_add_many_device and lb200_culling_remove_many_device.  lb200_culling_last_rebin_changers: the movers of the last
+ * batch whose cell or big-ness changed. */
 LB200_API int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities, const double* dev_pos3, const float* dev_radius, uint32_t n, uint32_t max_entity);
 LB200_API int lb200_culling_sync_host(lb200_culling* cs);
 LB200_API uint32_t lb200_culling_last_rebin_changers(const lb200_culling* cs);

@@ -20,6 +20,9 @@
 // Both keep per-type count deltas, which the batch's last read-back applies to the host's type counts (the cull's output layout).
 // The chain hash map counts its keys and is rehashed on the device into a larger table before a batch could fill it past half.
 // The pull-back of the host mirror (syncHostFromDevice) lives here too: it undoes what these kernels leave ahead of the host.
+// The device keys a chain by 18 bits per cell axis, so it holds only cells in [-131 072, 131 071] (about +-39 321 km).  A batch that
+// computes a cell outside that range, and any batch while the host mirror holds such a chain, is applied by the host bookkeeping instead:
+// the device never holds two chains whose packed keys alias.
 // =====================================================================================================================================
 #include "culling_internal.h"
 
@@ -30,13 +33,14 @@ using namespace lbcull;
 
 namespace {
 
-// counter words: [0, RB_WORDS) the state every batch reads back (RB_OVERFLOW holds OVERFLOW_PAGES | OVERFLOW_HASH), then the words of an
+// counter words: [0, RB_WORDS) the state every batch reads back (RB_OVERFLOW holds OVERFLOW_PAGES | OVERFLOW_HASH | OVERFLOW_RANGE), then the words of an
 // add batch's first read-back, then RB_TYPE_DELTA: 256 per-type count deltas of an add / remove batch (two's complement).  The batch
 // words are zeroed by the batch that uses them.
 enum { RB_HIGH_WATER = 0, RB_N_FREE, RB_N_CHANGERS, RB_N_DIRTY, RB_OVERFLOW, RB_BAD_RADIUS, RB_N_KEYS, RB_NEW_PAGES, RB_WORDS,
 	RB_REFUSED = RB_WORDS, RB_MAX_ID, RB_ADD_WORDS = RB_WORDS + 8 };
 constexpr uint32_t RB_TYPE_DELTA = RB_ADD_WORDS, RB_ALL_WORDS = RB_ADD_WORDS + 256;
-constexpr uint32_t OVERFLOW_PAGES = 1u, OVERFLOW_HASH = 2u;
+// OVERFLOW_RANGE: a batch computed a cell the packed key cannot hold; it is applied on the host, and the next batch rebuilds the counters
+constexpr uint32_t OVERFLOW_PAGES = 1u, OVERFLOW_HASH = 2u, OVERFLOW_RANGE = 4u;
 constexpr unsigned long long HASH_EMPTY = ~0ull;
 constexpr uint32_t NO_OPEN_PAGE = 0xffffffffu;
 constexpr uint32_t CLAIMED = 0xfffffffeu; // entity -> slot of an id an add batch has claimed and not placed yet (no page reaches it)
@@ -45,6 +49,10 @@ __host__ __device__ __forceinline__ unsigned long long packCellKey(int x, int y,
 	// 18 bits per axis (+-131 071 cells of 300 m), 8 bits type, 1 bit is_big
 	return ((unsigned long long)((uint32_t)x & 0x3ffffu)) | ((unsigned long long)((uint32_t)y & 0x3ffffu) << 18) | ((unsigned long long)((uint32_t)z & 0x3ffffu) << 36)
 		| ((unsigned long long)(type & 0xffu) << 54) | ((unsigned long long)(is_big & 1u) << 62);
+}
+// the cells packCellKey keeps apart: [-131 072, 131 071] on every axis
+__host__ __device__ __forceinline__ bool cellInKeyRange(int x, int y, int z) {
+	return (uint32_t)(x + 0x20000) < 0x40000u && (uint32_t)(y + 0x20000) < 0x40000u && (uint32_t)(z + 0x20000) < 0x40000u;
 }
 __host__ __device__ __forceinline__ uint32_t hashCellKey(unsigned long long k) {
 	k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
@@ -98,6 +106,7 @@ __global__ void __launch_bounds__(256) rebin_classify_kernel(uint32_t n, const i
 			const float r = radius[i];
 			const double inv = (double)(1 / LB200_CELL_SIZE); // culling_system.cpp:25-31: IVec3(pos * (1 / cell_size)), DVec3 * float
 			const int ix = (int)__dmul_rn(px, inv), iy = (int)__dmul_rn(py, inv), iz = (int)__dmul_rn(pz, inv);
+			if (!cellInKeyRange(ix, iy, iz)) atomicOr(&counters[RB_OVERFLOW], OVERFLOW_RANGE); // the batch goes to the host after the read-back
 			const int4 c = page_cell[page];
 			const bool was_big = ((uint32_t)c.w >> 8) != 0, is_big = r > LB200_CELL_SIZE;
 			if (was_big == is_big && ix == c.x && iy == c.y && iz == c.z) { // :228-233
@@ -211,6 +220,9 @@ __global__ void __launch_bounds__(256) rebin_add_claim_kernel(uint32_t n, const 
 		int ix;
 		keys[i] = chainKey(pos3, i, type, radius[i], &ix);
 		vals[i] = ((uint64_t)(uint32_t)ix) | ((uint64_t)i << 32);
+		const double inv = (double)(1 / LB200_CELL_SIZE);
+		if (!cellInKeyRange(ix, (int)__dmul_rn(pos3[3 * (size_t)i + 1], inv), (int)__dmul_rn(pos3[3 * (size_t)i + 2], inv)))
+			atomicOr(&counters[RB_OVERFLOW], OVERFLOW_RANGE); // the batch releases its claims and goes to the host
 	}
 	if (i == 0) counters[RB_N_CHANGERS] = n; // step 3 places every entity of an accepted batch
 	__syncthreads();
@@ -363,7 +375,11 @@ __global__ void __launch_bounds__(256) rebin_place_kernel(const uint64_t* __rest
 	}
 }
 
-// device-side tables for the re-binning, (re)built from the host mirror whenever it was edited since
+// ensureRebinState's answer when the host mirror holds a chain whose cell packCellKey cannot hold: the batch goes to the host bookkeeping
+constexpr int REBIN_ON_HOST = 1;
+
+// device-side tables for the re-binning, (re)built from the host mirror whenever it was edited since; REBIN_ON_HOST instead of a build
+// from a mirror with a chain outside the packed key's range (the device never holds one)
 int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	lb200_ctx* ctx = cs->ctx;
 	lb::CullingHost& h = cs->host;
@@ -404,6 +420,7 @@ int ensureRebinState(lb200_culling* cs, uint32_t max_entity) {
 	if (cs->rebin_built_gen == h.edit_gen && !cs->device_authoritative) return LB200_OK;
 	if (cs->device_authoritative) return LB200_OK; // the tables are live on the device
 	// ---- build from the host mirror ----
+	for (const auto& kv : h.cell_map) if (!cellInKeyRange(kv.first.x, kv.first.y, kv.first.z)) return REBIN_ON_HOST;
 	const uint32_t n_pages = h.high_water;
 	std::vector<int4> cells(n_pages);
 	for (uint32_t p = 0; p < n_pages; ++p) cells[p] = make_int4(h.keys[p].x, h.keys[p].y, h.keys[p].z, (int)(h.keys[p].type | ((uint32_t)h.keys[p].is_big << 8)));
@@ -530,6 +547,93 @@ void applyBatchCounts(lb200_culling* cs) {
 	cs->dev_high_water = cs->h_rebin_counters[RB_HIGH_WATER];
 }
 
+// ---- batches with a cell outside the packed key's range: the host bookkeeping applies them ----
+
+// the range flag belongs to the batch that raised it (the page and hash flags stay: their batch failed)
+int clearRangeOverflow(lb200_culling* cs) {
+	cs->h_rebin_counters[RB_OVERFLOW] &= ~OVERFLOW_RANGE;
+	LB200_CUDA(cs->ctx, cudaMemcpyAsync(cs->d_rebin_counters + RB_OVERFLOW, cs->h_rebin_counters + RB_OVERFLOW, sizeof(uint32_t), cudaMemcpyHostToDevice, cs->ctx->stream));
+	return LB200_OK;
+}
+
+template <class T> int copyBatch(lb200_ctx* ctx, std::vector<T>& out, const T* dev, size_t n) {
+	out.resize(n);
+	LB200_CUDA(ctx, cudaMemcpyAsync(out.data(), dev, sizeof(T) * n, cudaMemcpyDeviceToHost, ctx->stream));
+	return LB200_OK;
+}
+
+// set_many_device: CullingHost::set for every added mover (ids that are not added are skipped, as the classify kernel skips them), after
+// the pull-back (which brings the classify kernel's in-place writes home; set() writes them again).  The changer count
+// lb200_culling_last_rebin_changers reports is the classify kernel's: movers whose cell or big-ness changes.
+int setOnHost(lb200_culling* cs, const int32_t* dev_entities, const double* dev_pos3, const float* dev_radius, uint32_t n) {
+	lb200_ctx* ctx = cs->ctx;
+	int rc = syncHostFromDevice(cs);
+	std::vector<int32_t> ents; std::vector<double> pos; std::vector<float> rad;
+	if (!rc && dev_entities) rc = copyBatch(ctx, ents, dev_entities, n);
+	if (!rc) rc = copyBatch(ctx, pos, dev_pos3, 3 * (size_t)n);
+	if (!rc) rc = copyBatch(ctx, rad, dev_radius, n);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	lb::CullingHost& h = cs->host;
+	uint32_t changers = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		const int32_t e = dev_entities ? ents[i] : (int32_t)i;
+		if (!h.isAdded(e)) continue;
+		const uint32_t page = h.entity_to_slot[e] / PAGE_SLOTS;
+		const double* p = pos.data() + 3 * (size_t)i;
+		if (!lb::CullingHost::sameCell(lb::CullingHost::makeKey(p, 0, false), h.keys[page]) || (h.desc[page].is_big != 0) != (rad[i] > LB200_CELL_SIZE)) ++changers;
+		rc = h.set(e, p, rad[i]);
+		if (rc) return rc;
+	}
+	cs->h_rebin_counters[RB_N_CHANGERS] = changers;
+	return LB200_OK;
+}
+
+// add_many_device: the batch is refused whole for the same ids and types the claim kernel refuses; otherwise CullingHost::add for each
+int addOnHost(lb200_culling* cs, const int32_t* dev_entities, const uint8_t* dev_types, const double* dev_pos3, const float* dev_radius, uint32_t n,
+	uint32_t max_entity)
+{
+	lb200_ctx* ctx = cs->ctx;
+	int rc = syncHostFromDevice(cs);
+	std::vector<int32_t> ents; std::vector<uint8_t> types; std::vector<double> pos; std::vector<float> rad;
+	if (!rc && dev_entities) rc = copyBatch(ctx, ents, dev_entities, n);
+	if (!rc) rc = copyBatch(ctx, types, dev_types, n);
+	if (!rc) rc = copyBatch(ctx, pos, dev_pos3, 3 * (size_t)n);
+	if (!rc) rc = copyBatch(ctx, rad, dev_radius, n);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	lb::CullingHost& h = cs->host;
+	if (!dev_entities) { ents.resize(n); for (uint32_t i = 0; i < n; ++i) ents[i] = (int32_t)i; }
+	std::vector<int32_t> sorted(ents);
+	std::sort(sorted.begin(), sorted.end());
+	uint32_t refused = 0;
+	for (uint32_t i = 0; i < n; ++i) {
+		const int32_t e = ents[i];
+		if (e < 0 || (uint32_t)e > max_entity || types[i] == LB200_TYPE_ALL || h.isAdded(e) || (i && sorted[i] == sorted[i - 1])) ++refused;
+	}
+	if (refused) {
+		lb200_set_error(ctx, "add_many_device: %u of %u entities refused (an id added already, listed twice or outside [0, %u], or type 0xff)", refused, n, max_entity);
+		return LB200_ERR_INVALID;
+	}
+	for (uint32_t i = 0; i < n; ++i) {
+		rc = h.add(ents[i], types[i], pos.data() + 3 * (size_t)i, rad[i]);
+		if (rc) return rc;
+	}
+	return LB200_OK;
+}
+
+// remove_many_device: CullingHost::remove for every id (ids that are not added, and repeats, are skipped there)
+int removeOnHost(lb200_culling* cs, const int32_t* dev_entities, uint32_t n) {
+	lb200_ctx* ctx = cs->ctx;
+	int rc = syncHostFromDevice(cs);
+	std::vector<int32_t> ents;
+	if (!rc) rc = copyBatch(ctx, ents, dev_entities, n);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	for (uint32_t i = 0; i < n; ++i) cs->host.remove(ents[i]);
+	return LB200_OK;
+}
+
 } // namespace
 
 // pull the device state back into the host mirror (page arrays, counts, entity -> slot, chains regrouped by key with the open page as head)
@@ -598,6 +702,7 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 	lb200_ctx* ctx = cs->ctx;
 	lb200_range range("culling set many");
 	int rc = ensureRebinState(cs, max_entity);
+	if (rc == REBIN_ON_HOST) return setOnHost(cs, dev_entities, dev_pos3, dev_radius, n);
 	if (rc) return rc;
 	rc = ensureChangerBuffers(cs, n);
 	if (rc) return rc;
@@ -612,6 +717,10 @@ int lb200_culling_set_many_device(lb200_culling* cs, const int32_t* dev_entities
 	const uint32_t n_changers = cs->h_rebin_counters[RB_N_CHANGERS];
 	cs->device_authoritative = true;
 	cs->uploaded_since_last_cull = true; // the page arrays changed: the next cull must not overlap these kernels
+	if (cs->h_rebin_counters[RB_OVERFLOW] & OVERFLOW_RANGE) { // a mover's cell lies outside the packed key's range
+		rc = clearRangeOverflow(cs);
+		return rc ? rc : setOnHost(cs, dev_entities, dev_pos3, dev_radius, n);
+	}
 	if (n_changers) {
 		rc = resizePages(cs, cs->h_rebin_counters[RB_HIGH_WATER] + n_changers, true); // worst case: every changer opens a page
 		if (rc) return rc;
@@ -646,6 +755,7 @@ int lb200_culling_add_many_device(lb200_culling* cs, const int32_t* dev_entities
 	if (max_entity > (uint32_t)INT32_MAX) { lb200_set_error(ctx, "add_many_device: max_entity %u is not an entity id", max_entity); return LB200_ERR_INVALID; }
 	lb200_range range("culling add many");
 	int rc = ensureRebinState(cs, max_entity);
+	if (rc == REBIN_ON_HOST) return addOnHost(cs, dev_entities, dev_types, dev_pos3, dev_radius, n, max_entity);
 	if (rc) return rc;
 	rc = ensureChangerBuffers(cs, n);
 	if (rc) return rc;
@@ -660,14 +770,18 @@ int lb200_culling_add_many_device(lb200_culling* cs, const int32_t* dev_entities
 	LB200_CUDA(ctx, cudaMemcpyAsync(cs->h_rebin_counters, C, sizeof(uint32_t) * RB_ADD_WORDS, cudaMemcpyDeviceToHost, s));
 	LB200_CUDA(ctx, cudaStreamSynchronize(s));
 	const uint32_t refused = cs->h_rebin_counters[RB_REFUSED];
-	if (!refused) {
+	const bool out_of_range = (cs->h_rebin_counters[RB_OVERFLOW] & OVERFLOW_RANGE) != 0; // a cell the packed key cannot hold
+	if (!refused && !out_of_range) {
 		rc = resizePages(cs, cs->h_rebin_counters[RB_HIGH_WATER] + n, true); // worst case: every entity opens a page
 		if (!rc) rc = growCellMap(cs, cs->h_rebin_counters[RB_N_KEYS], n); // worst case: every entity starts a chain
 	}
-	if (refused || rc) { // the batch changes nothing: its claims are released
+	if (refused || out_of_range || rc) { // the device changes nothing: the batch's claims are released
 		rebin_add_release_kernel<<<blocks, 256, 0, s>>>(n, dev_entities, max_entity, cs->d_entity_to_slot);
 		LB200_CHECK_LAUNCH(ctx);
 		if (rc) return rc;
+		if (out_of_range) rc = clearRangeOverflow(cs);
+		if (rc) return rc;
+		if (out_of_range && !refused) return addOnHost(cs, dev_entities, dev_types, dev_pos3, dev_radius, n, max_entity);
 		lb200_set_error(ctx, "add_many_device: %u of %u entities refused (an id added already, listed twice or outside [0, %u], or type 0xff)", refused, n, max_entity);
 		return LB200_ERR_INVALID;
 	}
@@ -695,6 +809,7 @@ int lb200_culling_remove_many_device(lb200_culling* cs, const int32_t* dev_entit
 	lb200_ctx* ctx = cs->ctx;
 	lb200_range range("culling remove many");
 	int rc = ensureRebinState(cs, 0);
+	if (rc == REBIN_ON_HOST) return removeOnHost(cs, dev_entities, n);
 	if (rc) return rc;
 	cudaStream_t s = ctx->stream;
 	uint32_t* C = cs->d_rebin_counters;
