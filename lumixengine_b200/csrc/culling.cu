@@ -1,7 +1,8 @@
 // GPU CullingSystem: host side + C-ABI (include/lumix_b200.h "CullingSystem").
 //
 // Replaces CullingSystemImpl::cullInternal + doCulling (src/renderer/culling_system.cpp:260-369).  The cull itself is one kernel,
-// cull_pages_kernel (cull_kernel.cuh, which describes its phases, included here and nowhere else).  The culling system's sources:
+// cull_pages_kernel (cull_kernel.cuh, which describes its phases, included here and nowhere else; its culling core, cull_common.cuh, is
+// shared with cull_views_kernel).  The culling system's sources:
 //   culling.cu           the host-edit C API, the page upload (ensureDevice, resizePages, flushPages), the cull launch and its lanes,
 //                        the delivery of results to the caller (cull, begin / poll / end, cull_device[_n], read_bitmask, time_lone_cull)
 //   culling_exchange.cu  the multi-GPU exchange: all-gather of visible ids, NVLink push, bitmask exchange steps
@@ -247,33 +248,70 @@ int flushPages(lb200_culling* cs) {
 	return LB200_OK;
 }
 
+void fillFrustum(CullFrustum* F, const lb200_shifted_frustum* f) {
+	static const int point_of_plane[6] = {0, 4, 1, 0, 0, 2}; // geometry.cpp:134-142
+	for (int i = 0; i < 6; ++i) {
+		F->nx[i] = f->xs[i]; F->ny[i] = f->ys[i]; F->nz[i] = f->zs[i]; F->d[i] = f->ds[i];
+		F->px[i] = f->points[point_of_plane[i]][0];
+		F->py[i] = f->points[point_of_plane[i]][1];
+		F->pz[i] = f->points[point_of_plane[i]][2];
+	}
+	F->ox = f->origin[0]; F->oy = f->origin[1]; F->oz = f->origin[2];
+}
+
+CullLaunch prepareLaunch(lb200_culling* cs, uint32_t* type_base, uint32_t resident, uint32_t chunk_bound) {
+	const lb::CullingHost& h = cs->host;
+	CullLaunch L;
+	const uint32_t n_pages = livePages(cs);
+	L.n_pages = n_pages;
+	uint32_t acc = 0;
+	for (int t = 0; t < 256; ++t) { type_base[t] = acc; acc += h.type_counts[t]; }
+	const uint32_t r = cs->next_replica;
+	cs->next_replica = (cs->next_replica + 1) % cs->replicas;
+	L.off = (size_t)r * cs->dev_cap;
+	static const bool no_mask = getenv("LB200_NO_PLANE_MASKING") != nullptr;
+	L.plane_masking = (h.n_bad_radius == 0 && !no_mask && cs->launch_plane_masking != 0) ? 1u : 0u;
+	// Programmatic stream serialization: the kernel's prologue (up to cudaGridDependencySynchronize: descriptor reads, classification, the
+	// sphere tests of round 0, whose results sit in shared memory) only READS scene data.  Those arrays are written by flushPages alone, so
+	// unless something was uploaded since the last cull the prologue may overlap the tail of whatever kernel precedes it on the stream —
+	// for back-to-back views (main, shadow cascades, lights) that is the previous cull, which releases its dependents at its first
+	// instruction.  The flag is sticky: whichever call uploaded (flush, set_many, ...), the first cull after it is launched plain.
+	static const bool no_pdl = getenv("LB200_NO_PDL") != nullptr;
+	L.pdl = !no_pdl && !cs->uploaded_since_last_cull;
+	cs->uploaded_since_last_cull = false;
+	// chunk = pages per block per round: spread the pages over every resident block, at most one classify thread per page.
+	// lb200_culling_set_launch may force either: the kernels are correct for any grid (no co-residency, no grid barrier) and any chunk in
+	// 1..chunk_bound, so a forced block count is capped by neither residency nor the work; the floor of 32 pages is a speed choice.
+	const uint32_t spread = cs->launch_blocks > 0 ? (uint32_t)cs->launch_blocks : cs->launch_blocks < 0 ? (uint32_t)cs->grid : resident;
+	uint32_t chunk = (n_pages + spread - 1) / spread;
+	chunk = std::max(32u, std::min(chunk_bound, chunk));
+	if (cs->launch_chunk) chunk = std::min((uint32_t)cs->launch_chunk, chunk_bound);
+	L.chunk = chunk;
+	L.blocks = cs->launch_blocks ? spread : std::max(1u, std::min(resident, (n_pages + chunk - 1) / chunk));
+	return L;
+}
+
+void recordLaunch(lb200_culling* cs, const CullLaunch& L) {
+	cs->last_blocks = L.blocks; cs->last_chunk = L.chunk;
+	cs->last_rounds = (uint32_t)((L.n_pages + (uint64_t)L.blocks * L.chunk - 1) / ((uint64_t)L.blocks * L.chunk));
+	cs->last_pdl = L.pdl ? 1 : 0; cs->last_plane_masking = (int)L.plane_masking;
+}
+
 int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg, cudaStream_t stream, const CullOutput* dest) {
 	lb200_range range("culling"); // culling_system.cpp:330
 	lb200_ctx* ctx = cs->ctx;
-	lb::CullingHost& h = cs->host;
 	int rc = flushPages(cs);
 	if (rc) return rc;
 
 	CullParams P = {}; // outside exchange mode the exchange fields stay zero / null
-	static const int point_of_plane[6] = {0, 4, 1, 0, 0, 2}; // geometry.cpp:134-142
-	for (int i = 0; i < 6; ++i) {
-		P.nx[i] = f->xs[i]; P.ny[i] = f->ys[i]; P.nz[i] = f->zs[i]; P.d[i] = f->ds[i];
-		P.px[i] = f->points[point_of_plane[i]][0];
-		P.py[i] = f->points[point_of_plane[i]][1];
-		P.pz[i] = f->points[point_of_plane[i]][2];
-	}
-	P.ox = f->origin[0]; P.oy = f->origin[1]; P.oz = f->origin[2];
-	const uint32_t n_pages = livePages(cs);
-	P.n_pages = n_pages;
-	P.type_filter = type;
-	P.item_cap = cs->item_cap;
-	uint32_t acc = 0;
-	for (int t = 0; t < 256; ++t) { P.type_base[t] = acc; acc += h.type_counts[t]; }
+	fillFrustum(&P.f, f);
+	const CullLaunch L = prepareLaunch(cs, P.type_base, (uint32_t)(stream || xchg ? cs->grid_lanes : cs->grid), MAX_CHUNK);
 	memcpy(dest ? dest->type_base : cs->last_type_base, P.type_base, sizeof(P.type_base));
-
-	const uint32_t r = cs->next_replica;
-	cs->next_replica = (cs->next_replica + 1) % cs->replicas;
-	const size_t off = (size_t)r * cs->dev_cap;
+	P.n_pages = L.n_pages;
+	P.type_filter = type;
+	P.chunk = L.chunk;
+	P.plane_masking = L.plane_masking;
+	P.item_cap = cs->item_cap;
 	const uint32_t lane = (uint32_t)((xchg ? (uint64_t)xchg->epoch : cs->seq) % cs->lanes);
 	uint32_t* cur = cs->d_counters + ((size_t)lane * 2 + cs->lane_parity[lane]) * COUNTER_WORDS;
 	uint32_t* nxt = cs->d_counters + ((size_t)lane * 2 + (cs->lane_parity[lane] ^ 1u)) * COUNTER_WORDS;
@@ -287,41 +325,20 @@ int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, 
 		P.pub_epoch = xchg->pub_epoch; P.wait_epoch = xchg->wait_epoch; P.n_buffers = ctx->peer.n_buffers; P.rank = (uint32_t)ctx->rank;
 		if (xchg->pub_epoch) for (int r = 0; r < ctx->n_ranks; ++r) P.xprev[r] = peerSlab(ctx, xchg->pub_epoch, r);
 	}
-	static const bool no_mask = getenv("LB200_NO_PLANE_MASKING") != nullptr;
-	P.plane_masking = (h.n_bad_radius == 0 && !no_mask && cs->launch_plane_masking != 0) ? 1u : 0u;
-	// Programmatic stream serialization: the kernel's prologue (up to cudaGridDependencySynchronize: descriptor reads, classification, the
-	// sphere tests of round 0, whose results sit in shared memory) only READS scene data.  Those arrays are written by flushPages alone, so
-	// unless something was uploaded since the last cull the prologue may overlap the tail of whatever kernel precedes it on the stream —
-	// for back-to-back views (main, shadow cascades, lights) that is the previous cull, which releases its dependents at its first
-	// instruction.  The flag is sticky: whichever call uploaded (flush, set_many, ...), the first cull after it is launched plain.
-	static const bool no_pdl = getenv("LB200_NO_PDL") != nullptr;
-	const bool pdl = !no_pdl && !cs->uploaded_since_last_cull;
-	cs->uploaded_since_last_cull = false;
-	// chunk = pages per block per round: spread the pages over every resident block, at most one classify thread per page.
-	// lb200_culling_set_launch may force either: the kernel is correct for any grid (no co-residency, no grid barrier) and any chunk in
-	// 1..MAX_CHUNK, so a forced block count is capped by neither residency nor the work; the floor of 32 pages is a speed choice.
-	const uint32_t resident = (uint32_t)(stream || xchg ? cs->grid_lanes : cs->grid);
-	const uint32_t spread = cs->launch_blocks > 0 ? (uint32_t)cs->launch_blocks : cs->launch_blocks < 0 ? (uint32_t)cs->grid : resident;
-	uint32_t chunk = (n_pages + spread - 1) / spread;
-	chunk = std::max(32u, std::min((uint32_t)MAX_CHUNK, chunk));
-	if (cs->launch_chunk) chunk = (uint32_t)cs->launch_chunk;
-	const uint32_t blocks = cs->launch_blocks ? spread : std::max(1u, std::min(resident, (n_pages + chunk - 1) / chunk));
-	P.chunk = chunk;
 	cudaLaunchAttribute attr;
-	const cudaLaunchConfig_t cfg = launchConfig(blocks, CULL_THREADS, stream ? stream : ctx->stream, &attr, pdl);
+	const cudaLaunchConfig_t cfg = launchConfig(L.blocks, CULL_THREADS, stream ? stream : ctx->stream, &attr, L.pdl);
 	uint32_t* mask_arg = xchg ? (uint32_t*)nullptr : mask;
-	LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, cull_pages_kernel, P, (const lb200_page_desc*)(cs->d_desc + off), (const float4*)(cs->d_spheres + off * PAGE_SLOTS),
-		(const int*)(cs->d_entities + off * PAGE_SLOTS), out, cur, nxt, mask_arg));
+	LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, cull_pages_kernel, P, (const lb200_page_desc*)(cs->d_desc + L.off), (const float4*)(cs->d_spheres + L.off * PAGE_SLOTS),
+		(const int*)(cs->d_entities + L.off * PAGE_SLOTS), out, cur, nxt, mask_arg));
 	LB200_CHECK_LAUNCH(ctx);
 	if (!dest) {
 		cs->last_counters = cur; cs->last_out = out; cs->last_mask = mask_arg; // exchange culls keep their rows in the slabs
 		cs->last_is_view = false;
 		cs->lane_parity[lane] ^= 1u;
 		if (!xchg) ++cs->seq;
-		cs->last_pages = n_pages;
+		cs->last_pages = L.n_pages;
 	}
-	cs->last_blocks = blocks; cs->last_chunk = chunk; cs->last_rounds = (uint32_t)((n_pages + (uint64_t)blocks * chunk - 1) / ((uint64_t)blocks * chunk));
-	cs->last_pdl = pdl ? 1 : 0; cs->last_plane_masking = (int)P.plane_masking;
+	recordLaunch(cs, L);
 	return LB200_OK;
 }
 

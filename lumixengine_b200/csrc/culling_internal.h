@@ -151,10 +151,27 @@ struct Exchange { uint32_t epoch; uint32_t pub_epoch = 0, wait_epoch = 0; };
 // non-null: the cull writes here instead of into a lane, and leaves the lanes, the sequence and "the last cull" as they are
 struct CullOutput { uint32_t* ids; uint32_t* counters; uint32_t* next_counters; uint32_t* mask; uint32_t* type_base; };
 
+// What a launch of cull_pages_kernel and one of cull_views_kernel decide the same way (prepareLaunch)
+struct CullLaunch {
+	uint32_t n_pages;       // pages the kernel looks at
+	size_t off;             // first page of the replica it reads
+	uint32_t plane_masking; // 1 unless a negative / NaN radius, LB200_NO_PLANE_MASKING or set_launch switches it off
+	bool pdl;               // programmatic stream serialization behind the previous kernel of the stream
+	uint32_t blocks, chunk; // grid, pages per block per round
+};
+struct CullFrustum; // cull_common.cuh
+
 // culling.cu
 int ensureDevice(lb200_culling* cs);
 int flushPages(lb200_culling* cs);
 int resizePages(lb200_culling* cs, uint32_t min_pages, bool keep); // the one owner of the page arrays' size
+// a frustum as the cull kernels read it
+void fillFrustum(CullFrustum* F, const lb200_shifted_frustum* f);
+// type bases into type_base[256], the next replica, plane masking, PDL, and the launch shape: spread over `resident` blocks (or the
+// set_launch override), at most chunk_bound pages per block and round
+CullLaunch prepareLaunch(lb200_culling* cs, uint32_t* type_base, uint32_t resident, uint32_t chunk_bound);
+// the launch as lb200_culling_get_launch reports it
+void recordLaunch(lb200_culling* cs, const CullLaunch& L);
 int launchCull(lb200_culling* cs, const lb200_shifted_frustum* f, uint8_t type, const Exchange* xchg = nullptr, cudaStream_t stream = nullptr,
 	const CullOutput* out = nullptr);
 // counters of one cull (on the host) and the type bases it was culled with -> *res

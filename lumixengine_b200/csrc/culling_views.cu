@@ -57,57 +57,30 @@ int ensureViewBuffers(lb200_culling* cs, uint32_t n_views) {
 	return LB200_OK;
 }
 
-// the fused kernel for n_views >= 2 views on the context stream; launch shape and programmatic launch as in launchCull
+// the fused kernel for n_views >= 2 views on the context stream; launch shape and programmatic launch decided as for launchCull (prepareLaunch)
 int launchViews(lb200_culling* cs, const lb200_shifted_frustum* frusta, const uint8_t* types, uint32_t n_views, uint32_t* counters, uint32_t* next_counters) {
 	lb200_range range("culling views");
 	lb200_ctx* ctx = cs->ctx;
-	lb::CullingHost& h = cs->host;
 	ViewsParams P = {};
-	static const int point_of_plane[6] = {0, 4, 1, 0, 0, 2}; // geometry.cpp:134-142
 	for (uint32_t v = 0; v < n_views; ++v) {
-		const lb200_shifted_frustum* f = frusta + v;
-		for (int i = 0; i < 6; ++i) {
-			P.nx[v][i] = f->xs[i]; P.ny[v][i] = f->ys[i]; P.nz[v][i] = f->zs[i]; P.d[v][i] = f->ds[i];
-			P.px[v][i] = f->points[point_of_plane[i]][0];
-			P.py[v][i] = f->points[point_of_plane[i]][1];
-			P.pz[v][i] = f->points[point_of_plane[i]][2];
-		}
-		P.ox[v] = f->origin[0]; P.oy[v] = f->origin[1]; P.oz[v] = f->origin[2];
+		fillFrustum(&P.f[v], frusta + v);
 		P.type_filter[v] = types[v];
 	}
-	const uint32_t n_pages = livePages(cs);
-	P.n_views = n_views;
-	P.n_pages = n_pages;
-	uint32_t acc = 0;
-	for (int t = 0; t < 256; ++t) { P.type_base[t] = acc; acc += h.type_counts[t]; }
+	// the chunk bounded by the items a round holds: min(256, 512 / n_views) pages
+	const CullLaunch L = prepareLaunch(cs, P.type_base, (uint32_t)cs->grid, viewsChunkBound(n_views));
 	memcpy(cs->views_type_base, P.type_base, sizeof(P.type_base));
+	P.n_views = n_views;
+	P.n_pages = L.n_pages;
+	P.chunk = L.chunk;
+	P.plane_masking = L.plane_masking;
 	P.id_stride = cs->view_id_cap;
 	P.mask_stride = 8 * cs->dev_cap;
-
-	const uint32_t r = cs->next_replica;
-	cs->next_replica = (cs->next_replica + 1) % cs->replicas;
-	const size_t off = (size_t)r * cs->dev_cap;
-	static const bool no_mask = getenv("LB200_NO_PLANE_MASKING") != nullptr;
-	P.plane_masking = (h.n_bad_radius == 0 && !no_mask && cs->launch_plane_masking != 0) ? 1u : 0u;
-	static const bool no_pdl = getenv("LB200_NO_PDL") != nullptr;
-	const bool pdl = !no_pdl && !cs->uploaded_since_last_cull;
-	cs->uploaded_since_last_cull = false;
-	// launchCull's rule, with the chunk bounded by the items a round holds: min(256, 512 / n_views) pages
-	const uint32_t bound = viewsChunkBound(n_views);
-	const uint32_t resident = (uint32_t)cs->grid;
-	const uint32_t spread = cs->launch_blocks > 0 ? (uint32_t)cs->launch_blocks : resident;
-	uint32_t chunk = (n_pages + spread - 1) / spread;
-	chunk = std::max(32u, std::min(bound, chunk));
-	if (cs->launch_chunk) chunk = std::min((uint32_t)cs->launch_chunk, bound);
-	const uint32_t blocks = cs->launch_blocks ? spread : std::max(1u, std::min(resident, (n_pages + chunk - 1) / chunk));
-	P.chunk = chunk;
 	cudaLaunchAttribute attr;
-	const cudaLaunchConfig_t cfg = launchConfig(blocks, VIEW_THREADS, ctx->stream, &attr, pdl);
-	LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, cull_views_kernel, P, (const lb200_page_desc*)(cs->d_desc + off), (const float4*)(cs->d_spheres + off * LB200_PAGE_SLOTS),
-		(const int*)(cs->d_entities + off * LB200_PAGE_SLOTS), cs->d_view_ids.get(), counters, next_counters, cs->d_view_mask.get()));
+	const cudaLaunchConfig_t cfg = launchConfig(L.blocks, VIEW_THREADS, ctx->stream, &attr, L.pdl);
+	LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, cull_views_kernel, P, (const lb200_page_desc*)(cs->d_desc + L.off), (const float4*)(cs->d_spheres + L.off * LB200_PAGE_SLOTS),
+		(const int*)(cs->d_entities + L.off * LB200_PAGE_SLOTS), cs->d_view_ids.get(), counters, next_counters, cs->d_view_mask.get()));
 	LB200_CHECK_LAUNCH(ctx);
-	cs->last_blocks = blocks; cs->last_chunk = chunk; cs->last_rounds = (uint32_t)((n_pages + (uint64_t)blocks * chunk - 1) / ((uint64_t)blocks * chunk));
-	cs->last_pdl = pdl ? 1 : 0; cs->last_plane_masking = (int)P.plane_masking;
+	recordLaunch(cs, L);
 	return LB200_OK;
 }
 

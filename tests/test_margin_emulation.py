@@ -1,10 +1,12 @@
 """CPU emulation (numpy float32, no FMA) of the two conservative shortcuts of the cull kernels, checked against the exact expressions:
 
-* plane masking (cull_kernel.cuh phase A): a plane dropped for a cell can never give a sphere of that cell a negative t - r;
-* the cheap pass A1 of the lean variant (cull_kernel_lean.cuh): a page it drops is classified "outside" by the exact cell tests
-  (neither containsAABB(origin + cs, cs) nor intersectsAABB(origin - cs, 2cs), geometry.cpp:99-118, 159-178).
+* plane masking (plane_mask over relative_offsets, csrc/cull_common.cuh): a plane dropped for a cell can never give a sphere of that
+  cell a negative t - r (test_rows);
+* the cheap pass A1 (outside_by_margin, csrc/cull_common.cuh): a page it drops is classified "outside" by the exact cell tests of
+  classify_cell (neither containsAABB(origin + cs, cs) nor intersectsAABB(origin - cs, 2cs), geometry.cpp:99-118, 159-178).
 
-The emulation repeats the device expressions operation by operation; frustums come from the product's own host builders."""
+Both cull kernels call these functions.  The emulation repeats their expressions operation by operation; frustums come from the
+product's own host builders."""
 import numpy as np
 
 import lumixengine_b200 as lb
@@ -51,7 +53,7 @@ def test_lean_cheap_pass_never_drops_a_page_the_exact_tests_keep():
         nx, ny, nz, d, _, org = _planes(f)
         for spread in (600.0, 3000.0, 30000.0):
             cells = _cells_near(rng, org, 4000, spread)
-            # exact tests (phase A of cull_kernel.cuh): float32 op for op
+            # exact tests (classify_cell, csrc/cull_common.cuh): float32 op for op
             rel_c = ((cells + np.float64(CS)) - org).astype(F)
             max_c = rel_c + CS
             rel_i = ((cells - np.float64(CS)) - org).astype(F)
