@@ -298,7 +298,7 @@ typedef struct lb200_sk_view {
 	uint8_t layer_to_bucket[256]; /* View::layer_to_bucket */
 } lb200_sk_view;
 typedef struct lb200_sk_result { uint32_t n_keys, n_instances, n_pose, n_dirty, n_groups; } lb200_sk_result;
-typedef struct lb200_sk_outputs { /* device pointers, valid until the next create_keys */
+typedef struct lb200_sk_outputs { /* device pointers, valid until the next create_keys (create_keys_views for a view's) */
 	const uint64_t* keys;              /* n_keys sort keys (sorted if asked), pipeline.cpp:62-71 layout */
 	const uint64_t* values;            /* their sort values */
 	const uint32_t* group_count;       /* per mesh sort key g in [0, n_groups): instances of the group */
@@ -327,14 +327,35 @@ LB200_API int lb200_sortkeys_set_transforms(lb200_sortkeys* sk, const lb200_tran
 LB200_API int lb200_sortkeys_set_transforms_device(lb200_sortkeys* sk, const lb200_transform* dev_transforms, uint32_t n);
 /* createSortKeys (+ radixSort if `sort`) for the last cull of `cs` on the context stream.  Asynchronous unless `want_counts`. */
 LB200_API int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb200_sk_view* view, int sort, int want_counts, lb200_sk_result* result);
-/* Launch shape of later create_keys calls.  blocks: 0 = the default (LB200_SK_BLOCKS_PER_SM per SM, else 2, and at most one block per 256
+/* createSortKeys (+ radixSort if `sort`) for every view of the latest lb200_culling_cull_views call on `cs`, in one launch on the context
+ * stream.  View v reads the ids, per-type segments and counters of view v of that call (never "the last cull"); n_views must equal its
+ * view count.  The call does exactly what n_views calls of lb200_culling_select_view(cs, v) + lb200_sortkeys_create_keys(sk, cs,
+ * &views[v], sort, ...) do in the order v = 0, 1, ...: a later view sees the ModelInstance::lod and Pose::frame that the earlier views
+ * left, so a skinned instance joins the pose list of the first view that draws it and of no other.  The reference runs a frame's views
+ * as concurrent jobs in no fixed order; view order is one of the orders it can produce.
+ * Each view has its own outputs (keys, values, groups, instance data, pose and dirty lists; capacities max_keys / max_instances per
+ * view), apart from those of lb200_sortkeys_create_keys: neither call touches the other's.  They stay valid until the next
+ * create_keys_views on `sk` or its destroy; lb200_sortkeys_view_outputs hands them out.  The first call allocates them, a call with more
+ * views than any before it reallocates them.  want_counts != 0: one read-back of every view's counters and one synchronisation fill
+ * results[0, n_views); if a view exceeds a capacity the call returns LB200_ERR_CAPACITY with every results[v] still holding the sizes
+ * needed.  want_counts = 0: fully asynchronous, results may be NULL.
+ * LB200_ERR_STATE where lb200_culling_select_view refuses (no cull_views yet, an empty culling system, view buffers released by a growth
+ * of the page arrays or lb200_culling_set_replicas) and before set_models / set_transforms.  LB200_ERR_INVALID for n_views 0, above
+ * LB200_CULL_MAX_VIEWS or different from the cull's, for views whose max_sort_key differ (Renderer::getMaxSortKey() is renderer-wide),
+ * and for everything lb200_sortkeys_create_keys refuses.  A refused call leaves the earlier outputs as they were. */
+LB200_API int lb200_sortkeys_create_keys_views(lb200_sortkeys* sk, lb200_culling* cs, const lb200_sk_view* views, uint32_t n_views,
+                                               int sort, int want_counts, lb200_sk_result* results /* n_views */);
+/* Launch shape of later create_keys / create_keys_views calls.  blocks: 0 = the default (LB200_SK_BLOCKS_PER_SM per SM, else 2, and at most one block per 256
  * renderables the cull can emit), -1 = every block that is co-resident, n > 0 = min(n, co-resident blocks); only 0 caps the grid by the
  * work.  prefetch_ahead: 0..4 grid strides of L2 prefetch, -1 = the default (LB200_SK_PREFETCH, else 0).  Any other value is
- * LB200_ERR_INVALID.  get_launch reports the last create_keys launch: blocks, whether the group counters lived in shared memory
+ * LB200_ERR_INVALID.  get_launch reports the last launch of either call: blocks, whether the group counters lived in shared memory
  * (max_sort_key < 8192) and the prefetch distance (all 0 before the first). */
 LB200_API int lb200_sortkeys_set_launch(lb200_sortkeys* sk, int blocks, int prefetch_ahead);
 LB200_API int lb200_sortkeys_get_launch(lb200_sortkeys* sk, uint32_t* grid, int* groups_in_smem, uint32_t* prefetch_ahead);
 LB200_API int lb200_sortkeys_device_outputs(lb200_sortkeys* sk, lb200_sk_outputs* out);
+/* Device pointers of view k of the latest create_keys_views call (layout as lb200_sortkeys_device_outputs; lod / pose_frame are the
+ * shared per-entity state).  LB200_ERR_STATE before any create_keys_views, LB200_ERR_INVALID for k >= its n_views. */
+LB200_API int lb200_sortkeys_view_outputs(lb200_sortkeys* sk, uint32_t k, lb200_sk_outputs* out);
 /* RenderModuleImpl::onModelInstanceMoved (src/renderer/render_module.cpp:1544-1554) for n instances whose new transforms lie in device memory:
  * the transforms go into the entity records, ModelInstance::MOVED is set (createSortKeys then draws the instance as DRAW_MESH, pipeline.cpp
  * :3904-3909) and the instance joins m_moved_instances once.  With dev_bounding_radius (per moved instance: Model::getOriginBoundingRadius)

@@ -86,6 +86,18 @@ int launchViews(lb200_culling* cs, const lb200_shifted_frustum* frusta, const ui
 
 } // namespace
 
+int lb200_culling_internal_views(lb200_culling* cs, CullViewsResult* out) {
+	if (!cs || !cs->ctx || !out) return LB200_ERR_INVALID;
+	if (!cs->views_n) { lb200_set_error(cs->ctx, "no cull_views has been issued on this culling system yet"); return LB200_ERR_STATE; }
+	if (!cs->views_live) {
+		lb200_set_error(cs->ctx, "the latest cull_views call has no results (an empty culling system, or the page arrays grew / set_replicas since)");
+		return LB200_ERR_STATE;
+	}
+	out->n_views = cs->views_n; out->id_stride = cs->view_id_cap; out->counter_stride = COUNTER_WORDS;
+	out->ids = cs->d_view_ids; out->counters = cs->views_counters; out->type_base = cs->views_type_base; out->type_counts = cs->host.type_counts;
+	return LB200_OK;
+}
+
 extern "C" {
 
 int lb200_culling_cull_views(lb200_culling* cs, const lb200_shifted_frustum* frusta, const uint8_t* types, uint32_t n_views,

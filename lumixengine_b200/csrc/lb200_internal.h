@@ -159,6 +159,14 @@ struct lb200_range {
 };
 // culling.cu: where the last cull left its result (device: ids, counters; host: per-type segment bases and entity counts, 256 each)
 int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, const uint32_t** counters, const uint32_t** type_base, const uint32_t** type_counts);
+// culling_views.cu: where the latest cull_views call left its results: view v's ids at *ids + v * *id_stride, its counters at
+// *counters + v * *counter_stride, the per-type segment bases every view was culled with, and the host's entity counts (256 each).
+// LB200_ERR_STATE while select_view would refuse (no call yet, an empty system, view buffers released since).
+struct CullViewsResult {
+	uint32_t n_views, id_stride, counter_stride;
+	const uint32_t *ids, *counters, *type_base, *type_counts;
+};
+int lb200_culling_internal_views(lb200_culling* cs, CullViewsResult* out);
 // culling.cu: 1 + the largest entity id ever added (0 if none): every id a cull of cs can emit is below it
 uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs);
 // context.cu: *out = blocks of a cooperative kernel that can be co-resident on the context's device (threads per block, dynamic smem)

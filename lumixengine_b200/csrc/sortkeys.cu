@@ -9,7 +9,8 @@
 // mesh needs for its LOD and its keys; sector 1 = rotation, scale, Pose::frame — what the instance data adds.  (Round-2 profile of the
 // SoA form: 1.33 GB of DRAM reads per 1.5 M visible meshes, six 32-byte sectors per renderable and pass; profiles/r2_B_sortkeys_ncu.txt.)
 //
-//   create_keys_kernel one cooperative launch (grid = what is co-resident), one thread per visible renderable, grid-stride:
+//   create_keys_kernel one cooperative launch (grid = what is co-resident) for one view (create_keys) or every view of a cull_views call
+//   (create_keys_views), the views one after the other; per view one thread per visible renderable, grid-stride:
 //     pass 1  MESH: sector 0 -> squared distance to the LOD reference point in fp64 -> float, Model::getLODMeshIndices (model.h:173-179),
 //             the lod smoothing of :3926-3941 (ModelInstance::lod updated in place), the pose claim (the compare-exchange on Pose::frame,
 //             :3890-3897); what the renderable will emit is COUNTED (keys, pose entries per thread; instances per auto-instancer group
@@ -58,9 +59,30 @@ struct alignas(64) SkEntity {
 };
 static_assert(sizeof(SkEntity) == 64, "one burst per entity");
 
+constexpr uint32_t SK_MAX_VIEWS = LB200_CULL_MAX_VIEWS;
+// One view's lb200_sk_view without its tables (those are in EmitArgs::tables, SK_TABLE_WORDS per view)
+struct ViewScalars {
+	double camera_pos[3], lod_ref_point[3];
+	float time_delta, lod_multiplier;
+	uint32_t frame_number, is_shadow;
+};
+static_assert(sizeof(ViewScalars) == 64, "one view's scalars");
+constexpr uint32_t SK_TABLE_WORDS = 256 + 64; // bucket_map (256 words) then layer_to_bucket (256 bytes): 1,280 B per view
+
+// Where one view's outputs go (counts: CNT_WORDS counters; group tables: n_groups each)
+struct ViewOut {
+	uint64_t* keys; uint64_t* values; uint32_t* counts;
+	uint32_t* group_count; uint32_t* group_offset; uint32_t* group_cursor;
+	uint64_t* group_renderables; float4* instance_data;
+	uint32_t* pose_list; uint32_t* dirty_list;
+};
+
 struct EmitParams {
-	lb200_sk_view view;
-	uint32_t type_base[4]; // offsets of the MESH / DECAL / LOCAL_LIGHT / CURVE_DECAL segments inside out_ids
+	ViewScalars view[SK_MAX_VIEWS]; // views [0, n_views) of the launch
+	ViewOut out[SK_MAX_VIEWS];
+	uint32_t n_views;
+	uint32_t type_base[4]; // offsets of the MESH / DECAL / LOCAL_LIGHT / CURVE_DECAL segments inside every view's ids
+	uint32_t id_stride, counter_stride; // view v's ids at visible + v * id_stride, its cull counters at cull_counters + v * counter_stride
 	uint32_t cap_keys, cap_recs, cap_pose, cap_dirty;
 	uint32_t prefetch_ahead; // records requested into L2 this many grid strides ahead of their use (0 = off; LB200_SK_PREFETCH, default 0)
 };
@@ -83,11 +105,9 @@ __device__ __forceinline__ uint32_t warp_claim_keyed(uint32_t* counters, uint32_
 
 struct EmitArgs {
 	SkEntity* ent; const uint32_t* __restrict__ decal_sort_key; const uint8_t* __restrict__ decal_layer;
-	const lb200_sk_model* __restrict__ models; const lb200_sk_mesh* __restrict__ meshes;
-	uint64_t* __restrict__ keys; uint64_t* __restrict__ values; uint32_t* counts;
-	uint32_t* group_count; uint32_t* group_offset; uint32_t* group_cursor; const uint8_t* __restrict__ group_layer;
-	uint64_t* __restrict__ group_renderables; float4* __restrict__ instance_data;
-	uint32_t* __restrict__ pose_list; uint32_t* __restrict__ dirty_list; uint32_t* __restrict__ stash; float4* __restrict__ stash4; uint32_t stash_stride;
+	const lb200_sk_model* __restrict__ models; const lb200_sk_mesh* __restrict__ meshes; const uint32_t* __restrict__ tables;
+	const uint8_t* __restrict__ group_layer;
+	uint32_t* __restrict__ stash; float4* __restrict__ stash4; uint32_t stash_stride;
 	GridBar* bar;
 };
 
@@ -131,7 +151,7 @@ __device__ __forceinline__ MeshKind mesh_kind(const lb200_sk_mesh& mm, uint32_t 
 }
 
 // MESH renderable, pass 1 (:3868-3956): LOD selection + smoothing state + pose claim; counts what pass 2 will write
-__device__ __forceinline__ uint32_t mesh_count(const EmitParams& P, const EmitArgs& A, const uint32_t* s_bucket_map, uint32_t* s_grp, float lod_multiplier_rcp, int32_t e, uint32_t i, Counts& c) {
+__device__ __forceinline__ uint32_t mesh_count(const ViewScalars& W, const ViewOut& O, const EmitArgs& A, const uint32_t* s_bucket_map, uint32_t* s_grp, float lod_multiplier_rcp, int32_t e, uint32_t i, Counts& c) {
 	SkEntity* rec = A.ent + e;
 	// the whole record, one 64-byte burst (coherent loads: this kernel writes lod / pose_frame)
 	const int4* rp = reinterpret_cast<const int4*>(rec);
@@ -142,19 +162,19 @@ __device__ __forceinline__ uint32_t mesh_count(const EmitParams& P, const EmitAr
 	const uint32_t model_idx = model_flags & CODE_MODEL_MASK, fl = model_flags >> 24;
 	if (fl & LB200_SK_DIRTY) return CODE_DIRTY | model_idx; // mi.dirty, :3878-3881
 	const lb200_sk_model model = load_model(A.models + model_idx);
-	const double dx = LB_DSUB(px, P.view.lod_ref_point[0]), dy = LB_DSUB(py, P.view.lod_ref_point[1]), dz = LB_DSUB(pz, P.view.lod_ref_point[2]);
+	const double dx = LB_DSUB(px, W.lod_ref_point[0]), dy = LB_DSUB(py, W.lod_ref_point[1]), dz = LB_DSUB(pz, W.lod_ref_point[2]);
 	const float squared_length = (float)LB_DADD(LB_DADD(LB_DMUL(dx, dx), LB_DMUL(dy, dy)), LB_DMUL(dz, dz)); // squaredLength(DVec3), math.cpp:397
 	const float sd = LB_FMUL(squared_length, lod_multiplier_rcp);
 	const uint32_t lod_idx = sd < model.lod_distances[0] ? 0u : sd < model.lod_distances[1] ? 1u : sd < model.lod_distances[2] ? 2u : sd < model.lod_distances[3] ? 3u : 4u;
-	const bool is_shadow = P.view.is_shadow != 0;
+	const bool is_shadow = W.is_shadow != 0;
 	uint32_t lod0 = lod_idx;
 	bool two = false;
 	if (cur != (float)lod_idx) { // :3926-3941
 		const float d = LB_FSUB((float)lod_idx, cur);
 		const float ad = fabsf(d);
-		if (ad <= P.view.time_delta) cur = (float)lod_idx;
+		if (ad <= W.time_delta) cur = (float)lod_idx;
 		else {
-			if (!is_shadow) cur = LB_FADD(cur, LB_FMUL(LB_FDIV(d, ad), P.view.time_delta));
+			if (!is_shadow) cur = LB_FADD(cur, LB_FMUL(LB_FDIV(d, ad), W.time_delta));
 			lod0 = (uint32_t)cur;
 			two = lod0 < 3;
 		}
@@ -162,7 +182,7 @@ __device__ __forceinline__ uint32_t mesh_count(const EmitParams& P, const EmitAr
 	}
 	// what pass 2 writes per auto-instanced mesh (:3990-4008) or depth-sorted key (:3915-3922), stashed next to the decision in arrays indexed
 	// like the visible list: pass 2 reads them coalesced and never touches the record again
-	const double rx = LB_DSUB(px, P.view.camera_pos[0]), ry = LB_DSUB(py, P.view.camera_pos[1]), rz = LB_DSUB(pz, P.view.camera_pos[2]);
+	const double rx = LB_DSUB(px, W.camera_pos[0]), ry = LB_DSUB(py, W.camera_pos[1]), rz = LB_DSUB(pz, W.camera_pos[2]);
 	const uint32_t depth_bits = float_flip(__float_as_uint((float)LB_DADD(LB_DADD(LB_DMUL(rx, rx), LB_DMUL(ry, ry)), LB_DMUL(rz, rz))));
 	__stcs(A.stash4 + i, make_float4(__int_as_float(q2.x), __int_as_float(q2.y), __int_as_float(q2.z), __int_as_float(q2.w)));                 // rot
 	__stcs(A.stash4 + A.stash_stride + i, make_float4((float)rx, (float)ry, (float)rz, __uint_as_float(depth_bits)));                            // Vec3(tr.pos - camera_pos), depth key
@@ -182,33 +202,33 @@ __device__ __forceinline__ uint32_t mesh_count(const EmitParams& P, const EmitAr
 		c.k += kind.key ? 1u : 0u;
 		if (kind.inst) { // AutoInstancer::add, :3913-3914
 			if (s_grp) atomicAdd(&s_grp[mm.sort_key], 1u);
-			else warp_claim_keyed(A.group_count, mm.sort_key);
+			else warp_claim_keyed(O.group_count, mm.sort_key);
 		}
 	}
 	// once per instance and frame the palette has to be built (PoseProcessor::push; the compare-exchange on Pose::frame of :3890-3897 —
 	// one thread owns the instance within a view)
-	if (any_skinned && (uint32_t)q3.w != P.view.frame_number) { rec->pose_frame = P.view.frame_number; code |= CODE_POSE; ++c.p; }
+	if (any_skinned && (uint32_t)q3.w != W.frame_number) { rec->pose_frame = W.frame_number; code |= CODE_POSE; ++c.p; }
 	return code;
 }
 
-__device__ __forceinline__ void push_key(const EmitParams& P, const EmitArgs& A, uint32_t& slot, uint64_t key, uint64_t value) {
-	if (slot < P.cap_keys) { A.keys[slot] = key; A.values[slot] = value; }
+__device__ __forceinline__ void push_key(const EmitParams& P, const ViewOut& O, uint32_t& slot, uint64_t key, uint64_t value) {
+	if (slot < P.cap_keys) { O.keys[slot] = key; O.values[slot] = value; }
 	++slot;
 }
 
 // MESH renderable, pass 2: replay of the stashed decision, writes
-__device__ __forceinline__ void mesh_write(const EmitParams& P, const EmitArgs& A, const uint32_t* s_bucket_map, uint32_t* s_grp, int32_t e, uint32_t i, uint32_t code, uint32_t& k, uint32_t& p) {
+__device__ __forceinline__ void mesh_write(const EmitParams& P, const ViewScalars& W, const ViewOut& O, const EmitArgs& A, const uint32_t* s_bucket_map, uint32_t* s_grp, int32_t e, uint32_t i, uint32_t code, uint32_t& k, uint32_t& p) {
 	if (code & CODE_DIRTY) { // queueMaterialOverrideRefresh (rare: its own atomic)
-		const uint32_t slot = atomicAdd(&A.counts[CNT_DIRTY], 1u);
-		if (slot < P.cap_dirty) A.dirty_list[slot] = (uint32_t)e;
+		const uint32_t slot = atomicAdd(&O.counts[CNT_DIRTY], 1u);
+		if (slot < P.cap_dirty) O.dirty_list[slot] = (uint32_t)e;
 		return;
 	}
 	const lb200_sk_model model = load_model(A.models + (code & CODE_MODEL_MASK));
-	const bool moved_not_shadow = (code & CODE_MOVED) && P.view.is_shadow == 0;
+	const bool moved_not_shadow = (code & CODE_MOVED) && W.is_shadow == 0;
 	const uint32_t lod0 = (code >> CODE_LOD_SHIFT) & 7u;
 	const bool two = (code & CODE_TWO) != 0;
 	if (code & CODE_POSE) {
-		if (p < P.cap_pose) A.pose_list[p] = (uint32_t)e;
+		if (p < P.cap_pose) O.pose_list[p] = (uint32_t)e;
 		++p;
 	}
 	const float4 s_rot = __ldcs(A.stash4 + i), s_pos = __ldcs(A.stash4 + A.stash_stride + i), s_scl = __ldcs(A.stash4 + 2 * (size_t)A.stash_stride + i); // coalesced, read once
@@ -223,13 +243,13 @@ __device__ __forceinline__ void mesh_write(const EmitParams& P, const EmitArgs& 
 		const uint64_t mesh_value = sext(e) | ((uint64_t)mesh_idx << SORT_VALUE_MESH_IDX_SHIFT);
 		if (kind.key) {
 			const uint64_t low = kind.depth ? (uint64_t)__float_as_uint(s_pos.w) : (uint64_t)mm.sort_key;
-			push_key(P, A, k, low | ((uint64_t)(uint8_t)bucket << SORT_KEY_BUCKET_SHIFT), mesh_value | ((uint64_t)(kind.skinned ? DRAW_SKINNED : DRAW_MESH) << SORT_VALUE_TYPE_SHIFT));
+			push_key(P, O, k, low | ((uint64_t)(uint8_t)bucket << SORT_KEY_BUCKET_SHIFT), mesh_value | ((uint64_t)(kind.skinned ? DRAW_SKINNED : DRAW_MESH) << SORT_VALUE_TYPE_SHIFT));
 		}
 		if (kind.inst) { // instance data of the auto-instanced mesh, :3990-4008, at the group's offset + this block's slice + rank
-			const uint32_t at = s_grp ? atomicAdd(&s_grp[mm.sort_key], 1u) : warp_claim_keyed(A.group_cursor, mm.sort_key);
+			const uint32_t at = s_grp ? atomicAdd(&s_grp[mm.sort_key], 1u) : warp_claim_keyed(O.group_cursor, mm.sort_key);
 			if (at < P.cap_recs) {
-				__stcs(reinterpret_cast<unsigned long long*>(A.group_renderables) + at, (unsigned long long)mesh_value);
-				float4* dst = A.instance_data + (size_t)at * 3;
+				__stcs(reinterpret_cast<unsigned long long*>(O.group_renderables) + at, (unsigned long long)mesh_value);
+				float4* dst = O.instance_data + (size_t)at * 3;
 				__stcs(dst, s_rot);
 				__stcs(dst + 1, make_float4(s_pos.x, s_pos.y, s_pos.z, LB_FSUB(s_scl.w, mm.lod))); // camera-relative position, lod - mesh.lod
 				__stcs(dst + 2, make_float4(s_scl.x, s_scl.y, s_scl.z, __uint_as_float(mm.material_index)));
@@ -265,115 +285,128 @@ __device__ __forceinline__ uint32_t visible_at(const EmitParams& P, const uint32
 	return i < n_mesh ? visible[P.type_base[RT_MESH] + i] : i < n_mesh + n_decal ? visible[P.type_base[RT_DECAL] + (i - n_mesh)] : visible[P.type_base[RT_CURVE_DECAL] + (i - n_mesh - n_decal)];
 }
 
-__global__ void __launch_bounds__(SK_THREADS, 4) create_keys_kernel(const __grid_constant__ EmitParams P, const uint32_t* __restrict__ visible,
-	const uint32_t* __restrict__ cull_counters, EmitArgs A, uint32_t n_groups)
+// Views [0, P.n_views) one after the other, each exactly as a launch of its own would run it: pass 1, grid barrier, group scan (+ barrier
+// with the group cursors in HBM), pass 2.  A later view sees the lod / pose_frame stores of the earlier ones through the barrier behind
+// their pass 1 (records are read with ld.cg, never from L1).  No grid barrier separates a view's pass 2 from the next view's pass 1: pass 2
+// reads no record, every view has its own counters, group tables and outputs, and stash slot i is written (pass 1) and read (pass 2) by
+// the thread that owns index i in every view, the grid stride being the same.
+__global__ void __launch_bounds__(SK_THREADS, 4) create_keys_kernel(const __grid_constant__ EmitParams P, const uint32_t* __restrict__ visible_all,
+	const uint32_t* __restrict__ cull_counters_all, EmitArgs A, uint32_t n_groups)
 {
 	extern __shared__ uint32_t s_grp_mem[];
 	__shared__ uint32_t s_warp[SK_THREADS / 32];
 	__shared__ uint32_t s_base[2];
 	__shared__ uint32_t s_carry;
 	__shared__ uint32_t s_bucket_map[256];
-	s_bucket_map[threadIdx.x] = P.view.bucket_map[threadIdx.x]; // SK_THREADS == 256
-	uint32_t* s_grp = n_groups <= SK_SMEM_GROUPS ? s_grp_mem : nullptr;
-	if (s_grp) for (uint32_t g = threadIdx.x; g < n_groups; g += SK_THREADS) s_grp[g] = 0;
-	__syncthreads();
-	// the three segments as one index space: [MESH | DECAL | CURVE_DECAL]
-	const uint32_t n_mesh = __ldg(cull_counters + RT_MESH), n_decal = __ldg(cull_counters + RT_DECAL), n_curve = __ldg(cull_counters + RT_CURVE_DECAL);
-	const uint32_t n_all = n_mesh + n_decal + n_curve;
-	const float lod_multiplier_rcp = LB_FDIV(1.0f, P.view.lod_multiplier); // :3798-3799
-	const uint32_t stride = gridDim.x * SK_THREADS;
-
-	// ---- pass 1: decide + count ----
-	// The walk is a random gather by entity id: the id of the thread's NEXT renderable is read one iteration ahead and its record is
-	// requested into L2 while the current one is processed (a dependent chain id -> record -> model -> mesh per renderable otherwise).
-	Counts c = {0u, 0u, 0u};
-	{
-		uint32_t i = blockIdx.x * SK_THREADS + threadIdx.x;
-		uint32_t e = i < n_all ? visible_at(P, visible, i, n_mesh, n_decal) : 0u;
-		const uint32_t ahead = P.prefetch_ahead * stride;
-		for (; i < n_all; i += stride) {
-			const uint32_t i_next = i + stride;
-			uint32_t e_next = 0;
-			if (i_next < n_all) e_next = visible_at(P, visible, i_next, n_mesh, n_decal);
-			if (ahead) {
-				const uint32_t i_pf = i + ahead;
-				if (i_pf < n_all) {
-					const uint32_t e_pf = ahead == stride ? e_next : visible_at(P, visible, i_pf, n_mesh, n_decal);
-					if (i_pf < n_mesh) { prefetch_l2(A.ent + e_pf); prefetch_l2(reinterpret_cast<const char*>(A.ent + e_pf) + 32); }
-					else { prefetch_l2(A.decal_layer + e_pf); prefetch_l2(A.decal_sort_key + e_pf); }
-				}
-			}
-			if (i < n_mesh) A.stash[i] = mesh_count(P, A, s_bucket_map, s_grp, lod_multiplier_rcp, (int32_t)e, i, c);
-			else { // DECAL / CURVE_DECAL renderable (:3840-3867): one key if its layer is in the view; bucket and material sort key stashed for pass 2
-				const uint32_t bucket = (uint8_t)s_bucket_map[A.decal_layer[e]];
-				uint32_t key = 0;
-				if (bucket < 0xff) { key = A.decal_sort_key[e]; ++c.k; }
-				A.stash[i] = bucket;
-				A.stash4[i].x = __uint_as_float(key);
-			}
-			e = e_next;
-		}
-	}
-	uint32_t tk, tp;
-	const uint32_t pk = block_exclusive_scan(c.k, s_warp, &tk);
-	const uint32_t pp = block_exclusive_scan(c.p, s_warp, &tp);
-	if (threadIdx.x == 0) {
-		s_base[0] = tk ? atomicAdd(&A.counts[CNT_KEYS], tk) : 0u;
-		s_base[1] = tp ? atomicAdd(&A.counts[CNT_POSE], tp) : 0u;
-	}
-	// the block's slice of every group it has instances of: count -> start inside the group
-	if (s_grp) for (uint32_t g = threadIdx.x; g < n_groups; g += SK_THREADS) if (s_grp[g]) s_grp[g] = atomicAdd(&A.group_count[g], s_grp[g]);
-	uint32_t barriers_passed = 0;
-	grid_barrier(A.bar, barriers_passed); // every block's counts are in: group totals are final
-
-	// ---- group offsets = exclusive scan of the group totals; block 0 publishes them and one key/value per non-empty group (:3958-3969) ----
-	if (s_grp || blockIdx.x == 0) {
-		if (threadIdx.x == 0) s_carry = 0;
+	for (uint32_t v = 0; v < P.n_views; ++v) { // v is all the loop carries: what follows is derived from it and the parameters
+		uint32_t* s_grp = n_groups <= SK_SMEM_GROUPS ? s_grp_mem : nullptr;
+		const uint32_t stride = gridDim.x * SK_THREADS;
+		uint32_t barriers_passed = v * (s_grp ? 1u : 2u); // the earlier views' grid barriers
+		const ViewScalars& W = P.view[v];
+		const ViewOut& O = P.out[v];
+		const uint32_t* __restrict__ visible = visible_all + (size_t)v * P.id_stride;
+		const uint32_t* __restrict__ cull_counters = cull_counters_all + (size_t)v * P.counter_stride;
+		__syncthreads(); // the previous view's pass 2 is done with s_bucket_map / s_grp in this block
+		s_bucket_map[threadIdx.x] = __ldg(A.tables + (size_t)v * SK_TABLE_WORDS + threadIdx.x); // SK_THREADS == 256
+		if (s_grp) for (uint32_t g = threadIdx.x; g < n_groups; g += SK_THREADS) s_grp[g] = 0;
 		__syncthreads();
-		for (uint32_t base = 0; base < n_groups; base += SK_THREADS) {
-			const uint32_t g = base + threadIdx.x;
-			const uint32_t cnt = g < n_groups ? __ldcg(A.group_count + g) : 0u;
-			uint32_t total;
-			const uint32_t carry = s_carry; // read before the scan's barriers: thread 0 moves it on behind them
-			const uint32_t off = carry + block_exclusive_scan(cnt, s_warp, &total);
-			if (g < n_groups) {
-				if (s_grp) s_grp[g] += off; // cursor of this block inside the group, absolute
-				if (blockIdx.x == 0) {
-					A.group_offset[g] = off;
-					if (!s_grp) A.group_cursor[g] = off;
-					if (cnt) {
-						const uint32_t slot = atomicAdd(&A.counts[CNT_KEYS], 1u);
-						if (slot < P.cap_keys) {
-							A.keys[slot] = (uint64_t)g | SORT_KEY_INSTANCED_FLAG | ((uint64_t)P.view.layer_to_bucket[A.group_layer[g]] << SORT_KEY_BUCKET_SHIFT); // :100-102
-							A.values[slot] = (uint64_t)g | ((uint64_t)0 << SORT_VALUE_INSTANCER_SHIFT) | ((uint64_t)DRAW_AUTOINSTANCED << SORT_VALUE_TYPE_SHIFT); // :141-143
+		// the three segments as one index space: [MESH | DECAL | CURVE_DECAL]
+		const uint32_t n_mesh = __ldg(cull_counters + RT_MESH), n_decal = __ldg(cull_counters + RT_DECAL), n_curve = __ldg(cull_counters + RT_CURVE_DECAL);
+		const uint32_t n_all = n_mesh + n_decal + n_curve;
+		const float lod_multiplier_rcp = LB_FDIV(1.0f, W.lod_multiplier); // :3798-3799
+
+		// ---- pass 1: decide + count ----
+		// The walk is a random gather by entity id: the id of the thread's NEXT renderable is read one iteration ahead and its record is
+		// requested into L2 while the current one is processed (a dependent chain id -> record -> model -> mesh per renderable otherwise).
+		Counts c = {0u, 0u, 0u};
+		{
+			uint32_t i = blockIdx.x * SK_THREADS + threadIdx.x;
+			uint32_t e = i < n_all ? visible_at(P, visible, i, n_mesh, n_decal) : 0u;
+			const uint32_t ahead = P.prefetch_ahead * stride;
+			for (; i < n_all; i += stride) {
+				const uint32_t i_next = i + stride;
+				uint32_t e_next = 0;
+				if (i_next < n_all) e_next = visible_at(P, visible, i_next, n_mesh, n_decal);
+				if (ahead) {
+					const uint32_t i_pf = i + ahead;
+					if (i_pf < n_all) {
+						const uint32_t e_pf = ahead == stride ? e_next : visible_at(P, visible, i_pf, n_mesh, n_decal);
+						if (i_pf < n_mesh) { prefetch_l2(A.ent + e_pf); prefetch_l2(reinterpret_cast<const char*>(A.ent + e_pf) + 32); }
+						else { prefetch_l2(A.decal_layer + e_pf); prefetch_l2(A.decal_sort_key + e_pf); }
+					}
+				}
+				if (i < n_mesh) A.stash[i] = mesh_count(W, O, A, s_bucket_map, s_grp, lod_multiplier_rcp, (int32_t)e, i, c);
+				else { // DECAL / CURVE_DECAL renderable (:3840-3867): one key if its layer is in the view; bucket and material sort key stashed for pass 2
+					const uint32_t bucket = (uint8_t)s_bucket_map[A.decal_layer[e]];
+					uint32_t key = 0;
+					if (bucket < 0xff) { key = A.decal_sort_key[e]; ++c.k; }
+					A.stash[i] = bucket;
+					A.stash4[i].x = __uint_as_float(key);
+				}
+				e = e_next;
+			}
+		}
+		uint32_t tk, tp;
+		const uint32_t pk = block_exclusive_scan(c.k, s_warp, &tk);
+		const uint32_t pp = block_exclusive_scan(c.p, s_warp, &tp);
+		if (threadIdx.x == 0) {
+			s_base[0] = tk ? atomicAdd(&O.counts[CNT_KEYS], tk) : 0u;
+			s_base[1] = tp ? atomicAdd(&O.counts[CNT_POSE], tp) : 0u;
+		}
+		// the block's slice of every group it has instances of: count -> start inside the group
+		if (s_grp) for (uint32_t g = threadIdx.x; g < n_groups; g += SK_THREADS) if (s_grp[g]) s_grp[g] = atomicAdd(&O.group_count[g], s_grp[g]);
+		grid_barrier(A.bar, barriers_passed); // every block's counts are in: group totals are final; the view's lod / pose_frame stores are visible
+
+		// ---- group offsets = exclusive scan of the group totals; block 0 publishes them and one key/value per non-empty group (:3958-3969) ----
+		if (s_grp || blockIdx.x == 0) {
+			const uint8_t* __restrict__ layer_to_bucket = reinterpret_cast<const uint8_t*>(A.tables + (size_t)v * SK_TABLE_WORDS + 256);
+			if (threadIdx.x == 0) s_carry = 0;
+			__syncthreads();
+			for (uint32_t base = 0; base < n_groups; base += SK_THREADS) {
+				const uint32_t g = base + threadIdx.x;
+				const uint32_t cnt = g < n_groups ? __ldcg(O.group_count + g) : 0u;
+				uint32_t total;
+				const uint32_t carry = s_carry; // read before the scan's barriers: thread 0 moves it on behind them
+				const uint32_t off = carry + block_exclusive_scan(cnt, s_warp, &total);
+				if (g < n_groups) {
+					if (s_grp) s_grp[g] += off; // cursor of this block inside the group, absolute
+					if (blockIdx.x == 0) {
+						O.group_offset[g] = off;
+						if (!s_grp) O.group_cursor[g] = off;
+						if (cnt) {
+							const uint32_t slot = atomicAdd(&O.counts[CNT_KEYS], 1u);
+							if (slot < P.cap_keys) {
+								O.keys[slot] = (uint64_t)g | SORT_KEY_INSTANCED_FLAG | ((uint64_t)__ldg(layer_to_bucket + A.group_layer[g]) << SORT_KEY_BUCKET_SHIFT); // :100-102
+								O.values[slot] = (uint64_t)g | ((uint64_t)0 << SORT_VALUE_INSTANCER_SHIFT) | ((uint64_t)DRAW_AUTOINSTANCED << SORT_VALUE_TYPE_SHIFT); // :141-143
+							}
 						}
 					}
 				}
+				if (threadIdx.x == 0) s_carry += total;
+				__syncthreads();
 			}
-			if (threadIdx.x == 0) s_carry += total;
-			__syncthreads();
+			if (blockIdx.x == 0 && threadIdx.x == 0) { O.counts[CNT_INST] = s_carry; O.counts[CNT_RECS] = s_carry; }
 		}
-		if (blockIdx.x == 0 && threadIdx.x == 0) { A.counts[CNT_INST] = s_carry; A.counts[CNT_RECS] = s_carry; }
-	}
-	if (!s_grp) grid_barrier(A.bar, barriers_passed); // more groups than fit in shared memory: everybody waits for block 0's cursors in HBM
+		if (!s_grp) grid_barrier(A.bar, barriers_passed); // more groups than fit in shared memory: everybody waits for block 0's cursors in HBM
 
-	// ---- pass 2: write ----
-	uint32_t k = s_base[0] + pk, p = s_base[1] + pp;
-	{
-		uint32_t i = blockIdx.x * SK_THREADS + threadIdx.x;
-		uint32_t e = i < n_all ? visible_at(P, visible, i, n_mesh, n_decal) : 0u;
-		for (; i < n_all; i += stride) {
-			const uint32_t i_next = i + stride;
-			uint32_t e_next = 0;
-			if (i_next < n_all) e_next = visible_at(P, visible, i_next, n_mesh, n_decal);
-			if (i < n_mesh) mesh_write(P, A, s_bucket_map, s_grp, (int32_t)e, i, A.stash[i], k, p);
-			else {
-				const bool curve = i >= n_mesh + n_decal;
-				const uint32_t bucket = A.stash[i];
-				if (bucket < 0xff) push_key(P, A, k, (uint64_t)__float_as_uint(A.stash4[i].x) | ((uint64_t)bucket << SORT_KEY_BUCKET_SHIFT),
-					sext((int32_t)e) | ((uint64_t)(curve ? DRAW_CURVE_DECAL : DRAW_DECAL) << SORT_VALUE_TYPE_SHIFT));
+		// ---- pass 2: write ----
+		uint32_t k = s_base[0] + pk, p = s_base[1] + pp;
+		{
+			uint32_t i = blockIdx.x * SK_THREADS + threadIdx.x;
+			uint32_t e = i < n_all ? visible_at(P, visible, i, n_mesh, n_decal) : 0u;
+			for (; i < n_all; i += stride) {
+				const uint32_t i_next = i + stride;
+				uint32_t e_next = 0;
+				if (i_next < n_all) e_next = visible_at(P, visible, i_next, n_mesh, n_decal);
+				if (i < n_mesh) mesh_write(P, W, O, A, s_bucket_map, s_grp, (int32_t)e, i, A.stash[i], k, p);
+				else {
+					const bool curve = i >= n_mesh + n_decal;
+					const uint32_t bucket = A.stash[i];
+					if (bucket < 0xff) push_key(P, O, k, (uint64_t)__float_as_uint(A.stash4[i].x) | ((uint64_t)bucket << SORT_KEY_BUCKET_SHIFT),
+						sext((int32_t)e) | ((uint64_t)(curve ? DRAW_CURVE_DECAL : DRAW_DECAL) << SORT_VALUE_TYPE_SHIFT));
+				}
+				e = e_next;
 			}
-			e = e_next;
 		}
 	}
 }
@@ -457,6 +490,20 @@ __global__ void reset_word_kernel(uint32_t* w) { *w = 0; }
 } // namespace
 
 constexpr uint32_t NO_MODEL = 0xffffffffu;
+constexpr uint32_t SK_TABLE_SLOTS = 4; // pinned staging slots of the view tables: a copy waits for the one SK_TABLE_SLOTS copies before it
+
+namespace {
+// What create_keys leaves in HBM for n views: view v's part of each array at + v x its per-view size (EmitArgs).  The plain create_keys
+// writes a set of one view, create_keys_views a set of its own.
+struct OutputSet {
+	uint32_t n_views = 0;
+	DeviceArray<uint64_t> keys, values;                            // [n_views][cap_keys]
+	DeviceArray<uint32_t> counts; PinnedArray<uint32_t> h_counts;  // [n_views][CNT_WORDS]
+	DeviceArray<uint32_t> group_count, group_offset, group_cursor; // [n_views][max_groups]; a launch's views lie n_groups apart
+	DeviceArray<uint64_t> group_renderables; DeviceArray<float4> instance_data; // [n_views][cap_recs], [n_views][3 cap_recs]
+	DeviceArray<uint32_t> pose_list, dirty_list;                   // [n_views][max_entities]
+};
+} // namespace
 
 struct lb200_sortkeys {
 	lb200_ctx* ctx = nullptr;
@@ -468,23 +515,26 @@ struct lb200_sortkeys {
 	DeviceArray<uint32_t> d_decal_sort_key; DeviceArray<uint8_t> d_decal_layer;
 	DeviceArray<lb200_sk_model> d_models; DeviceArray<lb200_sk_mesh> d_meshes; // both set or both empty (lb200_sortkeys_set_models)
 	DeviceArray<uint8_t> d_group_layer; // layer of the mesh material a sort key (= auto-instancer group) belongs to
+	// the views' bucket_map + layer_to_bucket (SK_TABLE_WORDS each): copied from a pinned slot when they differ from what the device holds
+	DeviceArray<uint32_t> d_tables; PinnedArray<uint32_t> h_tables; Event tables_copied[SK_TABLE_SLOTS];
+	uint32_t table_slot = 0, tables_views = 0; // next pinned slot; views whose tables d_tables holds (0 = none yet)
+	uint32_t tables_now[SK_MAX_VIEWS * SK_TABLE_WORDS] = {};   // ... and what they are
 	// outputs
-	DeviceArray<uint64_t> d_keys[2], d_values[2];
-	DeviceArray<uint32_t> d_counts; PinnedArray<uint32_t> h_counts;
-	DeviceArray<uint32_t> d_group_count, d_group_offset, d_group_cursor;
-	DeviceArray<uint64_t> d_group_renderables; DeviceArray<float4> d_instance_data;
-	DeviceArray<uint32_t> d_pose_list, d_dirty_list, d_stash; DeviceArray<float4> d_stash4; // the two passes' hand-over: one word + 3 x float4 per visible renderable
+	OutputSet plain;                   // lb200_sortkeys_create_keys
+	OutputSet views;                   // lb200_sortkeys_create_keys_views, grown to the most views a call had
+	uint32_t views_n = 0, views_groups = 0; // views and group-table stride of the latest create_keys_views (0 = none yet)
+	DeviceArray<uint64_t> d_keys_alt, d_values_alt; // the sort's alternate buffers, shared by every view of both sets
+	DeviceArray<uint32_t> d_stash; DeviceArray<float4> d_stash4; // the two passes' hand-over: one word + 3 x float4 per visible renderable
 	DeviceArray<float> d_lod; DeviceArray<uint32_t> d_pose_frame; // unpacked on request (lb200_sortkeys_device_outputs)
 	DeviceArray<uint32_t> d_moved_list, d_moved_count; DeviceArray<lb200_transform> d_prev; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move onwards)
 	DeviceArray<GridBar> d_bar;
-	RadixSortScratch radix_scratch; // the sort of d_keys / d_values, with d_keys[1] / d_values[1] as its alternate buffers
-	uint32_t last_groups = 0;
+	RadixSortScratch radix_scratch; // the sort of every view's keys / values, with d_keys_alt / d_values_alt as its alternate buffers
 	uint32_t max_mesh_sort_key = 0; // largest sort key of the mesh table: every view's max_sort_key must reach it
 	uint32_t model_past_table = NO_MODEL; // first model whose meshes leave the mesh table (create_keys refuses to launch), NO_MODEL if none
 	char past_table_text[128] = {};
 	uint32_t keys_grid_limit[2] = {0, 0}; // co-resident blocks of create_keys_kernel: group counters in shared memory / in HBM
 	// lb200_sortkeys_set_launch (blocks 0 = environment switch, else 2 per SM; -1 = all co-resident; prefetch -1 = environment switch) and
-	// what the last create_keys launched
+	// what the last create_keys / create_keys_views launched
 	int launch_blocks = 0, launch_prefetch = -1;
 	uint32_t last_grid = 0, last_prefetch = 0;
 	int last_in_smem = 0;
@@ -498,6 +548,164 @@ template <typename T> int upload_temp(lb200_ctx* ctx, const T* host, size_t n, D
 	LB200_CUDA(ctx, cudaMemcpyAsync(dev, host, sizeof(T) * n, cudaMemcpyHostToDevice, ctx->stream));
 	return LB200_OK;
 }
+
+// An output set of n views, allocated whole before it replaces `out` (on failure `out` is left as it was)
+int alloc_outputs(const lb200_sortkeys* sk, uint32_t n, OutputSet& out) {
+	lb200_ctx* ctx = sk->ctx;
+	const size_t keys = (size_t)n * sk->cap_keys, recs = (size_t)n * sk->cap_recs, groups = (size_t)n * sk->max_groups, lists = (size_t)n * sk->max_entities;
+	OutputSet o;
+	o.n_views = n;
+	LB200_CUDA(ctx, o.keys.alloc(keys));
+	LB200_CUDA(ctx, o.values.alloc(keys));
+	LB200_CUDA(ctx, o.counts.alloc((size_t)n * CNT_WORDS));
+	LB200_CUDA(ctx, o.h_counts.alloc((size_t)n * CNT_WORDS));
+	LB200_CUDA(ctx, o.group_count.alloc(groups));
+	LB200_CUDA(ctx, o.group_offset.alloc(groups));
+	LB200_CUDA(ctx, o.group_cursor.alloc(groups));
+	LB200_CUDA(ctx, o.group_renderables.alloc(recs));
+	LB200_CUDA(ctx, o.instance_data.alloc(3 * recs)); // 48 bytes per instance
+	LB200_CUDA(ctx, o.pose_list.alloc(lists));
+	LB200_CUDA(ctx, o.dirty_list.alloc(lists));
+	out = std::move(o);
+	return LB200_OK;
+}
+
+// What create_keys checks of one view against the tables and the culling system (LB200_ERR_INVALID)
+int check_view(lb200_sortkeys* sk, const lb200_sk_view& view) {
+	lb200_ctx* ctx = sk->ctx;
+	if (view.max_sort_key >= sk->max_groups) { lb200_set_error(ctx, "view.max_sort_key %u >= max_groups %u", view.max_sort_key, sk->max_groups); return LB200_ERR_INVALID; }
+	if (sk->model_past_table != NO_MODEL) { lb200_set_error(ctx, "create_keys: %s", sk->past_table_text); return LB200_ERR_INVALID; }
+	if (view.max_sort_key < sk->max_mesh_sort_key) { lb200_set_error(ctx, "view.max_sort_key %u < sort key %u of the mesh table", view.max_sort_key, sk->max_mesh_sort_key); return LB200_ERR_INVALID; }
+	return LB200_OK;
+}
+int check_entity_range(lb200_sortkeys* sk, lb200_culling* cs) {
+	// the kernel indexes the entity records, the decal arrays and the stash by the culled ids without a bounds check
+	const uint32_t entity_range = lb200_culling_internal_entity_range(cs);
+	if (entity_range > sk->max_entities) { lb200_set_error(sk->ctx, "the culling system holds entity ids up to %u, max_entities is %u", entity_range - 1, sk->max_entities); return LB200_ERR_INVALID; }
+	return LB200_OK;
+}
+
+// The views' bucket_map + layer_to_bucket into d_tables, unless d_tables holds them already
+int upload_tables(lb200_sortkeys* sk, const lb200_sk_view* views, uint32_t n) {
+	lb200_ctx* ctx = sk->ctx;
+	uint32_t t[SK_MAX_VIEWS * SK_TABLE_WORDS];
+	for (uint32_t v = 0; v < n; ++v) {
+		memcpy(t + v * SK_TABLE_WORDS, views[v].bucket_map, sizeof(views[v].bucket_map));
+		memcpy(t + v * SK_TABLE_WORDS + 256, views[v].layer_to_bucket, sizeof(views[v].layer_to_bucket));
+	}
+	const size_t bytes = sizeof(uint32_t) * SK_TABLE_WORDS * n;
+	if (n <= sk->tables_views && !memcmp(t, sk->tables_now, bytes)) return LB200_OK;
+	const uint32_t slot = sk->table_slot;
+	uint32_t* h = sk->h_tables + (size_t)slot * SK_MAX_VIEWS * SK_TABLE_WORDS;
+	LB200_CUDA(ctx, cudaEventSynchronize(sk->tables_copied[slot])); // the copy that last used this slot has been made
+	memcpy(h, t, bytes);
+	sk->tables_views = 0; // unknown until the copy is enqueued
+	LB200_CUDA(ctx, cudaMemcpyAsync(sk->d_tables, h, bytes, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaEventRecord(sk->tables_copied[slot], ctx->stream));
+	sk->table_slot = (slot + 1) % SK_TABLE_SLOTS;
+	memcpy(sk->tables_now, t, bytes);
+	sk->tables_views = n;
+	return LB200_OK;
+}
+
+// view v of `set`, whose group tables lie `groups` apart
+ViewOut view_out(const lb200_sortkeys* sk, const OutputSet& set, uint32_t v, uint32_t groups) {
+	const size_t k = (size_t)v * sk->cap_keys, r = (size_t)v * sk->cap_recs, g = (size_t)v * groups, l = (size_t)v * sk->max_entities;
+	return {set.keys + k, set.values + k, set.counts + (size_t)v * CNT_WORDS, set.group_count + g, set.group_offset + g, set.group_cursor + g,
+		set.group_renderables + r, set.instance_data + 3 * r, set.pose_list + l, set.dirty_list + l};
+}
+void view_pointers(const lb200_sortkeys* sk, const OutputSet& set, uint32_t v, uint32_t groups, lb200_sk_outputs* out) {
+	const ViewOut o = view_out(sk, set, v, groups);
+	out->keys = o.keys; out->values = o.values; out->group_count = o.group_count; out->group_offset = o.group_offset;
+	out->group_renderables = o.group_renderables; out->instance_data = o.instance_data; out->pose_list = o.pose_list; out->dirty_list = o.dirty_list;
+}
+
+// createSortKeys of cv's views [0, n) into `out` (one cooperative launch), + radixSort of each view if `sort`, + one read-back of every view's
+// counters into results[0, n) if `want_counts`
+int launch_keys(lb200_sortkeys* sk, const CullViewsResult& cv, const lb200_sk_view* views, uint32_t n, OutputSet& out, int sort, int want_counts, lb200_sk_result* results) {
+	lb200_ctx* ctx = sk->ctx;
+	cudaStream_t s = ctx->stream;
+	int rc = upload_tables(sk, views, n);
+	if (rc) return rc;
+	uint32_t n_groups = views[0].max_sort_key + 1;
+	LB200_CUDA(ctx, cudaMemsetAsync(out.counts, 0, sizeof(uint32_t) * CNT_WORDS * n, s));
+	LB200_CUDA(ctx, cudaMemsetAsync(out.group_count, 0, sizeof(uint32_t) * n_groups * n, s));
+	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_bar, 0, sizeof(GridBar), s));
+	EmitParams EP = {};
+	for (uint32_t v = 0; v < n; ++v) {
+		ViewScalars& w = EP.view[v];
+		for (int c = 0; c < 3; ++c) { w.camera_pos[c] = views[v].camera_pos[c]; w.lod_ref_point[c] = views[v].lod_ref_point[c]; }
+		w.time_delta = views[v].time_delta; w.lod_multiplier = views[v].lod_multiplier; w.frame_number = views[v].frame_number; w.is_shadow = views[v].is_shadow;
+	}
+	EP.n_views = n;
+	for (int t = 0; t < 4; ++t) EP.type_base[t] = cv.type_base[t];
+	EP.id_stride = cv.id_stride; EP.counter_stride = cv.counter_stride;
+	EP.cap_keys = sk->cap_keys; EP.cap_recs = sk->cap_recs; EP.cap_pose = sk->max_entities; EP.cap_dirty = sk->max_entities;
+	static const uint32_t prefetch_ahead = [] { const char* e = getenv("LB200_SK_PREFETCH"); const int v = e ? atoi(e) : 0; return (uint32_t)std::max(0, std::min(v, 4)); }(); // off: on H100 the prefetch slows the pass (DESIGN.md 4.5)
+	EP.prefetch_ahead = sk->launch_prefetch >= 0 ? (uint32_t)sk->launch_prefetch : prefetch_ahead;
+	const bool in_smem = n_groups <= SK_SMEM_GROUPS;
+	size_t smem = in_smem ? sizeof(uint32_t) * n_groups : 0;
+	uint32_t& limit = sk->keys_grid_limit[in_smem ? 0 : 1];
+	if (!limit) { // co-resident blocks with the largest group table this path can ask for, so that the number holds for every view
+		rc = lb200_coop_grid_limit(ctx,(const void*)create_keys_kernel, SK_THREADS, in_smem ? sizeof(uint32_t) * SK_SMEM_GROUPS : 0, &limit);
+		if (rc) return rc;
+	}
+	const uint32_t work = cv.type_counts[RT_MESH] + cv.type_counts[RT_DECAL] + cv.type_counts[RT_CURVE_DECAL]; // upper bound of any view's visible renderables
+	static const uint32_t blocks_per_sm = [] { const char* e = getenv("LB200_SK_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 2; return (uint32_t)std::max(0, v); }(); // fewer resident blocks than fit (0 = all): 2 is fastest on H100
+	uint32_t grid = std::max(1u, std::min(blocks_per_sm ? std::min(limit, blocks_per_sm * (uint32_t)ctx->sm_count) : limit, (work + SK_THREADS - 1) / SK_THREADS));
+	if (sk->launch_blocks < 0) grid = limit; // lb200_sortkeys_set_launch: not capped by the work, so that threads with nothing to do still take part
+	else if (sk->launch_blocks > 0) grid = std::min((uint32_t)sk->launch_blocks, limit);
+	for (uint32_t v = 0; v < n; ++v) EP.out[v] = view_out(sk, out, v, n_groups);
+	EmitArgs EA = {sk->d_ent, sk->d_decal_sort_key, sk->d_decal_layer, sk->d_models, sk->d_meshes, sk->d_tables, sk->d_group_layer, sk->d_stash, sk->d_stash4, sk->max_entities, sk->d_bar};
+	const uint32_t* visible = cv.ids;
+	const uint32_t* cull_counters = cv.counters;
+	void* args[] = {&EP, &visible, &cull_counters, &EA, &n_groups};
+	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)create_keys_kernel, dim3(grid), dim3(SK_THREADS), args, smem, s));
+	LB200_CHECK_LAUNCH(ctx);
+	sk->last_grid = grid; sk->last_in_smem = in_smem ? 1 : 0; sk->last_prefetch = EP.prefetch_ahead;
+	if (sort) {
+		lb200_range r2("radixSort"); // pipeline.cpp:4101
+		for (uint32_t v = 0; v < n; ++v) { // every view: whether a view has keys is known on the device only
+			const size_t at = (size_t)v * sk->cap_keys;
+			rc = lb200_radix_sort_pairs(ctx, s, out.keys + at, sk->d_keys_alt, out.values + at, sk->d_values_alt, out.counts + v * CNT_WORDS + CNT_KEYS, sk->cap_keys,
+				sk->radix_scratch, 0, false, nullptr);
+			if (rc) return rc;
+		}
+	}
+	if (want_counts) {
+		if (!results) return LB200_ERR_INVALID;
+		LB200_CUDA(ctx, cudaMemcpyAsync(out.h_counts, out.counts, sizeof(uint32_t) * CNT_WORDS * n, cudaMemcpyDeviceToHost, s));
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		rc = LB200_OK;
+		for (uint32_t v = 0; v < n; ++v) {
+			const uint32_t* hc = out.h_counts + v * CNT_WORDS;
+			lb200_sk_result& r = results[v];
+			r.n_keys = hc[CNT_KEYS]; r.n_instances = hc[CNT_INST]; r.n_pose = hc[CNT_POSE]; r.n_dirty = hc[CNT_DIRTY]; r.n_groups = n_groups;
+			if (!rc && (r.n_keys > sk->cap_keys || hc[CNT_RECS] > sk->cap_recs)) {
+				lb200_set_error(ctx, "create_keys: view %u: %u keys / %u instances exceed the capacities %u / %u", v, r.n_keys, hc[CNT_RECS], sk->cap_keys, sk->cap_recs);
+				rc = LB200_ERR_CAPACITY;
+			}
+		}
+		return rc;
+	}
+	return LB200_OK;
+}
+
+// ModelInstance::lod / Pose::frame unpacked from the entity records into plain arrays (on the context stream)
+int unpack_state(lb200_sortkeys* sk, lb200_sk_outputs* out) {
+	lb200_ctx* ctx = sk->ctx;
+	if (!sk->d_lod || !sk->d_pose_frame) {
+		DeviceArray<float> lod; DeviceArray<uint32_t> pose_frame;
+		LB200_CUDA(ctx, lod.alloc(sk->max_entities));
+		LB200_CUDA(ctx, pose_frame.alloc(sk->max_entities));
+		sk->d_lod = std::move(lod); sk->d_pose_frame = std::move(pose_frame);
+	}
+	ent_unpack_state_kernel<<<(sk->max_entities + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, sk->d_lod, sk->d_pose_frame);
+	LB200_CHECK_LAUNCH(ctx);
+	out->lod = sk->d_lod; out->pose_frame = sk->d_pose_frame;
+	return LB200_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -519,26 +727,20 @@ int lb200_sortkeys_create(lb200_ctx* ctx, uint32_t max_entities, uint32_t max_gr
 	LB200_CUDA(ctx, sk->d_decal_layer.alloc(E));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_decal_sort_key, 0, sizeof(uint32_t) * E, ctx->stream));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_decal_layer, 0, E, ctx->stream));
-	for (int b = 0; b < 2; ++b) {
-		LB200_CUDA(ctx, sk->d_keys[b].alloc(sk->cap_keys));
-		LB200_CUDA(ctx, sk->d_values[b].alloc(sk->cap_keys));
-	}
-	LB200_CUDA(ctx, sk->d_counts.alloc(CNT_WORDS));
-	LB200_CUDA(ctx, sk->h_counts.alloc(CNT_WORDS));
-	LB200_CUDA(ctx, sk->d_group_count.alloc(max_groups));
-	LB200_CUDA(ctx, sk->d_group_offset.alloc(max_groups));
-	LB200_CUDA(ctx, sk->d_group_cursor.alloc(max_groups));
+	int rc = alloc_outputs(sk.get(), 1, sk->plain);
+	if (rc) return rc;
+	LB200_CUDA(ctx, sk->d_keys_alt.alloc(sk->cap_keys));
+	LB200_CUDA(ctx, sk->d_values_alt.alloc(sk->cap_keys));
 	LB200_CUDA(ctx, sk->d_group_layer.alloc(max_groups));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_group_layer, 0, max_groups, ctx->stream));
-	LB200_CUDA(ctx, sk->d_group_renderables.alloc(sk->cap_recs));
-	LB200_CUDA(ctx, sk->d_instance_data.alloc(3 * (size_t)sk->cap_recs)); // 48 bytes per instance
-	LB200_CUDA(ctx, sk->d_pose_list.alloc(E));
-	LB200_CUDA(ctx, sk->d_dirty_list.alloc(E));
+	LB200_CUDA(ctx, sk->d_tables.alloc((size_t)SK_MAX_VIEWS * SK_TABLE_WORDS));
+	LB200_CUDA(ctx, sk->h_tables.alloc((size_t)SK_TABLE_SLOTS * SK_MAX_VIEWS * SK_TABLE_WORDS));
+	for (Event& ev : sk->tables_copied) LB200_CUDA(ctx, cudaEventCreateWithFlags(ev.create(), cudaEventDisableTiming));
 	LB200_CUDA(ctx, sk->d_stash.alloc(E));
 	LB200_CUDA(ctx, sk->d_stash4.alloc(3 * E));
 	LB200_CUDA(ctx, sk->d_bar.alloc(1));
 	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_bar, 0, sizeof(GridBar), ctx->stream));
-	const int rc = lb200_radix_sort_alloc_scratch(ctx, (uint32_t)ctx->sm_count * 2, sk->radix_scratch);
+	rc = lb200_radix_sort_alloc_scratch(ctx, (uint32_t)ctx->sm_count * 2, sk->radix_scratch);
 	if (rc) return rc;
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	*out = sk.release();
@@ -660,59 +862,47 @@ int lb200_sortkeys_create_keys(lb200_sortkeys* sk, lb200_culling* cs, const lb20
 	lb200_ctx* ctx = sk->ctx;
 	lb200_range range("create keys"); // pipeline.cpp:3818
 	if (!sk->have_transforms || !sk->d_models) { lb200_set_error(ctx, "create_keys needs set_models and set_transforms first"); return LB200_ERR_STATE; }
-	if (view->max_sort_key >= sk->max_groups) { lb200_set_error(ctx, "view.max_sort_key %u >= max_groups %u", view->max_sort_key, sk->max_groups); return LB200_ERR_INVALID; }
-	if (sk->model_past_table != NO_MODEL) { lb200_set_error(ctx, "create_keys: %s", sk->past_table_text); return LB200_ERR_INVALID; }
-	if (view->max_sort_key < sk->max_mesh_sort_key) { lb200_set_error(ctx, "view.max_sort_key %u < sort key %u of the mesh table", view->max_sort_key, sk->max_mesh_sort_key); return LB200_ERR_INVALID; }
-	const uint32_t *visible = nullptr, *cull_counters = nullptr, *type_base = nullptr, *type_counts = nullptr;
-	int rc = lb200_culling_internal_last(cs, &visible, &cull_counters, &type_base, &type_counts);
+	int rc = check_view(sk, *view);
 	if (rc) return rc;
-	// the kernel indexes the entity records, the decal arrays and the stash by the culled ids without a bounds check
-	const uint32_t entity_range = lb200_culling_internal_entity_range(cs);
-	if (entity_range > sk->max_entities) { lb200_set_error(ctx, "the culling system holds entity ids up to %u, max_entities is %u", entity_range - 1, sk->max_entities); return LB200_ERR_INVALID; }
-	cudaStream_t s = ctx->stream;
-	uint32_t n_groups = view->max_sort_key + 1;
-	sk->last_groups = n_groups;
-	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_counts, 0, sizeof(uint32_t) * CNT_WORDS, s));
-	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_group_count, 0, sizeof(uint32_t) * n_groups, s));
-	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_bar, 0, sizeof(GridBar), s));
-	EmitParams EP;
-	EP.view = *view;
-	for (int t = 0; t < 4; ++t) EP.type_base[t] = type_base[t];
-	EP.cap_keys = sk->cap_keys; EP.cap_recs = sk->cap_recs; EP.cap_pose = sk->max_entities; EP.cap_dirty = sk->max_entities;
-	static const uint32_t prefetch_ahead = [] { const char* e = getenv("LB200_SK_PREFETCH"); const int v = e ? atoi(e) : 0; return (uint32_t)std::max(0, std::min(v, 4)); }(); // off: on H100 the prefetch slows the pass (DESIGN.md 4.5)
-	EP.prefetch_ahead = sk->launch_prefetch >= 0 ? (uint32_t)sk->launch_prefetch : prefetch_ahead;
-	const bool in_smem = n_groups <= SK_SMEM_GROUPS;
-	size_t smem = in_smem ? sizeof(uint32_t) * n_groups : 0;
-	uint32_t& limit = sk->keys_grid_limit[in_smem ? 0 : 1];
-	if (!limit) { // co-resident blocks with the largest group table this path can ask for, so that the number holds for every view
-		rc = lb200_coop_grid_limit(ctx,(const void*)create_keys_kernel, SK_THREADS, in_smem ? sizeof(uint32_t) * SK_SMEM_GROUPS : 0, &limit);
+	CullViewsResult cv = {1, 0, 0, nullptr, nullptr, nullptr, nullptr};
+	rc = lb200_culling_internal_last(cs, &cv.ids, &cv.counters, &cv.type_base, &cv.type_counts);
+	if (rc) return rc;
+	rc = check_entity_range(sk, cs);
+	if (rc) return rc;
+	return launch_keys(sk, cv, view, 1, sk->plain, sort, want_counts, result);
+}
+
+int lb200_sortkeys_create_keys_views(lb200_sortkeys* sk, lb200_culling* cs, const lb200_sk_view* views, uint32_t n_views, int sort, int want_counts, lb200_sk_result* results) {
+	if (!sk || !cs || !views || (want_counts && !results)) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = sk->ctx;
+	lb200_range range("create keys"); // pipeline.cpp:3818
+	if (n_views < 1 || n_views > SK_MAX_VIEWS) { lb200_set_error(ctx, "create_keys_views: n_views %u is not 1..%u", n_views, SK_MAX_VIEWS); return LB200_ERR_INVALID; }
+	if (!sk->have_transforms || !sk->d_models) { lb200_set_error(ctx, "create_keys_views needs set_models and set_transforms first"); return LB200_ERR_STATE; }
+	CullViewsResult cv;
+	int rc = lb200_culling_internal_views(cs, &cv);
+	if (rc) return rc;
+	if (n_views != cv.n_views) { lb200_set_error(ctx, "create_keys_views: %u views, the latest cull_views culled %u", n_views, cv.n_views); return LB200_ERR_INVALID; }
+	for (uint32_t v = 0; v < n_views; ++v) {
+		// Renderer::getMaxSortKey() is renderer-wide: it sizes the launch's group tables
+		if (views[v].max_sort_key != views[0].max_sort_key) {
+			lb200_set_error(ctx, "create_keys_views: view %u has max_sort_key %u, view 0 %u", v, views[v].max_sort_key, views[0].max_sort_key);
+			return LB200_ERR_INVALID;
+		}
+		rc = check_view(sk, views[v]);
 		if (rc) return rc;
 	}
-	const uint32_t work = type_counts[RT_MESH] + type_counts[RT_DECAL] + type_counts[RT_CURVE_DECAL]; // upper bound of visible renderables
-	static const uint32_t blocks_per_sm = [] { const char* e = getenv("LB200_SK_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 2; return (uint32_t)std::max(0, v); }(); // fewer resident blocks than fit (0 = all): 2 is fastest on H100
-	uint32_t grid = std::max(1u, std::min(blocks_per_sm ? std::min(limit, blocks_per_sm * (uint32_t)ctx->sm_count) : limit, (work + SK_THREADS - 1) / SK_THREADS));
-	if (sk->launch_blocks < 0) grid = limit; // lb200_sortkeys_set_launch: not capped by the work, so that threads with nothing to do still take part
-	else if (sk->launch_blocks > 0) grid = std::min((uint32_t)sk->launch_blocks, limit);
-	EmitArgs EA = {sk->d_ent, sk->d_decal_sort_key, sk->d_decal_layer, sk->d_models, sk->d_meshes, sk->d_keys[0], sk->d_values[0], sk->d_counts,
-		sk->d_group_count, sk->d_group_offset, sk->d_group_cursor, sk->d_group_layer, sk->d_group_renderables, sk->d_instance_data, sk->d_pose_list, sk->d_dirty_list, sk->d_stash, sk->d_stash4, sk->max_entities, sk->d_bar};
-	void* args[] = {&EP, &visible, &cull_counters, &EA, &n_groups};
-	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)create_keys_kernel, dim3(grid), dim3(SK_THREADS), args, smem, s));
-	LB200_CHECK_LAUNCH(ctx);
-	sk->last_grid = grid; sk->last_in_smem = in_smem ? 1 : 0; sk->last_prefetch = EP.prefetch_ahead;
-	if (sort) {
-		lb200_range r2("radixSort"); // pipeline.cpp:4101
-		rc = lb200_radix_sort_pairs(ctx, s, sk->d_keys[0], sk->d_keys[1], sk->d_values[0], sk->d_values[1], sk->d_counts + CNT_KEYS, sk->cap_keys, sk->radix_scratch, 0, false, nullptr);
+	rc = check_entity_range(sk, cs);
+	if (rc) return rc;
+	if (sk->views.n_views < n_views) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // nothing enqueued still uses the old set
+		sk->views_n = 0;
+		sk->views = OutputSet();
+		rc = alloc_outputs(sk, n_views, sk->views);
 		if (rc) return rc;
 	}
-	if (want_counts) {
-		if (!result) return LB200_ERR_INVALID;
-		LB200_CUDA(ctx, cudaMemcpyAsync(sk->h_counts, sk->d_counts, sizeof(uint32_t) * CNT_WORDS, cudaMemcpyDeviceToHost, s));
-		LB200_CUDA(ctx, cudaStreamSynchronize(s));
-		result->n_keys = sk->h_counts[CNT_KEYS]; result->n_instances = sk->h_counts[CNT_INST]; result->n_pose = sk->h_counts[CNT_POSE];
-		result->n_dirty = sk->h_counts[CNT_DIRTY]; result->n_groups = n_groups;
-		if (result->n_keys > sk->cap_keys || sk->h_counts[CNT_RECS] > sk->cap_recs) { lb200_set_error(ctx, "create_keys: %u keys / %u instances exceed the capacities %u / %u", result->n_keys, sk->h_counts[CNT_RECS], sk->cap_keys, sk->cap_recs); return LB200_ERR_CAPACITY; }
-	}
-	return LB200_OK;
+	sk->views_n = n_views;
+	sk->views_groups = views[0].max_sort_key + 1;
+	return launch_keys(sk, cv, views, n_views, sk->views, sort, want_counts, results);
 }
 
 int lb200_sortkeys_set_launch(lb200_sortkeys* sk, int blocks, int prefetch_ahead) {
@@ -736,18 +926,20 @@ int lb200_sortkeys_get_launch(lb200_sortkeys* sk, uint32_t* grid, int* groups_in
 // lod / pose-frame state is unpacked from the entity records into plain arrays for the caller (on the context stream)
 int lb200_sortkeys_device_outputs(lb200_sortkeys* sk, lb200_sk_outputs* out) {
 	if (!sk || !out) return LB200_ERR_INVALID;
-	lb200_ctx* ctx = sk->ctx;
-	if (!sk->d_lod || !sk->d_pose_frame) {
-		DeviceArray<float> lod; DeviceArray<uint32_t> pose_frame;
-		LB200_CUDA(ctx, lod.alloc(sk->max_entities));
-		LB200_CUDA(ctx, pose_frame.alloc(sk->max_entities));
-		sk->d_lod = std::move(lod); sk->d_pose_frame = std::move(pose_frame);
-	}
-	ent_unpack_state_kernel<<<(sk->max_entities + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, sk->d_lod, sk->d_pose_frame);
-	LB200_CHECK_LAUNCH(ctx);
-	out->keys = sk->d_keys[0]; out->values = sk->d_values[0]; out->group_count = sk->d_group_count; out->group_offset = sk->d_group_offset;
-	out->group_renderables = sk->d_group_renderables; out->instance_data = sk->d_instance_data; out->pose_list = sk->d_pose_list; out->dirty_list = sk->d_dirty_list;
-	out->lod = sk->d_lod; out->pose_frame = sk->d_pose_frame;
+	const int rc = unpack_state(sk, out);
+	if (rc) return rc;
+	view_pointers(sk, sk->plain, 0, sk->max_groups, out);
+	return LB200_OK;
+}
+
+// the same for view k of the latest create_keys_views (valid until the next one)
+int lb200_sortkeys_view_outputs(lb200_sortkeys* sk, uint32_t k, lb200_sk_outputs* out) {
+	if (!sk || !out) return LB200_ERR_INVALID;
+	if (!sk->views_n) { lb200_set_error(sk->ctx, "view_outputs needs a preceding create_keys_views"); return LB200_ERR_STATE; }
+	if (k >= sk->views_n) { lb200_set_error(sk->ctx, "view_outputs: view %u of a create_keys_views call of %u views", k, sk->views_n); return LB200_ERR_INVALID; }
+	const int rc = unpack_state(sk, out);
+	if (rc) return rc;
+	view_pointers(sk, sk->views, k, sk->views_groups, out);
 	return LB200_OK;
 }
 

@@ -104,6 +104,16 @@ class SortKeys:
         self._err(self.L.lb200_sortkeys_create_keys(self.h, culling.h, ptr(view), C.c_int(1 if sort else 0), C.c_int(1 if want_counts else 0), C.byref(res)))
         return res if want_counts else None
 
+    def createSortKeysViews(self, culling, views, sort=True, want_counts=True):
+        """For every view of the latest cull_views on `culling`, in one launch: the same as select_view(v) + createSortKeys(views[v]) for
+        v = 0, 1, ... (later views see the lod / Pose::frame the earlier ones left), each view into outputs of its own that readView(k)
+        reads.  -> list of SkResult, one per view (None if not want_counts: nothing is read back, nothing waits)."""
+        views = np.ascontiguousarray(np.concatenate([np.asarray(v, SK_VIEW_DTYPE).reshape(-1) for v in views]) if len(views) else np.zeros(0, SK_VIEW_DTYPE))
+        res = (SkResult * max(1, len(views)))()
+        self._err(self.L.lb200_sortkeys_create_keys_views(self.h, culling.h, ptr(views), C.c_uint32(len(views)), C.c_int(1 if sort else 0),
+                                                          C.c_int(1 if want_counts else 0), res))
+        return list(res)[:len(views)] if want_counts else None
+
     def setLaunch(self, blocks=0, prefetch_ahead=-1):
         """Launch shape of later createSortKeys calls: blocks 0 = the default (environment switch, else 2 per SM, at most one per 256
         renderables), -1 = all co-resident, n > 0 = min(n, co-resident); prefetch_ahead 0..4 grid strides, -1 = the default."""
@@ -138,6 +148,15 @@ class SortKeys:
         """Host copies of everything the last createSortKeys left in HBM."""
         o = SkOutputs()
         self._err(self.L.lb200_sortkeys_device_outputs(self.h, C.byref(o)))
+        return self._copy(o, res)
+
+    def readView(self, k, res):
+        """Host copies of what the latest createSortKeysViews left in HBM for view k (`res` = its SkResult)."""
+        o = SkOutputs()
+        self._err(self.L.lb200_sortkeys_view_outputs(self.h, C.c_uint32(k), C.byref(o)))
+        return self._copy(o, res)
+
+    def _copy(self, o, res):
         cp = self.ctx.copy_to_host
         g = res.n_groups
         return dict(keys=cp(o.keys, res.n_keys, np.uint64), values=cp(o.values, res.n_keys, np.uint64), group_count=cp(o.group_count, g, np.uint32),
