@@ -476,6 +476,29 @@ LB200_API int lb200_hierarchy_get_locals(lb200_hierarchy* h, lb200_transform* ou
  * (pipeline.cpp instance setup) take these instead of calling getRelativeMatrix per entity. */
 LB200_API int lb200_hierarchy_get_relative_matrices(lb200_hierarchy* h, const double base_pos[3], float* out_matrices);
 LB200_API uint64_t lb200_hierarchy_algorithmic_bytes(const lb200_hierarchy* h);
+/* Which entities a propagate moved: the entities whose `transformed` delegates World::transformEntity (world.cpp:255-282) fires, i.e. every
+ * entity set through setTransform / setLocalTransform and every descendant of one, each once — the set RenderModuleImpl::onModelInstanceMoved
+ * (render_module.cpp:1544-1566) hands to MOVED, m_moved_instances and CullingSystem::set.
+ * Marks: set_subset marks the nodes it lists (both forms); mark_moved marks nodes directly (a node >= n: LB200_ERR_INVALID, nothing marked).
+ * set_locals, set_root_globals, set_globals and compute_locals mark nothing, and plain propagate neither reads nor clears marks.
+ * set_entities: entity id per node (caller's node order, n entries); a negative id keeps the node out of every moved list (no component
+ * listens: onModelInstanceMoved's isAdded early-out, render_module.cpp:1545).  Default: node i = entity i.
+ * set_parents[_device] keeps the marks and entity ids of nodes i < min(old n, n); new nodes start unmarked with entity i. */
+LB200_API int lb200_hierarchy_set_entities(lb200_hierarchy* h, const int32_t* entity_of_node);
+LB200_API int lb200_hierarchy_mark_moved(lb200_hierarchy* h, const uint32_t* nodes, uint32_t count);
+typedef struct {
+	const int32_t* entities;          /* k entity ids, in ascending node index */
+	const lb200_transform* transforms; /* their new world transforms */
+	const double* pos3;               /* their world spheres (3 doubles each) and radii, as refresh_spheres computes them; NULL when no */
+	const float* radius;              /*   bounding radii are held */
+	const uint32_t* count;            /* k, in device memory */
+} lb200_hierarchy_moved;
+/* lb200_hierarchy_propagate (the same globals, byte for byte) + the moved list: every node that is marked or has a marked ancestor in the
+ * current topology and whose entity id is not negative, once, in ascending node index; then every mark is cleared.  bounding_radius (n, or
+ * NULL) is taken as refresh_spheres takes it: uploaded if given, otherwise the radii held are used, otherwise pos3 / radius are NULL.  The
+ * buffers belong to the hierarchy (capacity n) and stay valid until the next propagate_moved, set_parents[_device] or destroy.  With
+ * out_count, k is read back (4 bytes, one synchronisation); without it the call does not wait for the device. */
+LB200_API int lb200_hierarchy_propagate_moved(lb200_hierarchy* h, const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Animation — replaces AnimationModuleImpl::updateAnimable (src/animation/animation_module.cpp:439-472):

@@ -46,9 +46,10 @@ __global__ void __launch_bounds__(HT) aos_to_soa_kernel(const lb200_transform* _
 	out.sx[i] = t.scale[0]; out.sy[i] = t.scale[1]; out.sz[i] = t.scale[2];
 }
 
-// a few transforms (World::setTransform / setLocalTransform for some entities): node ids + values -> their level positions
+// a few transforms (World::setTransform / setLocalTransform for some entities): node ids + values -> their level positions, which are
+// marked as moved for the next propagate_moved
 __global__ void __launch_bounds__(HT) scatter_transforms_kernel(const uint32_t* __restrict__ nodes, const lb200_transform* __restrict__ values, uint32_t count,
-	const uint32_t* __restrict__ pos_of_node, SoaTransforms out)
+	const uint32_t* __restrict__ pos_of_node, SoaTransforms out, uint8_t* __restrict__ mark)
 {
 	const uint32_t k = blockIdx.x * HT + threadIdx.x;
 	if (k >= count) return;
@@ -57,6 +58,15 @@ __global__ void __launch_bounds__(HT) scatter_transforms_kernel(const uint32_t* 
 	out.px[i] = t.pos[0]; out.py[i] = t.pos[1]; out.pz[i] = t.pos[2];
 	out.rot[i] = make_float4(t.rot[0], t.rot[1], t.rot[2], t.rot[3]);
 	out.sx[i] = t.scale[0]; out.sy[i] = t.scale[1]; out.sz[i] = t.scale[2];
+	mark[i] = 1;
+}
+
+// lb200_hierarchy_mark_moved: node ids -> marks at their level positions
+__global__ void __launch_bounds__(HT) mark_nodes_kernel(const uint32_t* __restrict__ nodes, uint32_t count, const uint32_t* __restrict__ pos_of_node,
+	uint8_t* __restrict__ mark)
+{
+	const uint32_t k = blockIdx.x * HT + threadIdx.x;
+	if (k < count) mark[pos_of_node[nodes[k]]] = 1;
 }
 
 __global__ void __launch_bounds__(HT) soa_to_aos_kernel(SoaTransforms in, const uint32_t* __restrict__ order, uint32_t n, lb200_transform* __restrict__ out) {
@@ -117,21 +127,29 @@ __global__ void __launch_bounds__(HT) compute_locals_kernel(uint32_t begin, uint
 // One depth level: nodes [begin, end) in level order; parents live in earlier levels.
 // Launched with programmatic stream serialization: the block starts while the previous level is still draining, loads its
 // own locals (independent of that level) and only then waits for the parents' globals.
-__global__ void __launch_bounds__(HT) propagate_level_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G) {
+// FLAGS (propagate_moved): also flag[i] = mark[i] | flag[parent], i.e. the node or one of its ancestors was marked (World::transformEntity
+// recurses into every child of a moved entity, world.cpp:272-278).  The <false> instantiation is the plain propagate; mark / flag unused.
+template <bool FLAGS>
+__global__ void __launch_bounds__(HT) propagate_level_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G,
+	const uint8_t* __restrict__ mark, uint8_t* __restrict__ flag)
+{
 	const uint32_t i = begin + blockIdx.x * HT + threadIdx.x;
 	const bool active = i < end;
 	int p = 0;
 	D3 lpos = d3(0, 0, 0);
 	float4 lr = make_float4(0, 0, 0, 1);
 	V3 lscale = v3(1, 1, 1);
+	uint8_t m = 0;
 	if (active) {
 		p = parent[i];
 		lpos = d3(L.px[i], L.py[i], L.pz[i]);
 		lr = L.rot[i];
 		lscale = v3(L.sx[i], L.sy[i], L.sz[i]);
+		if (FLAGS) m = mark[i];
 	}
 	cudaGridDependencySynchronize();
 	if (!active) return;
+	if (FLAGS) flag[i] = m | flag[p];
 	const D3 ppos = d3(G.px[p], G.py[p], G.pz[p]);
 	const float4 pr = G.rot[p];
 	const Q4 prot = q4(pr.x, pr.y, pr.z, pr.w);
@@ -152,27 +170,113 @@ constexpr int SMALL_THREADS = 1024;
 constexpr int MAX_SMALL_LEVELS = 30;
 struct SmallLevels { uint32_t start[MAX_SMALL_LEVELS + 1]; uint32_t n; };
 
-__global__ void __launch_bounds__(SMALL_THREADS) propagate_small_levels_kernel(const __grid_constant__ SmallLevels S, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G) {
+template <bool FLAGS>
+__global__ void __launch_bounds__(SMALL_THREADS) propagate_small_levels_kernel(const __grid_constant__ SmallLevels S, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G,
+	const uint8_t* __restrict__ mark, uint8_t* __restrict__ flag)
+{
 	for (uint32_t l = 0; l < S.n; ++l) {
-		for (uint32_t i = S.start[l] + threadIdx.x; i < S.start[l + 1]; i += SMALL_THREADS) compose_node(i, parent, L, G);
+		for (uint32_t i = S.start[l] + threadIdx.x; i < S.start[l + 1]; i += SMALL_THREADS) {
+			compose_node(i, parent, L, G);
+			if (FLAGS) flag[i] = mark[i] | flag[parent[i]];
+		}
 		__syncthreads();
 	}
 }
 
-// render_module.cpp:1544-1554: world bounding sphere of a moved model instance
+// render_module.cpp:1544-1554: radius of the world bounding sphere of a moved model instance (level position i); its centre is the global position
+__device__ __forceinline__ float sphere_radius(const SoaTransforms& G, uint32_t i, float bounding_radius) {
+	const float sx = G.sx[i], sy = G.sy[i], sz = G.sz[i];
+	const float bc = sy > sz ? sy : sz; // maximum(a, b, c) = a > max(b, c) ? a : max(b, c), math.h:468-475
+	const float m = sx > bc ? sx : bc;
+	return LB_FMUL(bounding_radius, m);
+}
+
 __global__ void __launch_bounds__(HT) spheres_kernel(SoaTransforms G, const uint32_t* __restrict__ order, const float* __restrict__ bounding_radius, uint32_t n,
 	double* __restrict__ out_pos3, float* __restrict__ out_radius)
 {
 	const uint32_t i = blockIdx.x * HT + threadIdx.x;
 	if (i >= n) return;
 	const uint32_t node = order[i];
-	const float sx = G.sx[i], sy = G.sy[i], sz = G.sz[i];
-	const float bc = sy > sz ? sy : sz; // maximum(a, b, c) = a > max(b, c) ? a : max(b, c), math.h:468-475
-	const float m = sx > bc ? sx : bc;
 	out_pos3[3 * (size_t)node + 0] = G.px[i];
 	out_pos3[3 * (size_t)node + 1] = G.py[i];
 	out_pos3[3 * (size_t)node + 2] = G.pz[i];
-	out_radius[node] = LB_FMUL(bounding_radius[node], m);
+	out_radius[node] = sphere_radius(G, i, bounding_radius[node]);
+}
+
+// ---- The moved list of propagate_moved: nodes i (ascending) with flag[pos_of_node[i]] and entity[i] >= 0 ----
+// Two launches: every tile of MT nodes counts its listed nodes; then every tile sums the counts of the tiles before it (as many loads as
+// tiles: a few hundred at 1 M nodes) and writes its nodes in order, round by round of CT nodes with a ballot per warp.  No atomics: the
+// order is the node order whatever the schedule.
+constexpr int CT = 256, CT_WARPS = CT / 32, MT_ROUNDS = 8;
+constexpr uint32_t MT = CT * MT_ROUNDS;
+
+struct MovedOut { int32_t* entity; lb200_transform* transform; double* pos3; float* radius; uint32_t* count; };
+
+__device__ __forceinline__ bool listed(uint32_t i, uint32_t n, const uint32_t* __restrict__ pos_of_node, const uint8_t* __restrict__ flag,
+	const int32_t* __restrict__ entity)
+{
+	return i < n && entity[i] >= 0 && flag[pos_of_node[i]];
+}
+
+// sum of one value per thread over the block, in every thread.  All CT threads; s_warp is free again on return.
+__device__ __forceinline__ uint32_t block_sum(uint32_t v, uint32_t* s_warp) {
+	v = __reduce_add_sync(0xffffffffu, v);
+	if ((threadIdx.x & 31u) == 0) s_warp[threadIdx.x >> 5] = v;
+	__syncthreads();
+	uint32_t t = 0;
+#pragma unroll
+	for (int w = 0; w < CT_WARPS; ++w) t += s_warp[w];
+	__syncthreads();
+	return t;
+}
+
+__global__ void __launch_bounds__(CT) moved_count_kernel(uint32_t n, const uint32_t* __restrict__ pos_of_node, const uint8_t* __restrict__ flag,
+	const int32_t* __restrict__ entity, uint32_t* __restrict__ tile_count)
+{
+	__shared__ uint32_t s_warp[CT_WARPS];
+	uint32_t c = 0;
+#pragma unroll
+	for (int r = 0; r < MT_ROUNDS; ++r) c += listed(blockIdx.x * MT + r * CT + threadIdx.x, n, pos_of_node, flag, entity);
+	c = block_sum(c, s_warp);
+	if (threadIdx.x == 0) tile_count[blockIdx.x] = c;
+}
+
+__global__ void __launch_bounds__(CT) moved_gather_kernel(uint32_t n, const uint32_t* __restrict__ pos_of_node, const uint8_t* __restrict__ flag,
+	const int32_t* __restrict__ entity, const uint32_t* __restrict__ tile_count, SoaTransforms G, const float* __restrict__ bounding_radius, MovedOut out)
+{
+	__shared__ uint32_t s_warp[CT_WARPS];
+	const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+	uint32_t before = 0;
+	for (uint32_t t = threadIdx.x; t < blockIdx.x; t += CT) before += tile_count[t];
+	uint32_t o = block_sum(before, s_warp); // the tile's first output slot
+	for (int r = 0; r < MT_ROUNDS; ++r) {
+		const uint32_t i = blockIdx.x * MT + r * CT + threadIdx.x;
+		const bool f = listed(i, n, pos_of_node, flag, entity);
+		const uint32_t ballot = __ballot_sync(0xffffffffu, f);
+		if (lane == 0) s_warp[warp] = __popc(ballot);
+		__syncthreads();
+		uint32_t at = o + __popc(ballot & ((1u << lane) - 1u)), total = 0;
+#pragma unroll
+		for (int w = 0; w < CT_WARPS; ++w) { const uint32_t c = s_warp[w]; at += (uint32_t)w < warp ? c : 0u; total += c; }
+		__syncthreads();
+		o += total;
+		if (!f) continue;
+		const uint32_t k = pos_of_node[i];
+		out.entity[at] = entity[i];
+		lb200_transform t;
+		t.pos[0] = G.px[k]; t.pos[1] = G.py[k]; t.pos[2] = G.pz[k];
+		const float4 q = G.rot[k];
+		t.rot[0] = q.x; t.rot[1] = q.y; t.rot[2] = q.z; t.rot[3] = q.w;
+		t.scale[0] = G.sx[k]; t.scale[1] = G.sy[k]; t.scale[2] = G.sz[k];
+		out.transform[at] = t;
+		if (bounding_radius) {
+			out.pos3[3 * (size_t)at + 0] = t.pos[0];
+			out.pos3[3 * (size_t)at + 1] = t.pos[1];
+			out.pos3[3 * (size_t)at + 2] = t.pos[2];
+			out.radius[at] = sphere_radius(G, k, bounding_radius[i]);
+		}
+	}
+	if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *out.count = o;
 }
 
 // World::getRelativeMatrix, world.cpp:370-377: rot.toMatrix(), translation = Vec3(pos - base), multiply3x3(scale).
@@ -361,10 +465,11 @@ __device__ __forceinline__ void identity_transform(const SoaTransforms& dst, uin
 	dst.sx[to] = 1.f; dst.sy[to] = 1.f; dst.sz[to] = 1.f;
 }
 
-// The new level order -> pos_of_node, and every node's locals and globals from its old level position to its new one (the identity for
-// nodes >= old_n, which the hierarchy did not hold before).
+// The new level order -> pos_of_node, and every node's locals, globals and moved mark from its old level position to its new one, and its
+// entity id (the identity transforms, no mark and entity i for nodes i >= old_n, which the hierarchy did not hold before).
 __global__ void __launch_bounds__(HT) permute_kernel(const uint32_t* __restrict__ order, uint32_t n, const uint32_t* __restrict__ old_pos_of_node, uint32_t old_n,
-	SoaTransforms old_L, SoaTransforms old_G, uint32_t* __restrict__ pos_of_node, SoaTransforms L, SoaTransforms G)
+	SoaTransforms old_L, SoaTransforms old_G, const uint8_t* __restrict__ old_mark, const int32_t* __restrict__ old_entity,
+	uint32_t* __restrict__ pos_of_node, SoaTransforms L, SoaTransforms G, uint8_t* __restrict__ mark, int32_t* __restrict__ entity)
 {
 	const uint32_t k = blockIdx.x * HT + threadIdx.x;
 	if (k >= n) return;
@@ -374,10 +479,14 @@ __global__ void __launch_bounds__(HT) permute_kernel(const uint32_t* __restrict_
 		const uint32_t o = old_pos_of_node[i];
 		copy_transform(old_L, o, L, k);
 		copy_transform(old_G, o, G, k);
+		mark[k] = old_mark[o];
+		entity[i] = old_entity[i];
 	}
 	else {
 		identity_transform(L, k);
 		identity_transform(G, k);
+		mark[k] = 0;
+		entity[i] = (int32_t)i;
 	}
 }
 
@@ -412,6 +521,13 @@ struct lb200_hierarchy {
 	DeviceArray<uint8_t> d_subset[2]; PinnedArray<uint8_t> h_subset[2]; Event subset_done[2]; uint32_t subset_turn = 0;
 	DeviceArray<int> d_parent;           // level position -> parent's level position
 	SoaArrays L, G;
+	DeviceArray<uint8_t> d_mark;         // level position -> 1: set_subset / mark_moved named the node since the last propagate_moved
+	DeviceArray<int32_t> d_entity;       // caller node index -> entity id of the moved list (-1: never listed)
+	// propagate_moved: the flags (level position -> the node or an ancestor is marked), the per-tile counts and the moved list (capacity n),
+	// allocated together and released when n changes
+	DeviceArray<uint8_t> d_flag; DeviceArray<uint32_t> d_tile_count;
+	DeviceArray<int32_t> d_moved_entity; DeviceArray<lb200_transform> d_moved_transform; DeviceArray<double> d_moved_pos; DeviceArray<float> d_moved_radius;
+	DeviceArray<uint32_t> d_moved_count; PinnedArray<uint32_t> h_moved_count;
 	DeviceArray<lb200_transform> d_stage; // n Transforms (API boundary)
 	DeviceArray<float4> d_matrices;       // n relative matrices, 4 float4 each (lb200_hierarchy_get_relative_matrices)
 	// the inputs and outputs of spheres_kernel, allocated and released together
@@ -420,7 +536,7 @@ struct lb200_hierarchy {
 	DeviceArray<float> d_sphere_radius;
 	uint64_t gather_bytes = 0;
 	// buildTopology builds the next topology into `next` and swaps it with the current one only once it is known to be valid
-	struct Topology { DeviceArray<uint32_t> order, pos_of_node; DeviceArray<int> parent; SoaArrays L, G; } next;
+	struct Topology { DeviceArray<uint32_t> order, pos_of_node; DeviceArray<int> parent; SoaArrays L, G; DeviceArray<uint8_t> mark; DeviceArray<int32_t> entity; } next;
 	// buildTopology's scratch, grown to the largest n built (sizes are the capacities)
 	DeviceArray<int32_t> d_parents_in;                            // lb200_hierarchy_set_parents: the caller's parents, uploaded
 	DeviceArray<uint64_t> d_keys[2], d_nodes[2];                  // the sorted pairs and the sort's alternate buffers
@@ -474,6 +590,8 @@ int buildTopology(lb200_hierarchy* h, const int32_t* dev_parents, uint32_t n, ui
 		LB200_CUDA(ctx, next.parent.alloc(n));
 		rc = next.L.alloc(ctx, n);
 		if (!rc) rc = next.G.alloc(ctx, n);
+		if (!rc && next.mark.alloc(n) != cudaSuccess) rc = LB200_ERR_CUDA;
+		if (!rc && next.entity.alloc(n) != cudaSuccess) rc = LB200_ERR_CUDA;
 		if (rc) { next.order.reset(); return rc; }
 	}
 	DeviceArray<lb200_transform> stage;
@@ -508,7 +626,8 @@ int buildTopology(lb200_hierarchy* h, const int32_t* dev_parents, uint32_t n, ui
 		LB200_CUDA(ctx, cudaStreamSynchronize(s));
 	}
 
-	permute_kernel<<<(n + HT - 1) / HT, HT, 0, s>>>(next.order, n, h->d_pos_of_node, h->n, h->L, h->G, next.pos_of_node, next.L, next.G);
+	permute_kernel<<<(n + HT - 1) / HT, HT, 0, s>>>(next.order, n, h->d_pos_of_node, h->n, h->L, h->G, h->d_mark, h->d_entity,
+		next.pos_of_node, next.L, next.G, next.mark, next.entity);
 	LB200_CHECK_LAUNCH(ctx);
 	// valid: the new topology becomes the current one (the old arrays are kept for the next build: nothing is freed at an unchanged n)
 	std::swap(h->d_order, next.order);
@@ -516,10 +635,14 @@ int buildTopology(lb200_hierarchy* h, const int32_t* dev_parents, uint32_t n, ui
 	std::swap(h->d_parent, next.parent);
 	std::swap(h->L, next.L);
 	std::swap(h->G, next.G);
+	std::swap(h->d_mark, next.mark);
+	std::swap(h->d_entity, next.entity);
 	if (n != h->n) { // everything sized by n follows; the bounding radii go with the spheres, so the next sphere refresh has to pass them
 		h->d_stage = std::move(stage);
 		h->d_matrices.reset();
 		h->d_radius_in.reset(); h->d_sphere_pos.reset(); h->d_sphere_radius.reset();
+		h->d_flag.reset(); h->d_tile_count.reset();
+		h->d_moved_entity.reset(); h->d_moved_transform.reset(); h->d_moved_pos.reset(); h->d_moved_radius.reset();
 	}
 	h->n = n;
 	h->level_start = std::move(level_start);
@@ -533,6 +656,95 @@ int upload(lb200_hierarchy* h, const lb200_transform* src, SoaTransforms dst, ui
 	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_stage, src, sizeof(lb200_transform) * (size_t)h->n, cudaMemcpyHostToDevice, ctx->stream));
 	aos_to_soa_kernel<<<(count_levelorder + HT - 1) / HT, HT, 0, ctx->stream>>>(h->d_stage, h->d_order, count_levelorder, dst);
 	LB200_CHECK_LAUNCH(ctx);
+	return LB200_OK;
+}
+
+// The level launches of lb200_hierarchy_propagate (FLAGS = false) and lb200_hierarchy_propagate_moved (FLAGS = true: the flags of the
+// roots have to be in place before).
+template <bool FLAGS>
+int propagateLevels(lb200_hierarchy* h) {
+	lb200_ctx* ctx = h->ctx;
+	const uint8_t* mark = FLAGS ? (const uint8_t*)h->d_mark : nullptr;
+	uint8_t* flag = FLAGS ? (uint8_t*)h->d_flag : nullptr;
+	const size_t n_levels = h->level_start.size() - 1;
+	size_t l = 1;
+	// levels up to SMALL_LEVEL_NODES nodes run inside one block (no launch per level)
+	const uint32_t SMALL_LEVEL_NODES = 8192;
+	SmallLevels S;
+	S.n = 0;
+	while (l < n_levels && S.n < MAX_SMALL_LEVELS && h->level_start[l + 1] - h->level_start[l] <= SMALL_LEVEL_NODES) {
+		S.start[S.n] = h->level_start[l];
+		S.start[S.n + 1] = h->level_start[l + 1];
+		++S.n;
+		++l;
+	}
+	if (S.n) {
+		propagate_small_levels_kernel<FLAGS><<<1, SMALL_THREADS, 0, ctx->stream>>>(S, h->d_parent, h->L, h->G, mark, flag);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	bool chained = S.n != 0; // the first kernel of a propagate is a plain launch: whatever precedes it has fully completed
+	for (; l < n_levels; ++l) {
+		const uint32_t begin = h->level_start[l], end = h->level_start[l + 1];
+		if (end == begin) continue;
+		cudaLaunchConfig_t cfg = {};
+		cfg.gridDim = dim3((end - begin + HT - 1) / HT);
+		cfg.blockDim = dim3(HT);
+		cfg.stream = ctx->stream;
+		cudaLaunchAttribute attr[1];
+		attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+		attr[0].val.programmaticStreamSerializationAllowed = 1;
+		cfg.attrs = attr;
+		cfg.numAttrs = chained ? 1 : 0;
+		chained = true;
+		LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, propagate_level_kernel<FLAGS>, begin, end, (const int*)h->d_parent, h->L, h->G, mark, flag));
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	return LB200_OK;
+}
+
+// One of set_subset's / mark_moved's two staging pairs (pinned + device), `bytes` large: the upload before last has left it.  The caller
+// records subset_done[*turn] behind its launch.
+int stageSubset(lb200_hierarchy* h, size_t bytes, uint8_t** hs, uint8_t** ds, uint32_t* turn) {
+	lb200_ctx* ctx = h->ctx;
+	if (h->d_subset[1].size() < bytes) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		size_t cap = h->d_subset[1].size() ? h->d_subset[1].size() : 4096;
+		while (cap < bytes) cap *= 2;
+		for (int b = 0; b < 2; ++b) { h->d_subset[b].reset(); h->h_subset[b].reset(); } // before the new ones are allocated
+		DeviceArray<uint8_t> d_new[2]; PinnedArray<uint8_t> h_new[2];
+		for (int b = 0; b < 2; ++b) {
+			LB200_CUDA(ctx, d_new[b].alloc(cap));
+			LB200_CUDA(ctx, h_new[b].alloc(cap));
+			if (!h->subset_done[b]) LB200_CUDA(ctx, cudaEventCreateWithFlags(h->subset_done[b].create(), cudaEventDisableTiming));
+			LB200_CUDA(ctx, cudaEventRecord(h->subset_done[b], ctx->stream));
+		}
+		for (int b = 0; b < 2; ++b) { h->d_subset[b] = std::move(d_new[b]); h->h_subset[b] = std::move(h_new[b]); }
+	}
+	*turn = h->subset_turn++ & 1u;
+	LB200_CUDA(ctx, cudaEventSynchronize(h->subset_done[*turn])); // the upload before last has left this pair of buffers (no wait for the frame in flight)
+	*hs = h->h_subset[*turn];
+	*ds = h->d_subset[*turn];
+	return LB200_OK;
+}
+
+int allocMoved(lb200_hierarchy* h) {
+	if (h->d_flag) return LB200_OK;
+	lb200_ctx* ctx = h->ctx;
+	const size_t n = h->n;
+	if (!h->h_moved_count) {
+		LB200_CUDA(ctx, h->d_moved_count.alloc(1));
+		LB200_CUDA(ctx, h->h_moved_count.alloc(1));
+	}
+	DeviceArray<uint8_t> flag; DeviceArray<uint32_t> tile_count; DeviceArray<int32_t> entity; DeviceArray<lb200_transform> transform;
+	DeviceArray<double> pos; DeviceArray<float> radius;
+	LB200_CUDA(ctx, flag.alloc(n));
+	LB200_CUDA(ctx, tile_count.alloc((n + MT - 1) / MT));
+	LB200_CUDA(ctx, entity.alloc(n));
+	LB200_CUDA(ctx, transform.alloc(n));
+	LB200_CUDA(ctx, pos.alloc(3 * n));
+	LB200_CUDA(ctx, radius.alloc(n));
+	h->d_flag = std::move(flag); h->d_tile_count = std::move(tile_count);
+	h->d_moved_entity = std::move(entity); h->d_moved_transform = std::move(transform); h->d_moved_pos = std::move(pos); h->d_moved_radius = std::move(radius);
 	return LB200_OK;
 }
 
@@ -613,40 +825,67 @@ int lb200_hierarchy_set_root_globals(lb200_hierarchy* h, const lb200_transform* 
 int lb200_hierarchy_propagate(lb200_hierarchy* h) {
 	if (!h) return LB200_ERR_INVALID;
 	lb200_range range("transform hierarchy"); // World::transformEntity, world.cpp:255
+	LB200_CUDA(h->ctx, cudaSetDevice(h->ctx->device));
+	return propagateLevels<false>(h);
+}
+
+int lb200_hierarchy_set_entities(lb200_hierarchy* h, const int32_t* entity_of_node) {
+	if (!h || !entity_of_node) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	const size_t n_levels = h->level_start.size() - 1;
-	size_t l = 1;
-	// levels up to SMALL_LEVEL_NODES nodes run inside one block (no launch per level)
-	const uint32_t SMALL_LEVEL_NODES = 8192;
-	SmallLevels S;
-	S.n = 0;
-	while (l < n_levels && S.n < MAX_SMALL_LEVELS && h->level_start[l + 1] - h->level_start[l] <= SMALL_LEVEL_NODES) {
-		S.start[S.n] = h->level_start[l];
-		S.start[S.n + 1] = h->level_start[l + 1];
-		++S.n;
-		++l;
+	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_entity, entity_of_node, sizeof(int32_t) * (size_t)h->n, cudaMemcpyHostToDevice, ctx->stream));
+	return LB200_OK;
+}
+
+int lb200_hierarchy_mark_moved(lb200_hierarchy* h, const uint32_t* nodes, uint32_t count) {
+	if (!h || (count && !nodes)) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = h->ctx;
+	for (uint32_t k = 0; k < count; ++k) {
+		if (nodes[k] >= h->n) { lb200_set_error(ctx, "mark_moved: node %u out of range (%u nodes)", nodes[k], h->n); return LB200_ERR_INVALID; }
 	}
-	if (S.n) {
-		propagate_small_levels_kernel<<<1, SMALL_THREADS, 0, ctx->stream>>>(S, h->d_parent, h->L, h->G);
-		LB200_CHECK_LAUNCH(ctx);
-	}
-	bool chained = S.n != 0; // the first kernel of a propagate is a plain launch: whatever precedes it has fully completed
-	for (; l < n_levels; ++l) {
-		const uint32_t begin = h->level_start[l], end = h->level_start[l + 1];
-		if (end == begin) continue;
-		cudaLaunchConfig_t cfg = {};
-		cfg.gridDim = dim3((end - begin + HT - 1) / HT);
-		cfg.blockDim = dim3(HT);
-		cfg.stream = ctx->stream;
-		cudaLaunchAttribute attr[1];
-		attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-		attr[0].val.programmaticStreamSerializationAllowed = 1;
-		cfg.attrs = attr;
-		cfg.numAttrs = chained ? 1 : 0;
-		chained = true;
-		LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, propagate_level_kernel, begin, end, (const int*)h->d_parent, h->L, h->G));
-		LB200_CHECK_LAUNCH(ctx);
+	if (!count) return LB200_OK;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	uint8_t *hs, *ds; uint32_t turn;
+	const int rc = stageSubset(h, sizeof(uint32_t) * (size_t)count, &hs, &ds, &turn);
+	if (rc) return rc;
+	memcpy(hs, nodes, sizeof(uint32_t) * (size_t)count);
+	LB200_CUDA(ctx, cudaMemcpyAsync(ds, hs, sizeof(uint32_t) * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
+	mark_nodes_kernel<<<(count + HT - 1) / HT, HT, 0, ctx->stream>>>((const uint32_t*)ds, count, h->d_pos_of_node, h->d_mark);
+	LB200_CUDA(ctx, cudaEventRecord(h->subset_done[turn], ctx->stream));
+	LB200_CHECK_LAUNCH(ctx);
+	return LB200_OK;
+}
+
+int lb200_hierarchy_propagate_moved(lb200_hierarchy* h, const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count) {
+	if (!h || !out) return LB200_ERR_INVALID;
+	lb200_range range("transform hierarchy + moved list"); // World::transformEntity, world.cpp:255-282, with its `transformed` fan-out
+	lb200_ctx* ctx = h->ctx;
+	cudaStream_t s = ctx->stream;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	int rc = allocMoved(h);
+	if (!rc && bounding_radius) rc = allocSpheres(h);
+	if (rc) return rc;
+	if (bounding_radius) LB200_CUDA(ctx, cudaMemcpyAsync(h->d_radius_in, bounding_radius, sizeof(float) * h->n, cudaMemcpyHostToDevice, s));
+	const float* radius = h->d_radius_in; // NULL: no radii held, no spheres
+	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_flag, h->d_mark, h->level_start[1], cudaMemcpyDeviceToDevice, s)); // roots: their own mark
+	rc = propagateLevels<true>(h);
+	if (rc) return rc;
+	const uint32_t tiles = (h->n + MT - 1) / MT;
+	moved_count_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count);
+	LB200_CHECK_LAUNCH(ctx);
+	const MovedOut mo{h->d_moved_entity, h->d_moved_transform, h->d_moved_pos, h->d_moved_radius, h->d_moved_count};
+	moved_gather_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count, h->G, radius, mo);
+	LB200_CHECK_LAUNCH(ctx);
+	LB200_CUDA(ctx, cudaMemsetAsync(h->d_mark, 0, h->n, s));
+	out->entities = h->d_moved_entity;
+	out->transforms = h->d_moved_transform;
+	out->pos3 = radius ? (const double*)h->d_moved_pos : nullptr;
+	out->radius = radius ? (const float*)h->d_moved_radius : nullptr;
+	out->count = h->d_moved_count;
+	if (out_count) {
+		LB200_CUDA(ctx, cudaMemcpyAsync(h->h_moved_count, h->d_moved_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		*out_count = *h->h_moved_count;
 	}
 	return LB200_OK;
 }
@@ -682,30 +921,15 @@ int lb200_hierarchy_set_subset(lb200_hierarchy* h, const uint32_t* nodes, const 
 	if (!count) return LB200_OK;
 	lb200_ctx* ctx = h->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	const size_t bytes = (sizeof(uint32_t) + sizeof(lb200_transform)) * (size_t)count + 16;
-	if (h->d_subset[1].size() < bytes) {
-		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-		size_t cap = h->d_subset[1].size() ? h->d_subset[1].size() : 4096;
-		while (cap < bytes) cap *= 2;
-		for (int b = 0; b < 2; ++b) { h->d_subset[b].reset(); h->h_subset[b].reset(); } // before the new ones are allocated
-		DeviceArray<uint8_t> d_new[2]; PinnedArray<uint8_t> h_new[2];
-		for (int b = 0; b < 2; ++b) {
-			LB200_CUDA(ctx, d_new[b].alloc(cap));
-			LB200_CUDA(ctx, h_new[b].alloc(cap));
-			if (!h->subset_done[b]) LB200_CUDA(ctx, cudaEventCreateWithFlags(h->subset_done[b].create(), cudaEventDisableTiming));
-			LB200_CUDA(ctx, cudaEventRecord(h->subset_done[b], ctx->stream));
-		}
-		for (int b = 0; b < 2; ++b) { h->d_subset[b] = std::move(d_new[b]); h->h_subset[b] = std::move(h_new[b]); }
-	}
-	const uint32_t turn = h->subset_turn++ & 1u;
-	LB200_CUDA(ctx, cudaEventSynchronize(h->subset_done[turn])); // the upload before last has left this pair of buffers (no wait for the frame in flight)
-	uint8_t* hs = h->h_subset[turn];
-	uint8_t* ds = h->d_subset[turn];
 	const size_t tr_off = (sizeof(uint32_t) * (size_t)count + 15) & ~(size_t)15;
+	uint8_t *hs, *ds; uint32_t turn;
+	const int rc = stageSubset(h, tr_off + sizeof(lb200_transform) * (size_t)count, &hs, &ds, &turn);
+	if (rc) return rc;
 	memcpy(hs, nodes, sizeof(uint32_t) * (size_t)count);
 	memcpy(hs + tr_off, values, sizeof(lb200_transform) * (size_t)count);
 	LB200_CUDA(ctx, cudaMemcpyAsync(ds, hs, tr_off + sizeof(lb200_transform) * (size_t)count, cudaMemcpyHostToDevice, ctx->stream));
-	scatter_transforms_kernel<<<(count + HT - 1) / HT, HT, 0, ctx->stream>>>((const uint32_t*)ds, (const lb200_transform*)(ds + tr_off), count, h->d_pos_of_node, globals ? h->G : h->L);
+	scatter_transforms_kernel<<<(count + HT - 1) / HT, HT, 0, ctx->stream>>>((const uint32_t*)ds, (const lb200_transform*)(ds + tr_off), count, h->d_pos_of_node,
+		globals ? h->G : h->L, h->d_mark);
 	LB200_CUDA(ctx, cudaEventRecord(h->subset_done[turn], ctx->stream));
 	LB200_CHECK_LAUNCH(ctx);
 	return LB200_OK;

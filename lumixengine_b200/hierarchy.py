@@ -4,6 +4,7 @@ Transforms cross the boundary as the engine's 56-byte `Transform` (src/core/math
 TRANSFORM_DTYPE = {pos: 3 x f64, rot: 4 x f32 (xyzw), scale: 3 x f32}.
 """
 import ctypes as C
+from typing import NamedTuple, Optional
 
 import numpy as np
 
@@ -13,6 +14,20 @@ from ._lib import check, ptr, vp
 TRANSFORM_DTYPE = np.dtype({"names": ["pos", "rot", "scale"], "formats": [(np.float64, 3), (np.float32, 4), (np.float32, 3)],
                             "offsets": [0, 24, 40], "itemsize": 56})
 assert TRANSFORM_DTYPE.itemsize == 56
+
+
+class _Moved(C.Structure):  # lb200_hierarchy_moved
+    _fields_ = [("entities", C.c_void_p), ("transforms", C.c_void_p), ("pos3", C.c_void_p), ("radius", C.c_void_p), ("count", C.c_void_p)]
+
+
+class MovedList(NamedTuple):
+    """Device pointers of a propagateMoved list (valid until the next propagateMoved, setParents* or close) and its length k."""
+    entities: int
+    transforms: int
+    pos3: Optional[int]
+    radius: Optional[int]
+    count_ptr: int
+    count: Optional[int]
 
 
 class Hierarchy:
@@ -125,6 +140,32 @@ class Hierarchy:
         p, r = C.c_void_p(), C.c_void_p()
         check(self.L.lb200_hierarchy_refresh_spheres(self.h, ptr(b) if b is not None else None, C.byref(p), C.byref(r)), self.ctx.h)
         return p.value, r.value
+
+    def setEntities(self, entity_of_node):
+        """Entity id per node (n entries, caller order) for the moved lists of propagateMoved; -1 = never listed (no component listens).
+        Until the first call node i is entity i."""
+        e = np.ascontiguousarray(entity_of_node, np.int32)
+        assert len(e) == self.n
+        check(self.L.lb200_hierarchy_set_entities(self.h, ptr(e)), self.ctx.h)
+
+    def markMoved(self, nodes):
+        """World::setTransform / setLocalTransform happened to these nodes elsewhere: their subtrees go into the next propagateMoved's list.
+        A node >= n raises and marks nothing."""
+        nd = np.ascontiguousarray(nodes, np.uint32)
+        check(self.L.lb200_hierarchy_mark_moved(self.h, ptr(nd), C.c_uint32(len(nd))), self.ctx.h)
+
+    def propagateMoved(self, bounding_radius=None, read_count=True):
+        """propagate + the entities World::transformEntity's fan-out reaches (every marked node and its descendants, entity >= 0, once, in
+        ascending node index); clears the marks.  Returns a MovedList of device pointers (entities i32[k], transforms TRANSFORM_DTYPE[k],
+        pos f64[k,3] and radius f32[k] or None when no bounding radii are held, count u32 in device memory) and k, or None for k when
+        read_count is False (then nothing waits for the device)."""
+        b = None if bounding_radius is None else np.ascontiguousarray(bounding_radius, np.float32)
+        if b is not None:
+            assert len(b) == self.n
+        out = _Moved()
+        k = C.c_uint32()
+        check(self.L.lb200_hierarchy_propagate_moved(self.h, ptr(b) if b is not None else None, C.byref(out), C.byref(k) if read_count else None), self.ctx.h)
+        return MovedList(out.entities, out.transforms, out.pos3, out.radius, out.count, k.value if read_count else None)
 
     def getRelativeMatrices(self, base_pos):
         """World::getRelativeMatrix(entity, base_pos) (world.cpp:370-377) for every node: float32[n,16], column-major."""
