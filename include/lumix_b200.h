@@ -366,6 +366,45 @@ LB200_API int lb200_sortkeys_move_device(lb200_sortkeys* sk, const int32_t* dev_
  * since the last call; lb200_sortkeys_prev_transforms hands out the per-entity device array of those transforms. */
 LB200_API int lb200_sortkeys_end_frame(lb200_sortkeys* sk);
 LB200_API int lb200_sortkeys_prev_transforms(lb200_sortkeys* sk, const lb200_transform** dev_prev);
+/* m_moved_instances as it stands: *dev_list (device memory, NULL before the first move or spawn) holds *n entity ids, each at most once
+ * (what end_frame will take prev_frame_transform of).  Reads the count back: synchronises the stream. */
+LB200_API int lb200_sortkeys_moved_list(lb200_sortkeys* sk, const uint32_t** dev_list, uint32_t* n);
+/* The entity ids the per-entity arrays hold, [0, max_entities): max_entities of create, or what a spawn call grew it to. */
+LB200_API uint32_t lb200_sortkeys_max_entities(const lb200_sortkeys* sk);
+/* Spawns on the device (the spawn lists of lb200_culling_add_many_device, for the stage behind the cull).
+ * lb200_sortkeys_spawn_instances_device: RenderModuleImpl::createModelInstance + setModel + modelLoaded (render_module.cpp:3284-3292,
+ * :3107-3148, :2911-2951) for n new model instances whose data lies in device memory.  For e = dev_entities[i] the entity's record ends as
+ * the reference leaves ModelInstance and its Pose: transform dev_transforms[i] (what createSortKeys reads of World::getTransforms()),
+ * model dev_model_of[i], lod = the highest l in 3 .. 0 whose lod_to[l] != -1 in that model (4 if none), MOVED off (VALID | ENABLED),
+ * dirty = dev_dirty[i] != 0 (the instance has a material override; dev_dirty NULL = none has), Pose::frame 0xffffffff,
+ * prev_frame_transform = dev_transforms[i] (the moved-list arrays are allocated if they do not exist yet).  An entity already in this
+ * frame's moved list stays in it once: a later move in the same frame does not list it again, and end_frame takes its
+ * prev_frame_transform as for any listed entity.
+ * lb200_sortkeys_spawn_decals_device: createDecal / createCurveDecal + updateDecalInfo: the material sort key and layer createSortKeys
+ * reads for DECAL / CURVE_DECAL renderables (pipeline.cpp:3841-3867).
+ * Both: n = 0 returns LB200_OK and launches nothing, before any other check.  Otherwise LB200_ERR_INVALID for a NULL required pointer,
+ * max_entity above INT32_MAX, an id outside [0, max_entity], an id listed twice or (instances) a model index at or above the current
+ * model table's count; LB200_ERR_STATE (instances) before set_models.  A refused call changes nothing, capacity included.  The ids are
+ * checked on the device, in one pass ahead of the writes, with one read-back and one synchronisation per call (two for a call that
+ * grows).  A spawn of instances counts as set_transforms for create_keys, which reads only the records of culled ids.
+ * Growth: max_entity >= max_entities grows every per-entity array (records, decal arrays, moved list, prev_frame_transform, the pose and
+ * dirty lists of both output sets, scratch) to the next doubling of max_entities that holds max_entity, waiting for the stream first,
+ * once the batch has been checked without refusals.  Everything keeps its contents (ModelInstance::lod, Pose::frame, the moved list,
+ * prev_frame_transform, the latest create_keys / create_keys_views outputs), new ids start as create leaves them, max_keys and
+ * max_instances keep the values create fixed, and set_instances / set_transforms take n up to the new max_entities.  A failed
+ * allocation returns LB200_ERR_CUDA and leaves the object as it was.  Device pointers handed out before a call that grows (device_outputs,
+ * view_outputs, prev_transforms, moved_list) are stale after it: ask again.
+ * Despawn needs no call here: an id removed with lb200_culling_remove_many_device is in no visible list, so createSortKeys never reads
+ * its record, and a later spawn of the id rewrites all of it (destroyModelInstance / destroyDecal reach createSortKeys only through the
+ * cull). */
+LB200_API int lb200_sortkeys_spawn_instances_device(lb200_sortkeys* sk, const int32_t* dev_entities, const uint32_t* dev_model_of,
+                                                    const lb200_transform* dev_transforms, const uint8_t* dev_dirty, uint32_t n, uint32_t max_entity);
+LB200_API int lb200_sortkeys_spawn_decals_device(lb200_sortkeys* sk, const int32_t* dev_entities, const uint32_t* dev_sort_key, const uint8_t* dev_layer,
+                                                 uint32_t n, uint32_t max_entity);
+/* mi.dirty = false of PipelineImpl::refreshMaterialOverrides (pipeline.cpp:3685-3721) for n instances whose refresh finished (device ids):
+ * only the dirty bit changes, MOVED and the rest of the record stay.  Ids outside [0, max_entities) are skipped.  n = 0 returns LB200_OK
+ * before any other check; otherwise a NULL dev_entities is LB200_ERR_INVALID.  Asynchronous. */
+LB200_API int lb200_sortkeys_clear_dirty_device(lb200_sortkeys* sk, const int32_t* dev_entities, uint32_t n);
 /* The stable LSD radix sort create_keys and the device re-binning use, on caller device buffers, on the context stream: sorts
  * n = min(*dev_count, cap) (u64 key, u64 value) pairs in place (the count is read on the device, like the two callers do).
  * max_blocks caps the cooperative grid (0 = as many as are co-resident; the grid is also at most ceil(cap / 2048)); force_tiled != 0 takes

@@ -100,7 +100,8 @@ SYMBOLS = [
     "lb200_sortkeys_create", "lb200_sortkeys_destroy", "lb200_sortkeys_set_models", "lb200_sortkeys_set_instances", "lb200_sortkeys_set_transforms",
     "lb200_sortkeys_set_transforms_device", "lb200_sortkeys_create_keys", "lb200_sortkeys_create_keys_views", "lb200_sortkeys_set_launch", "lb200_sortkeys_get_launch", "lb200_sortkeys_device_outputs",
     "lb200_sortkeys_view_outputs",
-    "lb200_sortkeys_move_device", "lb200_sortkeys_end_frame", "lb200_sortkeys_prev_transforms", "lb200_radix_sort_device", "lb200_animation_bone_attachments_device",
+    "lb200_sortkeys_move_device", "lb200_sortkeys_end_frame", "lb200_sortkeys_prev_transforms", "lb200_sortkeys_moved_list", "lb200_sortkeys_max_entities",
+    "lb200_sortkeys_spawn_instances_device", "lb200_sortkeys_spawn_decals_device", "lb200_sortkeys_clear_dirty_device", "lb200_radix_sort_device", "lb200_animation_bone_attachments_device",
     "lb200_hierarchy_create", "lb200_hierarchy_destroy", "lb200_hierarchy_depth",
     "lb200_hierarchy_set_parents", "lb200_hierarchy_set_parents_device", "lb200_hierarchy_get_level_order", "lb200_hierarchy_set_locals", "lb200_hierarchy_set_root_globals", "lb200_hierarchy_set_subset",
     "lb200_hierarchy_propagate", "lb200_hierarchy_get_globals", "lb200_hierarchy_get_spheres", "lb200_hierarchy_refresh_spheres", "lb200_hierarchy_get_relative_matrices", "lb200_hierarchy_set_globals", "lb200_hierarchy_compute_locals", "lb200_hierarchy_get_locals", "lb200_hierarchy_algorithmic_bytes",
@@ -160,6 +161,8 @@ def lib():
     L.lb200_culling_exchange_slab_words.restype = C.c_uint32
     L.lb200_culling_page_id.restype = C.c_int32
     L.lb200_culling_last_algorithmic_bytes.restype = C.c_uint64
+    L.lb200_sortkeys_max_entities.restype = C.c_uint32
+    L.lb200_sortkeys_max_entities.argtypes = [vp]
     L.lb200_hierarchy_depth.restype = C.c_uint32
     L.lb200_hierarchy_algorithmic_bytes.restype = C.c_uint64
     L.lb200_animation_algorithmic_bytes.restype = C.c_uint64

@@ -198,13 +198,6 @@ inline int hostView(const lb200_culling* cs) { return cs && cs->device_authorita
 		if (const int rc__ = lbcull::hostView(cs)) return rc__;           \
 	} while (0)
 
-// grow by doubling: `cap`, or `first` while there is none, doubled until it holds `need`
-inline size_t grownCapacity(size_t cap, size_t first, size_t need) {
-	if (!cap) cap = first;
-	while (cap < need) cap *= 2;
-	return cap;
-}
-
 // rank r's exchange buffer of epoch `epoch` as this process addresses it, and in it the slab this rank writes
 inline uint32_t* peerBuffer(const lb200_ctx* ctx, uint32_t epoch, int r) { return ctx->peer.gather[epoch % ctx->peer.n_buffers][r]; }
 inline uint32_t* peerSlab(const lb200_ctx* ctx, uint32_t epoch, int r) { return peerBuffer(ctx, epoch, r) + ctx->peer.slab_words * (size_t)ctx->rank; }

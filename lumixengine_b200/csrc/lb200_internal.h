@@ -149,6 +149,14 @@ struct lb200_ctx {
 
 void lb200_set_error(lb200_ctx* ctx, const char* fmt, ...);
 
+// grow by doubling: `cap`, or `first` while there is none, doubled until it holds `need` (the culling system's buffers, the sort keys'
+// per-entity arrays)
+inline size_t grownCapacity(size_t cap, size_t first, size_t need) {
+	if (!cap) cap = first;
+	while (cap < need) cap *= 2;
+	return cap;
+}
+
 // NVTX range named like the reference's PROFILE_BLOCK / PROFILE_FUNCTION scopes (SURVEY.md §5: culling_system.cpp:330 "culling",
 // animation_module.cpp:743 "update animables"), so that a timeline of the engine with this library reads like the reference's own.
 struct lb200_range {

@@ -412,6 +412,11 @@ __global__ void __launch_bounds__(SK_THREADS, 4) create_keys_kernel(const __grid
 }
 
 // ---- per-entity records: packing what the caller hands over as arrays, unpacking the state the pass keeps ----
+// Bit 7 of the record's flag byte, internal: the entity is in this frame's moved list.  ent_move_kernel sets it with MOVED, end_frame
+// clears both, a spawn clears MOVED (createModelInstance) and leaves it: move -> spawn -> move lists the entity once.  createSortKeys
+// reads MOVED and DIRTY only.
+constexpr uint32_t FLAG_MOVED = (uint32_t)LB200_SK_MOVED << 24, FLAG_DIRTY = (uint32_t)LB200_SK_DIRTY << 24, FLAG_LISTED = 0x80u << 24;
+
 __global__ void __launch_bounds__(256) ent_init_kernel(SkEntity* ent, uint32_t n) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
@@ -437,7 +442,7 @@ __global__ void __launch_bounds__(256) ent_pack_fields_kernel(SkEntity* ent, uin
 	if (model_of || flags) {
 		uint32_t mf = r.model_flags;
 		if (model_of) mf = (mf & ~CODE_MODEL_MASK) | (model_of[i] & CODE_MODEL_MASK);
-		if (flags) mf = (mf & CODE_MODEL_MASK) | ((uint32_t)flags[i] << 24);
+		if (flags) mf = (mf & CODE_MODEL_MASK) | (((uint32_t)flags[i] << 24) & ~FLAG_LISTED); // the whole flag byte, "listed" included: off
 		r.model_flags = mf;
 	}
 	if (lod) r.lod = lod[i];
@@ -467,8 +472,8 @@ __global__ void __launch_bounds__(256) ent_move_kernel(SkEntity* ent, uint32_t m
 	r.pos[0] = t.pos[0]; r.pos[1] = t.pos[1]; r.pos[2] = t.pos[2];
 	r.rot[0] = t.rot[0]; r.rot[1] = t.rot[1]; r.rot[2] = t.rot[2]; r.rot[3] = t.rot[3];
 	r.scale[0] = t.scale[0]; r.scale[1] = t.scale[1]; r.scale[2] = t.scale[2];
-	const uint32_t before = atomicOr(&r.model_flags, (uint32_t)LB200_SK_MOVED << 24);
-	if (!(before & ((uint32_t)LB200_SK_MOVED << 24))) moved_list[atomicAdd(moved_count, 1u)] = e; // m_moved_instances.push(entity), once
+	const uint32_t before = atomicOr(&r.model_flags, FLAG_MOVED | FLAG_LISTED);
+	if (!(before & (FLAG_MOVED | FLAG_LISTED))) moved_list[atomicAdd(moved_count, 1u)] = e; // m_moved_instances.push(entity), once
 }
 
 // RenderModuleImpl::endFrame (render_module.cpp:526-534): MOVED off, prev_frame_transform = the transform of this frame
@@ -477,7 +482,7 @@ __global__ void __launch_bounds__(256) ent_end_frame_kernel(SkEntity* ent, const
 	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const uint32_t e = moved_list[i];
 		SkEntity& r = ent[e];
-		r.model_flags &= ~((uint32_t)LB200_SK_MOVED << 24);
+		r.model_flags &= ~(FLAG_MOVED | FLAG_LISTED);
 		lb200_transform t;
 		t.pos[0] = r.pos[0]; t.pos[1] = r.pos[1]; t.pos[2] = r.pos[2];
 		t.rot[0] = r.rot[0]; t.rot[1] = r.rot[1]; t.rot[2] = r.rot[2]; t.rot[3] = r.rot[3];
@@ -486,6 +491,63 @@ __global__ void __launch_bounds__(256) ent_end_frame_kernel(SkEntity* ent, const
 	}
 }
 __global__ void reset_word_kernel(uint32_t* w) { *w = 0; }
+
+// ---- spawns: one thread per batch entry ----
+// The refusal count of a spawn batch: an id outside [0, max_entity], a model index >= n_models (model_of may be null: no model check) or
+// an id listed twice (the second of two entries that stamp the same entity with this batch's sequence number sees it there).
+__global__ void __launch_bounds__(256) spawn_check_kernel(const int32_t* __restrict__ entities, uint32_t n, uint32_t max_entity, const uint32_t* __restrict__ model_of,
+	uint32_t n_models, uint32_t* stamp, uint32_t seq, uint32_t* refused)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const int32_t e = entities[i];
+	bool bad = e < 0 || (uint32_t)e > max_entity || (model_of && model_of[i] >= n_models);
+	if (!bad) bad = atomicExch(&stamp[e], seq) == seq;
+	if (bad) atomicAdd(refused, 1u);
+}
+
+// createModelInstance + setModel + modelLoaded (render_module.cpp:3284-3292, :3107-3148, :2911-2951) of a checked batch: the whole record
+// in two 32-byte sectors of 16-byte stores, and prev_frame_transform.  Nothing when the batch was refused.
+__global__ void __launch_bounds__(256) spawn_instances_kernel(SkEntity* ent, const int32_t* __restrict__ entities, const uint32_t* __restrict__ model_of,
+	const lb200_transform* __restrict__ tr, const uint8_t* __restrict__ dirty, uint32_t n, const lb200_sk_model* __restrict__ models, lb200_transform* __restrict__ prev,
+	const uint32_t* __restrict__ refused)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n || *refused) return;
+	const uint32_t e = (uint32_t)entities[i], m = model_of[i];
+	const lb200_transform t = tr[i];
+	float lod = 4.0f; // ModelInstance::lod (render_module.h:221) unless a LOD 3 .. 0 has meshes (modelLoaded, :2942-2948)
+	for (int l = 3; l >= 0; --l) {
+		if (__ldg(&models[m].lod_to[l]) != -1) { lod = (float)l; break; }
+	}
+	int4* r = reinterpret_cast<int4*>(ent + e);
+	// VALID | ENABLED (:3290): MOVED off; dirty = the instance has a material override (:2950); "listed" stays as it was
+	const uint32_t mf = (m & CODE_MODEL_MASK) | (r[1].z & FLAG_LISTED) | (dirty && dirty[i] ? FLAG_DIRTY : 0u);
+	r[0] = make_int4(__double2loint(t.pos[0]), __double2hiint(t.pos[0]), __double2loint(t.pos[1]), __double2hiint(t.pos[1]));
+	r[1] = make_int4(__double2loint(t.pos[2]), __double2hiint(t.pos[2]), (int)mf, __float_as_int(lod));
+	r[2] = make_int4(__float_as_int(t.rot[0]), __float_as_int(t.rot[1]), __float_as_int(t.rot[2]), __float_as_int(t.rot[3]));
+	r[3] = make_int4(__float_as_int(t.scale[0]), __float_as_int(t.scale[1]), __float_as_int(t.scale[2]), (int)0xffffffffu); // a new Pose: frame "never" (pose.h:29)
+	prev[e] = t; // setModel, :3109
+}
+
+// createDecal / createCurveDecal + updateDecalInfo of a checked batch: what createSortKeys reads of a decal (pipeline.cpp:3841-3867)
+__global__ void __launch_bounds__(256) spawn_decals_kernel(uint32_t* decal_sort_key, uint8_t* decal_layer, const int32_t* __restrict__ entities, const uint32_t* __restrict__ sort_key,
+	const uint8_t* __restrict__ layer, uint32_t n, const uint32_t* __restrict__ refused)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n || *refused) return;
+	const uint32_t e = (uint32_t)entities[i];
+	decal_sort_key[e] = sort_key[i];
+	decal_layer[e] = layer[i];
+}
+
+// mi.dirty = false of refreshMaterialOverrides (pipeline.cpp:3685-3721); ids outside the records are skipped
+__global__ void __launch_bounds__(256) clear_dirty_kernel(SkEntity* ent, uint32_t max_entities, const int32_t* __restrict__ entities, uint32_t n) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const uint32_t e = (uint32_t)entities[i];
+	if (e < max_entities) atomicAnd(&ent[e].model_flags, ~FLAG_DIRTY);
+}
 
 } // namespace
 
@@ -526,7 +588,10 @@ struct lb200_sortkeys {
 	DeviceArray<uint64_t> d_keys_alt, d_values_alt; // the sort's alternate buffers, shared by every view of both sets
 	DeviceArray<uint32_t> d_stash; DeviceArray<float4> d_stash4; // the two passes' hand-over: one word + 3 x float4 per visible renderable
 	DeviceArray<float> d_lod; DeviceArray<uint32_t> d_pose_frame; // unpacked on request (lb200_sortkeys_device_outputs)
-	DeviceArray<uint32_t> d_moved_list, d_moved_count; DeviceArray<lb200_transform> d_prev; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move onwards)
+	DeviceArray<uint32_t> d_moved_list, d_moved_count; DeviceArray<lb200_transform> d_prev; // RenderModule::m_moved_instances, ModelInstance::prev_frame_transform (first move or spawn onwards)
+	// spawns: per entity the sequence number of the last batch that listed it (duplicate check), the refusal count of a batch and its read-back
+	DeviceArray<uint32_t> d_stamp, d_refused; PinnedArray<uint32_t> h_refused;
+	uint32_t spawn_seq = 0;
 	DeviceArray<GridBar> d_bar;
 	RadixSortScratch radix_scratch; // the sort of every view's keys / values, with d_keys_alt / d_values_alt as its alternate buffers
 	uint32_t max_mesh_sort_key = 0; // largest sort key of the mesh table: every view's max_sort_key must reach it
@@ -704,6 +769,130 @@ int unpack_state(lb200_sortkeys* sk, lb200_sk_outputs* out) {
 	LB200_CHECK_LAUNCH(ctx);
 	out->lod = sk->d_lod; out->pose_frame = sk->d_pose_frame;
 	return LB200_OK;
+}
+
+// the moved list and prev_frame_transform, allocated by the first move or spawn (end_frame tests d_moved_list alone: all three or none)
+int ensure_moved(lb200_sortkeys* sk) {
+	lb200_ctx* ctx = sk->ctx;
+	if (sk->d_moved_list && sk->d_moved_count && sk->d_prev) return LB200_OK;
+	DeviceArray<uint32_t> moved_list, moved_count; DeviceArray<lb200_transform> prev;
+	LB200_CUDA(ctx, moved_list.alloc(sk->max_entities));
+	LB200_CUDA(ctx, moved_count.alloc(1));
+	LB200_CUDA(ctx, cudaMemsetAsync(moved_count, 0, sizeof(uint32_t), ctx->stream));
+	LB200_CUDA(ctx, prev.alloc(sk->max_entities));
+	LB200_CUDA(ctx, cudaMemsetAsync(prev, 0, sizeof(lb200_transform) * (size_t)sk->max_entities, ctx->stream));
+	sk->d_moved_list = std::move(moved_list); sk->d_moved_count = std::move(moved_count); sk->d_prev = std::move(prev);
+	return LB200_OK;
+}
+
+// `to` holds the first n_old elements of `from` (on the context stream), the rest filled with byte `fill` (fill < 0: left as allocated)
+template <typename T> int grow_copy(lb200_ctx* ctx, const DeviceArray<T>& from, size_t n_old, size_t n_new, int fill, DeviceArray<T>& to) {
+	LB200_CUDA(ctx, to.alloc(n_new));
+	if (n_old) LB200_CUDA(ctx, cudaMemcpyAsync(to, from, sizeof(T) * n_old, cudaMemcpyDeviceToDevice, ctx->stream));
+	if (fill >= 0) LB200_CUDA(ctx, cudaMemsetAsync(to + n_old, fill, sizeof(T) * (n_new - n_old), ctx->stream));
+	return LB200_OK;
+}
+// a set's pose / dirty lists ([n_views][max_entities]) at the row stride `cap`, each view's row copied over
+int grow_lists(lb200_ctx* ctx, const DeviceArray<uint32_t>& from, uint32_t n_views, uint32_t old_cap, uint32_t cap, DeviceArray<uint32_t>& to) {
+	LB200_CUDA(ctx, to.alloc((size_t)n_views * cap));
+	LB200_CUDA(ctx, cudaMemcpy2DAsync(to, sizeof(uint32_t) * cap, from, sizeof(uint32_t) * old_cap, sizeof(uint32_t) * old_cap, n_views, cudaMemcpyDeviceToDevice, ctx->stream));
+	return LB200_OK;
+}
+
+// Every per-entity array grown to `cap` entity ids: allocated and filled first, swapped in once the stream has finished the copies, so
+// that a failure leaves the object as it was.  Records, decal arrays, moved list, prev_frame_transform and the pose / dirty lists of both
+// output sets keep their contents (the new records in ent_init_kernel's state); the stash and the unpacked lod / pose-frame arrays hold
+// nothing across calls and are allocated anew; `stamp` (cap entries, the batch that asked for the growth already checked with it)
+// becomes the stamp array.
+int grow_entities(lb200_sortkeys* sk, size_t cap, DeviceArray<uint32_t>& stamp) {
+	lb200_ctx* ctx = sk->ctx;
+	const size_t old = sk->max_entities;
+	cudaStream_t s = ctx->stream;
+	DeviceArray<SkEntity> ent;
+	LB200_CUDA(ctx, ent.alloc(cap));
+	LB200_CUDA(ctx, cudaMemcpyAsync(ent, sk->d_ent, sizeof(SkEntity) * old, cudaMemcpyDeviceToDevice, s));
+	ent_init_kernel<<<(uint32_t)((cap - old + 255) / 256), 256, 0, s>>>(ent + old, (uint32_t)(cap - old));
+	LB200_CHECK_LAUNCH(ctx);
+	DeviceArray<uint32_t> decal_sort_key, stash, moved_list, pose_frame, plain_pose, plain_dirty, views_pose, views_dirty;
+	DeviceArray<uint8_t> decal_layer; DeviceArray<float4> stash4; DeviceArray<lb200_transform> prev; DeviceArray<float> lod;
+	int rc = grow_copy(ctx, sk->d_decal_sort_key, old, cap, 0, decal_sort_key);
+	if (!rc) rc = grow_copy(ctx, sk->d_decal_layer, old, cap, 0, decal_layer);
+	if (rc) return rc;
+	LB200_CUDA(ctx, stash.alloc(cap));
+	LB200_CUDA(ctx, stash4.alloc(3 * cap));
+	if (sk->d_moved_list) {
+		rc = grow_copy(ctx, sk->d_moved_list, old, cap, -1, moved_list);
+		if (!rc) rc = grow_copy(ctx, sk->d_prev, old, cap, 0, prev);
+		if (rc) return rc;
+	}
+	if (sk->d_lod) {
+		LB200_CUDA(ctx, lod.alloc(cap));
+		LB200_CUDA(ctx, pose_frame.alloc(cap));
+	}
+	rc = grow_lists(ctx, sk->plain.pose_list, sk->plain.n_views, (uint32_t)old, (uint32_t)cap, plain_pose);
+	if (!rc) rc = grow_lists(ctx, sk->plain.dirty_list, sk->plain.n_views, (uint32_t)old, (uint32_t)cap, plain_dirty);
+	if (!rc && sk->views.n_views) {
+		rc = grow_lists(ctx, sk->views.pose_list, sk->views.n_views, (uint32_t)old, (uint32_t)cap, views_pose);
+		if (!rc) rc = grow_lists(ctx, sk->views.dirty_list, sk->views.n_views, (uint32_t)old, (uint32_t)cap, views_dirty);
+	}
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaStreamSynchronize(s)); // the copies are done and nothing enqueued still uses the old arrays
+	sk->d_ent = std::move(ent);
+	sk->d_decal_sort_key = std::move(decal_sort_key); sk->d_decal_layer = std::move(decal_layer);
+	sk->d_stash = std::move(stash); sk->d_stash4 = std::move(stash4); sk->d_stamp = std::move(stamp);
+	if (sk->d_moved_list) { sk->d_moved_list = std::move(moved_list); sk->d_prev = std::move(prev); }
+	if (sk->d_lod) { sk->d_lod = std::move(lod); sk->d_pose_frame = std::move(pose_frame); }
+	sk->plain.pose_list = std::move(plain_pose); sk->plain.dirty_list = std::move(plain_dirty);
+	if (sk->views.n_views) { sk->views.pose_list = std::move(views_pose); sk->views.dirty_list = std::move(views_dirty); }
+	sk->max_entities = (uint32_t)cap;
+	return LB200_OK;
+}
+
+// The read-back of a spawn batch's refusal count (synchronises the stream)
+int spawn_result(lb200_sortkeys* sk, const char* what, const char* reasons, uint32_t max_entity) {
+	lb200_ctx* ctx = sk->ctx;
+	LB200_CUDA(ctx, cudaMemcpyAsync(sk->h_refused, sk->d_refused, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	if (const uint32_t bad = *sk->h_refused) {
+		lb200_set_error(ctx, "%s: %u entries refused (%s; ids in [0, %u]): nothing spawned", what, bad, reasons, max_entity);
+		return LB200_ERR_INVALID;
+	}
+	return LB200_OK;
+}
+
+// What both spawn calls do ahead of their writes: the refusal count of the batch (model check if model_of).  A batch whose max_entity
+// needs more entity ids is checked against a stamp array of the grown size first, and only a batch without refusals grows the object
+// (one more synchronisation, on a call that waits for the stream anyway): a refused call changes nothing.
+int spawn_check(lb200_sortkeys* sk, const int32_t* entities, uint32_t n, uint32_t max_entity, const uint32_t* model_of, const char* what, const char* reasons) {
+	lb200_ctx* ctx = sk->ctx;
+	cudaStream_t s = ctx->stream;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	if (!sk->d_refused) {
+		DeviceArray<uint32_t> refused; PinnedArray<uint32_t> h_refused;
+		LB200_CUDA(ctx, refused.alloc(1));
+		LB200_CUDA(ctx, h_refused.alloc(1));
+		sk->d_refused = std::move(refused); sk->h_refused = std::move(h_refused);
+	}
+	const bool grow = (size_t)max_entity >= sk->max_entities;
+	const size_t stamps = grow ? grownCapacity(sk->max_entities, 4096, (size_t)max_entity + 1) : sk->max_entities;
+	DeviceArray<uint32_t> grown_stamp;
+	if (grow || !sk->d_stamp) { // zero: no stamp holds a batch number yet
+		DeviceArray<uint32_t>& st = grow ? grown_stamp : sk->d_stamp;
+		LB200_CUDA(ctx, st.alloc(stamps));
+		LB200_CUDA(ctx, cudaMemsetAsync(st, 0, sizeof(uint32_t) * stamps, s));
+	}
+	uint32_t* stamp = grow ? grown_stamp.get() : sk->d_stamp.get();
+	if (++sk->spawn_seq == 0) { // wrapped: no stamp may hold the new number already
+		LB200_CUDA(ctx, cudaMemsetAsync(stamp, 0, sizeof(uint32_t) * stamps, s));
+		sk->spawn_seq = 1;
+	}
+	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_refused, 0, sizeof(uint32_t), s));
+	spawn_check_kernel<<<(n + 255) / 256, 256, 0, s>>>(entities, n, max_entity, model_of, (uint32_t)sk->d_models.size(), stamp, sk->spawn_seq, sk->d_refused);
+	LB200_CHECK_LAUNCH(ctx);
+	if (!grow) return LB200_OK;
+	const int rc = spawn_result(sk, what, reasons, max_entity);
+	if (rc) return rc;
+	return grow_entities(sk, stamps, grown_stamp);
 }
 
 } // namespace
@@ -954,15 +1143,8 @@ int lb200_sortkeys_move_device(lb200_sortkeys* sk, const int32_t* dev_entities, 
 	if (!n) return LB200_OK;
 	lb200_ctx* ctx = sk->ctx;
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	if (!sk->d_moved_list || !sk->d_moved_count || !sk->d_prev) { // end_frame tests d_moved_list alone: all three or none
-		DeviceArray<uint32_t> moved_list, moved_count; DeviceArray<lb200_transform> prev;
-		LB200_CUDA(ctx, moved_list.alloc(sk->max_entities));
-		LB200_CUDA(ctx, moved_count.alloc(1));
-		LB200_CUDA(ctx, cudaMemsetAsync(moved_count, 0, sizeof(uint32_t), ctx->stream));
-		LB200_CUDA(ctx, prev.alloc(sk->max_entities));
-		LB200_CUDA(ctx, cudaMemsetAsync(prev, 0, sizeof(lb200_transform) * (size_t)sk->max_entities, ctx->stream));
-		sk->d_moved_list = std::move(moved_list); sk->d_moved_count = std::move(moved_count); sk->d_prev = std::move(prev);
-	}
+	const int rc = ensure_moved(sk);
+	if (rc) return rc;
 	ent_move_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, dev_entities, dev_transforms, n, dev_bounding_radius, dev_out_pos3, dev_out_radius, sk->d_moved_list, sk->d_moved_count);
 	LB200_CHECK_LAUNCH(ctx);
 	return LB200_OK;
@@ -981,10 +1163,74 @@ int lb200_sortkeys_end_frame(lb200_sortkeys* sk) {
 	return LB200_OK;
 }
 
-// ModelInstance::prev_frame_transform per entity (device array, zero until an instance has been through move + end_frame), valid while sk lives
+// ModelInstance::prev_frame_transform per entity (device array, zero until an instance has been through move + end_frame or a spawn), valid
+// while sk lives and until a spawn grows it
 int lb200_sortkeys_prev_transforms(lb200_sortkeys* sk, const lb200_transform** dev_prev) {
 	if (!sk || !dev_prev) return LB200_ERR_INVALID;
 	*dev_prev = sk->d_prev;
+	return LB200_OK;
+}
+
+int lb200_sortkeys_moved_list(lb200_sortkeys* sk, const uint32_t** dev_list, uint32_t* n) {
+	if (!sk || !dev_list || !n) return LB200_ERR_INVALID;
+	*dev_list = sk->d_moved_list;
+	*n = 0;
+	if (!sk->d_moved_count) return LB200_OK;
+	lb200_ctx* ctx = sk->ctx;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	LB200_CUDA(ctx, cudaMemcpyAsync(n, sk->d_moved_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	return LB200_OK;
+}
+
+uint32_t lb200_sortkeys_max_entities(const lb200_sortkeys* sk) { return sk ? sk->max_entities : 0u; }
+
+// createModelInstance + setModel + modelLoaded for a batch of new model instances whose data lies in device memory (SURVEY 8f N1)
+int lb200_sortkeys_spawn_instances_device(lb200_sortkeys* sk, const int32_t* dev_entities, const uint32_t* dev_model_of, const lb200_transform* dev_transforms,
+	const uint8_t* dev_dirty, uint32_t n, uint32_t max_entity)
+{
+	if (!sk) return LB200_ERR_INVALID;
+	if (!n) return LB200_OK;
+	if (!dev_entities || !dev_model_of || !dev_transforms) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = sk->ctx;
+	if (!sk->d_models) { lb200_set_error(ctx, "spawn_instances_device needs set_models first"); return LB200_ERR_STATE; }
+	if (max_entity > (uint32_t)INT32_MAX) { lb200_set_error(ctx, "spawn_instances_device: max_entity %u is not an entity id", max_entity); return LB200_ERR_INVALID; }
+	const char* what = "spawn_instances_device";
+	const char* reasons = "an id out of range, an id listed twice or a model index past the model table";
+	int rc = spawn_check(sk, dev_entities, n, max_entity, dev_model_of, what, reasons);
+	if (!rc) rc = ensure_moved(sk);
+	if (rc) return rc;
+	spawn_instances_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, dev_entities, dev_model_of, dev_transforms, dev_dirty, n, sk->d_models, sk->d_prev, sk->d_refused);
+	LB200_CHECK_LAUNCH(ctx);
+	rc = spawn_result(sk, what, reasons, max_entity);
+	if (!rc) sk->have_transforms = true; // create_keys reads only the records of culled ids: a spawned one holds its transform
+	return rc;
+}
+
+// createDecal / createCurveDecal + updateDecalInfo for a batch of new decals whose data lies in device memory
+int lb200_sortkeys_spawn_decals_device(lb200_sortkeys* sk, const int32_t* dev_entities, const uint32_t* dev_sort_key, const uint8_t* dev_layer, uint32_t n, uint32_t max_entity) {
+	if (!sk) return LB200_ERR_INVALID;
+	if (!n) return LB200_OK;
+	if (!dev_entities || !dev_sort_key || !dev_layer) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = sk->ctx;
+	if (max_entity > (uint32_t)INT32_MAX) { lb200_set_error(ctx, "spawn_decals_device: max_entity %u is not an entity id", max_entity); return LB200_ERR_INVALID; }
+	const char* what = "spawn_decals_device";
+	const char* reasons = "an id out of range or an id listed twice";
+	const int rc = spawn_check(sk, dev_entities, n, max_entity, nullptr, what, reasons);
+	if (rc) return rc;
+	spawn_decals_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_decal_sort_key, sk->d_decal_layer, dev_entities, dev_sort_key, dev_layer, n, sk->d_refused);
+	LB200_CHECK_LAUNCH(ctx);
+	return spawn_result(sk, what, reasons, max_entity);
+}
+
+int lb200_sortkeys_clear_dirty_device(lb200_sortkeys* sk, const int32_t* dev_entities, uint32_t n) {
+	if (!sk) return LB200_ERR_INVALID;
+	if (!n) return LB200_OK;
+	if (!dev_entities) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = sk->ctx;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	clear_dirty_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, dev_entities, n);
+	LB200_CHECK_LAUNCH(ctx);
 	return LB200_OK;
 }
 

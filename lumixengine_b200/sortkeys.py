@@ -131,6 +131,33 @@ class SortKeys:
         self._err(self.L.lb200_sortkeys_move_device(self.h, vp(dev_entities), vp(dev_transforms), C.c_uint32(n), vp(dev_bounding_radius) if dev_bounding_radius else None,
                                                     vp(dev_out_pos3) if dev_out_pos3 else None, vp(dev_out_radius) if dev_out_radius else None))
 
+    def spawnInstancesDevice(self, dev_entities, dev_model_of, dev_transforms, n, max_entity, dev_dirty=None):
+        """createModelInstance + setModel + modelLoaded for n new instances whose ids (i32), models (u32), transforms and dirty flags (u8, None =
+        no material override) lie in device memory (pointers as ints).  Grows the per-entity arrays when max_entity >= max_entities.  Raises
+        LumixB200Error (nothing spawned) for an id outside [0, max_entity], a duplicate id or a model index past the table."""
+        try:
+            self._err(self.L.lb200_sortkeys_spawn_instances_device(self.h, vp(dev_entities), vp(dev_model_of), vp(dev_transforms), vp(dev_dirty) if dev_dirty else None,
+                                                                   C.c_uint32(n), C.c_uint32(max_entity)))
+        finally:
+            self.max_entities = int(self.L.lb200_sortkeys_max_entities(self.h))
+
+    def spawnDecalsDevice(self, dev_entities, dev_sort_key, dev_layer, n, max_entity):
+        """createDecal + updateDecalInfo for n new decals: material sort keys (u32) and layers (u8) in device memory; ids as spawnInstancesDevice."""
+        try:
+            self._err(self.L.lb200_sortkeys_spawn_decals_device(self.h, vp(dev_entities), vp(dev_sort_key), vp(dev_layer), C.c_uint32(n), C.c_uint32(max_entity)))
+        finally:
+            self.max_entities = int(self.L.lb200_sortkeys_max_entities(self.h))
+
+    def clearDirtyDevice(self, dev_entities, n):
+        """ModelInstance::dirty = false for n instances (device ids) whose material-override refresh finished; MOVED stays.  Asynchronous."""
+        self._err(self.L.lb200_sortkeys_clear_dirty_device(self.h, vp(dev_entities), C.c_uint32(n)))
+
+    def movedList(self):
+        """Host copy of m_moved_instances as it stands (entity ids, each listed once until endFrame)."""
+        p, n = vp(), C.c_uint32()
+        self._err(self.L.lb200_sortkeys_moved_list(self.h, C.byref(p), C.byref(n)))
+        return self.ctx.copy_to_host(p.value, n.value, np.uint32) if n.value else np.zeros(0, np.uint32)
+
     def endFrame(self):
         """RenderModule::endFrame: MOVED cleared, prev_frame_transform taken for the instances moved since the last call."""
         self._err(self.L.lb200_sortkeys_end_frame(self.h))
