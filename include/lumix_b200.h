@@ -468,6 +468,7 @@ LB200_API uint32_t lb200_culling_exchange_slab_words(lb200_culling* cs);
  * Nodes are given in any order with parent indices (-1 = root); the library orders them by depth once.
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct lb200_hierarchy lb200_hierarchy;
+typedef struct lb200_animation lb200_animation; /* the Animation section below; bone attachments of a hierarchy take its systems */
 
 LB200_API int lb200_hierarchy_create(lb200_ctx* ctx, const int32_t* parents, uint32_t n, lb200_hierarchy** out);
 LB200_API void lb200_hierarchy_destroy(lb200_hierarchy* h);
@@ -538,6 +539,34 @@ typedef struct {
  * buffers belong to the hierarchy (capacity n) and stay valid until the next propagate_moved, set_parents[_device] or destroy.  With
  * out_count, k is read back (4 bytes, one synchronisation); without it the call does not wait for the device. */
 LB200_API int lb200_hierarchy_propagate_moved(lb200_hierarchy* h, const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count);
+/* Bone attachments held by the hierarchy (RenderModuleImpl::m_bone_attachments, render_module.cpp:377-405): attachment k moves node
+ * attached[k] to bone bone[k] of instance instance[k] of animation system slot system[k] (the slot indexes the systems array of
+ * propagate_attached), parent node parent[k], relative7[k] = BoneAttachment::relative_transform (pos xyz, rot xyzw).  n = 0 removes the
+ * table.  Host arrays; copied.  A node >= n, attached[k] == parent[k] or the same attached node twice (an entity has one BoneAttachment):
+ * LB200_ERR_INVALID, the table left as it was.  set_parents[_device] keeps the table (node indices), and the rounds are rebuilt. */
+LB200_API int lb200_hierarchy_set_attachments(lb200_hierarchy* h, uint32_t n, const uint32_t* attached, const uint32_t* parent,
+                                              const uint32_t* system, const uint32_t* instance, const uint32_t* bone, const float* relative7);
+/* propagate_moved + every attachment round, one moved list (the same buffers, lifetime and count read-back as propagate_moved's).  The
+ * frame World::setTransform (world.cpp:255-282, 337-342) and onModelInstanceMoved (render_module.cpp:1544-1566) make of it:
+ *  1. the marked edits propagate; an attached non-root node is recomposed only when it is marked or an ancestor moved in this pass, so the
+ *     global an attachment set stays bit for bit (compose o computeLocal is not exact);
+ *  2. the attachments run in rounds: X after Y when Y's attached node is an ancestor-or-self of X's parent node or a strict ancestor of
+ *     X's attached node.  X is active when posed[system] != 0 (posed == NULL: every system was updated this frame) or its parent node has
+ *     moved so far in this call and has an entity id >= 0.  An active X sets its node's global to parent.compose(bone * relative) with the
+ *     node's current global scale, and its local to computeLocal(world parent, global) (roots: no local); then the round's active nodes'
+ *     subtrees are recomposed.  Inactive attachments leave their node alone.
+ * Every system needs absolute poses (an update with LB200_PALETTE_POSE).  Refused, with globals, locals, marks and the table unchanged:
+ * LB200_ERR_INVALID for a slot >= n_systems, an instance >= its system's instance count or a bone >= its bone count, or a cycle (an
+ * attached node that is an ancestor-or-self of its own parent node, directly or through other attachments); LB200_ERR_STATE for a NULL
+ * system, one of another context or one without absolute poses, and for a table whose nodes set_parents has shrunk away (until the next
+ * set_attachments).  The rounds are built on the device at the first call after set_attachments or set_parents[_device] (a few
+ * read-backs); later calls read nothing back unless out_count is asked for.  A slot is only checked here (set_attachments cannot know
+ * n_systems).  An empty table is propagate_moved: the systems are not looked at. */
+LB200_API int lb200_hierarchy_propagate_attached(lb200_hierarchy* h, lb200_animation* const* systems, const uint8_t* posed, uint32_t n_systems,
+                                                 const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count);
+/* Introspection: rounds[k] = the round of attachment k (1-based, table order) and *n_rounds as the last round build made them
+ * (LB200_ERR_STATE before one); rounds may be NULL. */
+LB200_API int lb200_hierarchy_get_attachment_rounds(lb200_hierarchy* h, uint32_t* rounds, uint32_t* n_rounds);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Animation — replaces AnimationModuleImpl::updateAnimable (src/animation/animation_module.cpp:439-472):
@@ -594,7 +623,6 @@ typedef struct {
 	const int16_t* indices4;
 } lb200_mesh;
 
-typedef struct lb200_animation lb200_animation;
 
 #define LB200_PALETTE_DUAL_QUAT 1u  /* 32 B/bone, pipeline.cpp:2680-2745 */
 #define LB200_PALETTE_MATRIX 2u     /* 64 B/bone, model.cpp:132-137 */
@@ -643,7 +671,9 @@ LB200_API int lb200_animation_blend_pose(lb200_animation* a, const lb200_animati
 LB200_API int lb200_animation_bone_attachments(lb200_animation* a, uint32_t n, const uint32_t* instance, const uint32_t* bone, const float* relative7,
                                                const lb200_transform* parent_transforms, const float* original_scale3, lb200_transform* out_transforms);
 /* The same with every table in device memory and the transforms left there: the device-side chain pose -> attached entity transform ->
- * lb200_sortkeys_move_device -> lb200_culling_set_many_device -> cull (SURVEY 8f N4).  No index validation. */
+ * lb200_sortkeys_move_device -> lb200_culling_set_many_device -> cull (SURVEY 8f N4).  No index validation.  Both forms move the attached
+ * entities alone: for attachments inside a hierarchy (parent globals read from it, the attached subtrees and the locals following,
+ * attachments of attachments) use lb200_hierarchy_set_attachments + lb200_hierarchy_propagate_attached. */
 LB200_API int lb200_animation_bone_attachments_device(lb200_animation* a, uint32_t n, const uint32_t* dev_instance, const uint32_t* dev_bone, const float* dev_relative7,
                                                       const lb200_transform* dev_parent_transforms, const float* dev_original_scale3, lb200_transform* dev_out_transforms);
 LB200_API int lb200_animation_get_times(lb200_animation* a, uint32_t first, uint32_t count, uint32_t* out_ticks);

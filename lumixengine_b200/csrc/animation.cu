@@ -536,12 +536,11 @@ __global__ void __launch_bounds__(256) bone_attachments_kernel(const float* __re
 	rel.rot = q4(r[3], r[4], r[5], r[6]);
 	const Rigid local = rmul(b, rel); // LocalRigidTransform::operator*, math.cpp:859-861
 	const lb200_transform p = parent_tr[i];
-	const Q4 prot = q4(p.rot[0], p.rot[1], p.rot[2], p.rot[3]);
-	// Transform::compose(const LocalRigidTransform&), math.cpp:763: pos + rot.rotate(rhs.pos * scale) in fp32, added to the fp64 position
-	const V3 rotated = rotate(prot, mul(local.pos, v3(p.scale[0], p.scale[1], p.scale[2])));
-	const Q4 rot = qmul(prot, local.rot);
+	D3 pos;
+	Q4 rot;
+	compose_rigid(d3(p.pos[0], p.pos[1], p.pos[2]), q4(p.rot[0], p.rot[1], p.rot[2], p.rot[3]), v3(p.scale[0], p.scale[1], p.scale[2]), local, pos, rot);
 	lb200_transform o;
-	o.pos[0] = LB_DADD(p.pos[0], (double)rotated.x); o.pos[1] = LB_DADD(p.pos[1], (double)rotated.y); o.pos[2] = LB_DADD(p.pos[2], (double)rotated.z);
+	o.pos[0] = pos.x; o.pos[1] = pos.y; o.pos[2] = pos.z;
 	o.rot[0] = rot.x; o.rot[1] = rot.y; o.rot[2] = rot.z; o.rot[3] = rot.w;
 	o.scale[0] = original_scale3[3 * (size_t)i]; o.scale[1] = original_scale3[3 * (size_t)i + 1]; o.scale[2] = original_scale3[3 * (size_t)i + 2];
 	out[i] = o;
@@ -966,6 +965,16 @@ int lb200_animation_bone_attachments_device(lb200_animation* a, uint32_t n, cons
 	LB200_CHECK_LAUNCH(ctx);
 	return LB200_OK;
 }
+
+} // extern "C"
+
+int lb200_animation_internal_poses(const lb200_animation* a, AnimationPoses* out) {
+	if (!a->d_pos || !a->n_instances) return LB200_ERR_STATE;
+	*out = AnimationPoses{a->ctx, a->d_pos, a->d_rot, a->bone_count, a->n_instances};
+	return LB200_OK;
+}
+
+extern "C" {
 
 int lb200_animation_compute_relative(lb200_animation* a) {
 	if (!a) return LB200_ERR_INVALID;

@@ -104,10 +104,7 @@ __device__ __forceinline__ void compose_node(uint32_t i, const int* __restrict__
 
 // The update_local branch of World::transformEntity (world.cpp:267-270) for every non-root node at once:
 // local = Transform::computeLocal(parent global, own global), math.cpp:809-816.  No dependency between nodes: one flat launch.
-__global__ void __launch_bounds__(HT) compute_locals_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms G, SoaTransforms L) {
-	const uint32_t i = begin + blockIdx.x * HT + threadIdx.x;
-	if (i >= end) return;
-	const int p = parent[i];
+__device__ __forceinline__ void compute_local_node(uint32_t i, int p, const SoaTransforms& G, const SoaTransforms& L) {
 	const float4 pr = G.rot[p];
 	const Q4 c = q4(pr.x, pr.y, pr.z, -pr.w); // Quat::conjugated() = (x, y, z, -w), math.cpp:664-667
 	const double psx = (double)G.sx[p], psy = (double)G.sy[p], psz = (double)G.sz[p];
@@ -122,6 +119,12 @@ __global__ void __launch_bounds__(HT) compute_locals_kernel(uint32_t begin, uint
 	L.px[i] = lpos.x; L.py[i] = lpos.y; L.pz[i] = lpos.z;
 	L.rot[i] = make_float4(lrot.x, lrot.y, lrot.z, lrot.w);
 	L.sx[i] = LB_FDIV(G.sx[i], G.sx[p]); L.sy[i] = LB_FDIV(G.sy[i], G.sy[p]); L.sz[i] = LB_FDIV(G.sz[i], G.sz[p]); // Vec3 / Vec3, math.cpp:468
+}
+
+__global__ void __launch_bounds__(HT) compute_locals_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms G, SoaTransforms L) {
+	const uint32_t i = begin + blockIdx.x * HT + threadIdx.x;
+	if (i >= end) return;
+	compute_local_node(i, parent[i], G, L);
 }
 
 // One depth level: nodes [begin, end) in level order; parents live in earlier levels.
@@ -301,6 +304,179 @@ __global__ void __launch_bounds__(HT) relative_matrices_kernel(SoaTransforms G, 
 	dst[1] = make_float4(m[4], m[5], m[6], m[7]);
 	dst[2] = make_float4(m[8], m[9], m[10], m[11]);
 	dst[3] = make_float4(m[12], m[13], m[14], m[15]);
+}
+
+// ---- Bone attachments (lb200_hierarchy_set_attachments / lb200_hierarchy_propagate_attached) ----
+// An attached node's global is set by its attachment, and compose o computeLocal is not exact: recomposing the node from the local computed
+// for it would move it by an ulp.  So the propagate of a frame with attachments skips a pinned (attached) node unless it is marked (its local
+// was written) or its parent's flag is set in this pass (an ancestor moved, World::transformEntity recomposes the node from its local).
+__global__ void __launch_bounds__(HT) propagate_pinned_level_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G,
+	const uint8_t* __restrict__ mark, const uint8_t* __restrict__ pinned, uint8_t* __restrict__ flag)
+{
+	const uint32_t i = begin + blockIdx.x * HT + threadIdx.x;
+	const bool active = i < end;
+	int p = 0;
+	uint8_t m = 0, pin = 0;
+	if (active) { p = parent[i]; m = mark[i]; pin = pinned[i]; }
+	cudaGridDependencySynchronize();
+	if (!active) return;
+	const uint8_t f = m | flag[p];
+	flag[i] = f;
+	if (!pin || f) compose_node(i, parent, L, G);
+}
+
+__global__ void __launch_bounds__(SMALL_THREADS) propagate_pinned_small_levels_kernel(const __grid_constant__ SmallLevels S, const int* __restrict__ parent,
+	SoaTransforms L, SoaTransforms G, const uint8_t* __restrict__ mark, const uint8_t* __restrict__ pinned, uint8_t* __restrict__ flag)
+{
+	for (uint32_t l = 0; l < S.n; ++l) {
+		for (uint32_t i = S.start[l] + threadIdx.x; i < S.start[l + 1]; i += SMALL_THREADS) {
+			const uint8_t f = mark[i] | flag[parent[i]];
+			flag[i] = f;
+			if (!pinned[i] || f) compose_node(i, parent, L, G);
+		}
+		__syncthreads();
+	}
+}
+
+// One attachment of the table in round order: level positions of the attached and the parent node, the parent's node index (its entity
+// id decides whether its move triggers), the system slot, instance, bone and BoneAttachment::relative_transform (pos xyz, rot xyzw).
+struct AttachRecord { uint32_t pos_a, pos_p, node_p, slot, instance, bone; float rel[7]; };
+// One animation system of a propagate_attached call: its absolute poses and whether it was updated this frame
+struct AttachSystem { const float* pos; const float* rot; uint32_t bone_count, posed; };
+
+// The attachments [begin, end) of one round.  Active (the system was posed, or the parent node moved so far in this call and listens):
+// RenderModuleImpl::updateBoneAttachment (render_module.cpp:377-405) into the SoA globals, then World::setTransform's update_local
+// (world.cpp:267-270) for a node with a world parent.  The node is flagged (moved) and stamped: the round's recompose starts below it.
+__global__ void __launch_bounds__(HT) attach_round_kernel(const AttachRecord* __restrict__ rec, uint32_t begin, uint32_t end, const AttachSystem* __restrict__ systems,
+	const int32_t* __restrict__ entity, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G, uint8_t* __restrict__ flag, uint32_t* __restrict__ stamps,
+	uint32_t stamp)
+{
+	const uint32_t k = begin + blockIdx.x * HT + threadIdx.x;
+	if (k >= end) return;
+	const AttachRecord x = rec[k];
+	const AttachSystem sys = systems[x.slot];
+	if (!sys.posed && !(flag[x.pos_p] && entity[x.node_p] >= 0)) return;
+	const size_t bi = (size_t)x.instance * sys.bone_count + x.bone;
+	Rigid b;
+	b.pos = v3(sys.pos[3 * bi], sys.pos[3 * bi + 1], sys.pos[3 * bi + 2]);
+	b.rot = q4(sys.rot[4 * bi], sys.rot[4 * bi + 1], sys.rot[4 * bi + 2], sys.rot[4 * bi + 3]);
+	Rigid rel;
+	rel.pos = v3(x.rel[0], x.rel[1], x.rel[2]);
+	rel.rot = q4(x.rel[3], x.rel[4], x.rel[5], x.rel[6]);
+	const uint32_t p = x.pos_p, a = x.pos_a;
+	const float4 pr = G.rot[p];
+	D3 pos;
+	Q4 rot;
+	compose_rigid(d3(G.px[p], G.py[p], G.pz[p]), q4(pr.x, pr.y, pr.z, pr.w), v3(G.sx[p], G.sy[p], G.sz[p]), rmul(b, rel), pos, rot); // math.cpp:859-861, 763
+	G.px[a] = pos.x; G.py[a] = pos.y; G.pz[a] = pos.z;
+	G.rot[a] = make_float4(rot.x, rot.y, rot.z, rot.w); // the scale stays the node's own (result.scale = original_scale)
+	const int w = parent[a];
+	if (w >= 0) compute_local_node(a, w, G, L);
+	flag[a] = 1;
+	stamps[a] = stamp;
+}
+
+// The recompose behind a round: a node whose parent was written in this round (stamp) is composed from its local, flagged and stamped.
+__global__ void __launch_bounds__(HT) recompose_level_kernel(uint32_t begin, uint32_t end, const int* __restrict__ parent, SoaTransforms L, SoaTransforms G,
+	uint32_t* __restrict__ stamps, uint32_t stamp, uint8_t* __restrict__ flag)
+{
+	const uint32_t i = begin + blockIdx.x * HT + threadIdx.x;
+	const bool active = i < end;
+	const int p = active ? parent[i] : 0;
+	cudaGridDependencySynchronize();
+	if (!active || stamps[p] != stamp) return;
+	compose_node(i, parent, L, G);
+	stamps[i] = stamp;
+	flag[i] = 1;
+}
+
+__global__ void __launch_bounds__(SMALL_THREADS) recompose_small_levels_kernel(const __grid_constant__ SmallLevels S, const int* __restrict__ parent,
+	SoaTransforms L, SoaTransforms G, uint32_t* __restrict__ stamps, uint32_t stamp, uint8_t* __restrict__ flag)
+{
+	for (uint32_t l = 0; l < S.n; ++l) {
+		for (uint32_t i = S.start[l] + threadIdx.x; i < S.start[l + 1]; i += SMALL_THREADS) {
+			if (stamps[parent[i]] != stamp) continue;
+			compose_node(i, parent, L, G);
+			stamps[i] = stamp;
+			flag[i] = 1;
+		}
+		__syncthreads();
+	}
+}
+
+// The round build.  Attachment k -> its attached node's level position: the position's attachment and pin; every round starts at 1.
+__global__ void __launch_bounds__(HT) attach_index_kernel(const uint32_t* __restrict__ attached, uint32_t count, const uint32_t* __restrict__ pos_of_node,
+	int32_t* __restrict__ att_of_pos, uint8_t* __restrict__ pinned, uint32_t* __restrict__ round)
+{
+	const uint32_t k = blockIdx.x * HT + threadIdx.x;
+	if (k >= count) return;
+	const uint32_t a = pos_of_node[attached[k]];
+	att_of_pos[a] = (int32_t)k;
+	pinned[a] = 1;
+	round[k] = 1;
+}
+
+struct RoundState { uint32_t changed, max_round, count, pad; }; // count: the pairs the round sort takes
+
+// max(r, 1 + the round of every attachment whose attached node is q or an ancestor of q)
+__device__ __forceinline__ uint32_t rounds_above(int q, const int* __restrict__ parent, const int32_t* __restrict__ att_of_pos, const uint32_t* round, uint32_t r) {
+	for (; q >= 0; q = parent[q]) {
+		const int32_t y = att_of_pos[q];
+		if (y >= 0) r = max(r, __ldcg(round + y) + 1);
+	}
+	return r;
+}
+
+// One step towards the least fixed point of round[X] = 1 + max(round[Y]) over the attachments Y whose attached node is an ancestor-or-self of
+// X's parent node or a strict ancestor of X's attached node (1 when there is none).  In place: rounds only grow, and every value stays at or
+// below the fixed point.  A cycle has none: its rounds grow past the attachment count.
+__global__ void __launch_bounds__(HT) attach_rounds_kernel(const uint32_t* __restrict__ attached, const uint32_t* __restrict__ parent_node, uint32_t count,
+	const uint32_t* __restrict__ pos_of_node, const int* __restrict__ parent, const int32_t* __restrict__ att_of_pos, uint32_t* round, RoundState* st)
+{
+	const uint32_t k = blockIdx.x * HT + threadIdx.x;
+	if (k >= count) return;
+	uint32_t r = rounds_above((int)pos_of_node[parent_node[k]], parent, att_of_pos, round, 1u);
+	r = rounds_above(parent[pos_of_node[attached[k]]], parent, att_of_pos, round, r);
+	if (r > __ldcg(round + k)) {
+		__stcg(round + k, r);
+		st->changed = 1;
+	}
+	atomicMax(&st->max_round, r);
+}
+
+__global__ void __launch_bounds__(HT) attach_keys_kernel(const uint32_t* __restrict__ round, uint32_t count, uint64_t* __restrict__ keys, uint64_t* __restrict__ values,
+	RoundState* st)
+{
+	const uint32_t k = blockIdx.x * HT + threadIdx.x;
+	if (k == 0) st->count = count;
+	if (k >= count) return;
+	keys[k] = round[k];
+	values[k] = k;
+}
+
+// The table sorted by round -> records in round order; starts[r - 1] = the first record of round r (R + 1 entries, rounds are contiguous:
+// a round r > 1 exists because of one of round r - 1), starts[R + 1 + r - 1] = the smallest attached level position of round r (pre-set
+// to all ones): its level is where the round's recompose starts.
+__global__ void __launch_bounds__(HT) attach_records_kernel(const uint64_t* __restrict__ keys, const uint64_t* __restrict__ values, uint32_t count, uint32_t n_rounds,
+	const uint32_t* __restrict__ table, const float* __restrict__ relative7, const uint32_t* __restrict__ pos_of_node, AttachRecord* __restrict__ rec,
+	uint32_t* __restrict__ starts)
+{
+	const uint32_t j = blockIdx.x * HT + threadIdx.x;
+	if (j >= count) return;
+	const uint32_t k = (uint32_t)values[j], r = (uint32_t)keys[j];
+	AttachRecord x;
+	x.pos_a = pos_of_node[table[k]];
+	x.node_p = table[count + k];
+	x.pos_p = pos_of_node[x.node_p];
+	x.slot = table[2 * (size_t)count + k];
+	x.instance = table[3 * (size_t)count + k];
+	x.bone = table[4 * (size_t)count + k];
+#pragma unroll
+	for (int c = 0; c < 7; ++c) x.rel[c] = relative7[7 * (size_t)k + c];
+	rec[j] = x;
+	if (j == 0 || keys[j - 1] != keys[j]) starts[r - 1] = j;
+	if (j + 1 == count) starts[n_rounds] = count;
+	atomicMin(&starts[n_rounds + r], x.pos_a);
 }
 
 // ---- The level-order builder ----
@@ -544,6 +720,21 @@ struct lb200_hierarchy {
 	DeviceArray<uint8_t> d_build_state; DeviceArray<uint32_t> d_block_sum; PinnedArray<uint8_t> h_readback;
 	RadixSortScratch sort;
 	uint32_t expand_grid = 0; // blocks of expand_levels_kernel that can be co-resident
+	// bone attachments: the table of set_attachments in caller node indices, on the device as [attached][parent][system][instance][bone] (u32,
+	// att_count each) + 7 floats each, and per system slot the table names the largest instance and bone (host checks of every call)
+	// (a vector that scales with the slot value would let one large slot ask for gigabytes)
+	struct SlotUse { uint32_t slot, max_instance, max_bone; };
+	uint32_t att_count = 0, att_max_node = 0;
+	std::vector<SlotUse> att_slots; // the distinct slots the table names, ascending
+	DeviceArray<uint32_t> d_att_table; DeviceArray<float> d_att_relative;
+	// the rounds of the table in the current topology (rebuilt when att_rounds_valid is false): records in round order, round r = records
+	// [att_round_start[r - 1], att_round_start[r]), its recompose starting below level att_round_level[r - 1]; per attachment its round; the
+	// pins (level position -> attached) and the stamps of the recomposes (level position -> the last (call, round) that wrote the node)
+	bool att_rounds_valid = false;
+	std::vector<uint32_t> att_round_start, att_round_level;
+	DeviceArray<AttachRecord> d_att_records; DeviceArray<uint32_t> d_att_round;
+	DeviceArray<uint8_t> d_pinned; DeviceArray<uint32_t> d_stamp; uint32_t stamp = 0;
+	DeviceArray<AttachSystem> d_att_systems; std::vector<AttachSystem> att_systems;
 };
 
 namespace {
@@ -647,6 +838,7 @@ int buildTopology(lb200_hierarchy* h, const int32_t* dev_parents, uint32_t n, ui
 	h->n = n;
 	h->level_start = std::move(level_start);
 	h->gather_bytes = (uint64_t)r.distinct * 52;
+	h->att_rounds_valid = false; // the attachments' level positions, pins and rounds belong to the old level order
 	return LB200_OK;
 }
 
@@ -659,15 +851,13 @@ int upload(lb200_hierarchy* h, const lb200_transform* src, SoaTransforms dst, ui
 	return LB200_OK;
 }
 
-// The level launches of lb200_hierarchy_propagate (FLAGS = false) and lb200_hierarchy_propagate_moved (FLAGS = true: the flags of the
-// roots have to be in place before).
-template <bool FLAGS>
-int propagateLevels(lb200_hierarchy* h) {
+// One pass over levels [first, depth): the narrow levels at its top run in one block (small(S) launches it), then level(cfg, begin, end)
+// launches one kernel per level, chained by programmatic stream serialization.
+template <class Small, class Level>
+int launchLevels(lb200_hierarchy* h, size_t first, Small small, Level level) {
 	lb200_ctx* ctx = h->ctx;
-	const uint8_t* mark = FLAGS ? (const uint8_t*)h->d_mark : nullptr;
-	uint8_t* flag = FLAGS ? (uint8_t*)h->d_flag : nullptr;
 	const size_t n_levels = h->level_start.size() - 1;
-	size_t l = 1;
+	size_t l = first;
 	// levels up to SMALL_LEVEL_NODES nodes run inside one block (no launch per level)
 	const uint32_t SMALL_LEVEL_NODES = 8192;
 	SmallLevels S;
@@ -679,10 +869,10 @@ int propagateLevels(lb200_hierarchy* h) {
 		++l;
 	}
 	if (S.n) {
-		propagate_small_levels_kernel<FLAGS><<<1, SMALL_THREADS, 0, ctx->stream>>>(S, h->d_parent, h->L, h->G, mark, flag);
+		small(S);
 		LB200_CHECK_LAUNCH(ctx);
 	}
-	bool chained = S.n != 0; // the first kernel of a propagate is a plain launch: whatever precedes it has fully completed
+	bool chained = S.n != 0; // the first kernel of a pass is a plain launch: whatever precedes it has fully completed
 	for (; l < n_levels; ++l) {
 		const uint32_t begin = h->level_start[l], end = h->level_start[l + 1];
 		if (end == begin) continue;
@@ -696,10 +886,23 @@ int propagateLevels(lb200_hierarchy* h) {
 		cfg.attrs = attr;
 		cfg.numAttrs = chained ? 1 : 0;
 		chained = true;
-		LB200_CUDA(ctx, cudaLaunchKernelEx(&cfg, propagate_level_kernel<FLAGS>, begin, end, (const int*)h->d_parent, h->L, h->G, mark, flag));
+		LB200_CUDA(ctx, level(cfg, begin, end));
 		LB200_CHECK_LAUNCH(ctx);
 	}
 	return LB200_OK;
+}
+
+// The level launches of lb200_hierarchy_propagate (FLAGS = false) and lb200_hierarchy_propagate_moved (FLAGS = true: the flags of the
+// roots have to be in place before).
+template <bool FLAGS>
+int propagateLevels(lb200_hierarchy* h) {
+	const uint8_t* mark = FLAGS ? (const uint8_t*)h->d_mark : nullptr;
+	uint8_t* flag = FLAGS ? (uint8_t*)h->d_flag : nullptr;
+	return launchLevels(h, 1,
+		[&](const SmallLevels& S) { propagate_small_levels_kernel<FLAGS><<<1, SMALL_THREADS, 0, h->ctx->stream>>>(S, h->d_parent, h->L, h->G, mark, flag); },
+		[&](const cudaLaunchConfig_t& cfg, uint32_t begin, uint32_t end) {
+			return cudaLaunchKernelEx(&cfg, propagate_level_kernel<FLAGS>, begin, end, (const int*)h->d_parent, h->L, h->G, mark, flag);
+		});
 }
 
 // One of set_subset's / mark_moved's two staging pairs (pinned + device), `bytes` large: the upload before last has left it.  The caller
@@ -756,6 +959,137 @@ int allocSpheres(lb200_hierarchy* h) {
 	LB200_CUDA(ctx, sphere_pos.alloc(3 * (size_t)h->n));
 	LB200_CUDA(ctx, sphere_radius.alloc(h->n));
 	h->d_radius_in = std::move(radius_in); h->d_sphere_pos = std::move(sphere_pos); h->d_sphere_radius = std::move(sphere_radius);
+	return LB200_OK;
+}
+
+// propagate_moved's frame around `levels`, the launches that leave the globals and the flags: the radii and the roots' flags before, the
+// moved list and the cleared marks after.
+template <class Levels>
+int movedFrame(lb200_hierarchy* h, const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count, Levels levels) {
+	lb200_ctx* ctx = h->ctx;
+	cudaStream_t s = ctx->stream;
+	int rc = allocMoved(h);
+	if (!rc && bounding_radius) rc = allocSpheres(h);
+	if (rc) return rc;
+	if (bounding_radius) LB200_CUDA(ctx, cudaMemcpyAsync(h->d_radius_in, bounding_radius, sizeof(float) * h->n, cudaMemcpyHostToDevice, s));
+	const float* radius = h->d_radius_in; // NULL: no radii held, no spheres
+	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_flag, h->d_mark, h->level_start[1], cudaMemcpyDeviceToDevice, s)); // roots: their own mark
+	rc = levels();
+	if (rc) return rc;
+	const uint32_t tiles = (h->n + MT - 1) / MT;
+	moved_count_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count);
+	LB200_CHECK_LAUNCH(ctx);
+	const MovedOut mo{h->d_moved_entity, h->d_moved_transform, h->d_moved_pos, h->d_moved_radius, h->d_moved_count};
+	moved_gather_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count, h->G, radius, mo);
+	LB200_CHECK_LAUNCH(ctx);
+	LB200_CUDA(ctx, cudaMemsetAsync(h->d_mark, 0, h->n, s));
+	out->entities = h->d_moved_entity;
+	out->transforms = h->d_moved_transform;
+	out->pos3 = radius ? (const double*)h->d_moved_pos : nullptr;
+	out->radius = radius ? (const float*)h->d_moved_radius : nullptr;
+	out->count = h->d_moved_count;
+	if (out_count) {
+		LB200_CUDA(ctx, cudaMemcpyAsync(h->h_moved_count, h->d_moved_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		*out_count = *h->h_moved_count;
+	}
+	return LB200_OK;
+}
+
+// The rounds of the attachment table in the current level order (see attach_rounds_kernel), on the device: the pins, the fixed point (one
+// 8-byte read-back per step), the stable radix sort of the table by round, the records in round order with the round starts and every
+// round's shallowest attached node (one read-back).  A cycle: LB200_ERR_INVALID, the rounds stay invalid.
+int buildRounds(lb200_hierarchy* h) {
+	lb200_ctx* ctx = h->ctx;
+	cudaStream_t s = ctx->stream;
+	const uint32_t count = h->att_count, n = h->n;
+	h->att_round_start.clear(); // no rounds to report unless this build succeeds
+	if (h->d_pinned.size() != n) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		LB200_CUDA(ctx, h->d_pinned.alloc(n));
+		LB200_CUDA(ctx, h->d_stamp.alloc(n));
+		LB200_CUDA(ctx, cudaMemsetAsync(h->d_stamp, 0, sizeof(uint32_t) * n, s)); // stamps are never 0
+	}
+	if (h->d_att_round.size() < count) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		LB200_CUDA(ctx, h->d_att_round.alloc(count));
+		LB200_CUDA(ctx, h->d_att_records.alloc(count));
+	}
+	DeviceArray<int32_t> att_of_pos; DeviceArray<uint32_t> starts; DeviceArray<RoundState> st;
+	LB200_CUDA(ctx, att_of_pos.alloc(n));
+	LB200_CUDA(ctx, starts.alloc(2 * (size_t)count + 1));
+	LB200_CUDA(ctx, st.alloc(1));
+	LB200_CUDA(ctx, cudaMemsetAsync(att_of_pos, 0xff, sizeof(int32_t) * n, s));
+	LB200_CUDA(ctx, cudaMemsetAsync(h->d_pinned, 0, n, s));
+	const uint32_t* table = h->d_att_table;
+	const uint32_t grid = (count + HT - 1) / HT;
+	attach_index_kernel<<<grid, HT, 0, s>>>(table, count, h->d_pos_of_node, att_of_pos, h->d_pinned, h->d_att_round);
+	LB200_CHECK_LAUNCH(ctx);
+	RoundState r{};
+	do {
+		LB200_CUDA(ctx, cudaMemsetAsync(st, 0, sizeof(RoundState), s));
+		attach_rounds_kernel<<<grid, HT, 0, s>>>(table, table + count, count, h->d_pos_of_node, h->d_parent, att_of_pos, h->d_att_round, st);
+		LB200_CHECK_LAUNCH(ctx);
+		LB200_CUDA(ctx, cudaMemcpyAsync(&r, st, sizeof(RoundState), cudaMemcpyDeviceToHost, s));
+		LB200_CUDA(ctx, cudaStreamSynchronize(s));
+		if (r.max_round > count) { lb200_set_error(ctx, "bone attachments form a cycle (an attached node is an ancestor of its own parent node)"); return LB200_ERR_INVALID; }
+	} while (r.changed);
+	const uint32_t n_rounds = r.max_round;
+	attach_keys_kernel<<<grid, HT, 0, s>>>(h->d_att_round, count, h->d_keys[0], h->d_nodes[0], st);
+	LB200_CHECK_LAUNCH(ctx);
+	int rc = lb200_radix_sort_pairs(ctx, s, h->d_keys[0], h->d_keys[1], h->d_nodes[0], h->d_nodes[1], &st.get()->count, count, h->sort, 0, false, nullptr);
+	if (rc) return rc;
+	LB200_CUDA(ctx, cudaMemsetAsync(starts.get() + n_rounds + 1, 0xff, sizeof(uint32_t) * n_rounds, s));
+	attach_records_kernel<<<grid, HT, 0, s>>>(h->d_keys[0], h->d_nodes[0], count, n_rounds, table, h->d_att_relative, h->d_pos_of_node, h->d_att_records, starts);
+	LB200_CHECK_LAUNCH(ctx);
+	std::vector<uint32_t> rb(2 * (size_t)n_rounds + 1);
+	LB200_CUDA(ctx, cudaMemcpyAsync(rb.data(), starts, sizeof(uint32_t) * rb.size(), cudaMemcpyDeviceToHost, s));
+	LB200_CUDA(ctx, cudaStreamSynchronize(s));
+	h->att_round_start.assign(rb.begin(), rb.begin() + n_rounds + 1);
+	h->att_round_level.resize(n_rounds);
+	for (uint32_t k = 0; k < n_rounds; ++k) // the level of the round's shallowest attached node: the last level starting at or before it
+		h->att_round_level[k] = (uint32_t)(std::upper_bound(h->level_start.begin(), h->level_start.end(), rb[n_rounds + 1 + k]) - h->level_start.begin()) - 1;
+	h->att_rounds_valid = true;
+	return LB200_OK;
+}
+
+// next stamp of a recompose; stamps restart (all cleared) when the counter wraps
+int nextStamp(lb200_hierarchy* h, uint32_t* stamp) {
+	if (++h->stamp == 0) {
+		LB200_CUDA(h->ctx, cudaMemsetAsync(h->d_stamp, 0, sizeof(uint32_t) * h->n, h->ctx->stream));
+		h->stamp = 1;
+	}
+	*stamp = h->stamp;
+	return LB200_OK;
+}
+
+// propagate_attached's launches between the roots' flags and the moved list: the pinned propagate, then per round the attachments and the
+// recompose of their subtrees
+int attachedLevels(lb200_hierarchy* h) {
+	lb200_ctx* ctx = h->ctx;
+	cudaStream_t s = ctx->stream;
+	int rc = launchLevels(h, 1,
+		[&](const SmallLevels& S) { propagate_pinned_small_levels_kernel<<<1, SMALL_THREADS, 0, s>>>(S, h->d_parent, h->L, h->G, h->d_mark, h->d_pinned, h->d_flag); },
+		[&](const cudaLaunchConfig_t& cfg, uint32_t begin, uint32_t end) {
+			return cudaLaunchKernelEx(&cfg, propagate_pinned_level_kernel, begin, end, (const int*)h->d_parent, h->L, h->G, (const uint8_t*)h->d_mark,
+				(const uint8_t*)h->d_pinned, (uint8_t*)h->d_flag);
+		});
+	if (rc) return rc;
+	for (size_t r = 0; r + 1 < h->att_round_start.size(); ++r) {
+		const uint32_t begin = h->att_round_start[r], end = h->att_round_start[r + 1];
+		uint32_t stamp;
+		rc = nextStamp(h, &stamp);
+		if (rc) return rc;
+		attach_round_kernel<<<(end - begin + HT - 1) / HT, HT, 0, s>>>(h->d_att_records, begin, end, h->d_att_systems, h->d_entity, h->d_parent, h->L, h->G,
+			h->d_flag, h->d_stamp, stamp);
+		LB200_CHECK_LAUNCH(ctx);
+		rc = launchLevels(h, h->att_round_level[r] + 1,
+			[&](const SmallLevels& S) { recompose_small_levels_kernel<<<1, SMALL_THREADS, 0, s>>>(S, h->d_parent, h->L, h->G, h->d_stamp, stamp, h->d_flag); },
+			[&](const cudaLaunchConfig_t& cfg, uint32_t b, uint32_t e) {
+				return cudaLaunchKernelEx(&cfg, recompose_level_kernel, b, e, (const int*)h->d_parent, h->L, h->G, (uint32_t*)h->d_stamp, stamp, (uint8_t*)h->d_flag);
+			});
+		if (rc) return rc;
+	}
 	return LB200_OK;
 }
 
@@ -859,33 +1193,123 @@ int lb200_hierarchy_mark_moved(lb200_hierarchy* h, const uint32_t* nodes, uint32
 int lb200_hierarchy_propagate_moved(lb200_hierarchy* h, const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count) {
 	if (!h || !out) return LB200_ERR_INVALID;
 	lb200_range range("transform hierarchy + moved list"); // World::transformEntity, world.cpp:255-282, with its `transformed` fan-out
+	LB200_CUDA(h->ctx, cudaSetDevice(h->ctx->device));
+	return movedFrame(h, bounding_radius, out, out_count, [&] { return propagateLevels<true>(h); });
+}
+
+int lb200_hierarchy_set_attachments(lb200_hierarchy* h, uint32_t n, const uint32_t* attached, const uint32_t* parent, const uint32_t* system,
+	const uint32_t* instance, const uint32_t* bone, const float* relative7)
+{
+	if (!h || (n && (!attached || !parent || !system || !instance || !bone || !relative7))) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = h->ctx;
-	cudaStream_t s = ctx->stream;
+	// everything the call may refuse or fail on comes before the table is replaced
+	std::vector<uint8_t> seen;
+	std::vector<lb200_hierarchy::SlotUse> slots;
+	uint32_t max_node = 0;
+	try {
+		seen.assign(h->n, 0);
+		slots.reserve(n);
+		for (uint32_t k = 0; k < n; ++k) {
+			if (attached[k] >= h->n || parent[k] >= h->n) { lb200_set_error(ctx, "attachment %u: node %u / %u out of range (%u nodes)", k, attached[k], parent[k], h->n); return LB200_ERR_INVALID; }
+			if (attached[k] == parent[k]) { lb200_set_error(ctx, "attachment %u: node %u attached to itself", k, attached[k]); return LB200_ERR_INVALID; }
+			if (seen[attached[k]]++) { lb200_set_error(ctx, "attachment %u: node %u is attached twice", k, attached[k]); return LB200_ERR_INVALID; }
+			max_node = std::max(max_node, std::max(attached[k], parent[k]));
+			slots.push_back({system[k], instance[k], bone[k]});
+		}
+	} catch (const std::bad_alloc&) {
+		lb200_set_error(ctx, "set_attachments: out of host memory");
+		return LB200_ERR_CUDA;
+	}
+	// one entry per slot with its largest instance and bone: sort by slot, then fold each run into its first entry
+	std::sort(slots.begin(), slots.end(), [](const lb200_hierarchy::SlotUse& a, const lb200_hierarchy::SlotUse& b) { return a.slot < b.slot; });
+	size_t distinct = 0;
+	for (size_t k = 0; k < slots.size(); ++k) {
+		if (distinct && slots[distinct - 1].slot == slots[k].slot) {
+			slots[distinct - 1].max_instance = std::max(slots[distinct - 1].max_instance, slots[k].max_instance);
+			slots[distinct - 1].max_bone = std::max(slots[distinct - 1].max_bone, slots[k].max_bone);
+		}
+		else slots[distinct++] = slots[k];
+	}
+	slots.resize(distinct);
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	int rc = allocMoved(h);
-	if (!rc && bounding_radius) rc = allocSpheres(h);
-	if (rc) return rc;
-	if (bounding_radius) LB200_CUDA(ctx, cudaMemcpyAsync(h->d_radius_in, bounding_radius, sizeof(float) * h->n, cudaMemcpyHostToDevice, s));
-	const float* radius = h->d_radius_in; // NULL: no radii held, no spheres
-	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_flag, h->d_mark, h->level_start[1], cudaMemcpyDeviceToDevice, s)); // roots: their own mark
-	rc = propagateLevels<true>(h);
-	if (rc) return rc;
-	const uint32_t tiles = (h->n + MT - 1) / MT;
-	moved_count_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count);
-	LB200_CHECK_LAUNCH(ctx);
-	const MovedOut mo{h->d_moved_entity, h->d_moved_transform, h->d_moved_pos, h->d_moved_radius, h->d_moved_count};
-	moved_gather_kernel<<<tiles, CT, 0, s>>>(h->n, h->d_pos_of_node, h->d_flag, h->d_entity, h->d_tile_count, h->G, radius, mo);
-	LB200_CHECK_LAUNCH(ctx);
-	LB200_CUDA(ctx, cudaMemsetAsync(h->d_mark, 0, h->n, s));
-	out->entities = h->d_moved_entity;
-	out->transforms = h->d_moved_transform;
-	out->pos3 = radius ? (const double*)h->d_moved_pos : nullptr;
-	out->radius = radius ? (const float*)h->d_moved_radius : nullptr;
-	out->count = h->d_moved_count;
-	if (out_count) {
-		LB200_CUDA(ctx, cudaMemcpyAsync(h->h_moved_count, h->d_moved_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-		LB200_CUDA(ctx, cudaStreamSynchronize(s));
-		*out_count = *h->h_moved_count;
+	DeviceArray<uint32_t> table; DeviceArray<float> relative;
+	if (n) {
+		LB200_CUDA(ctx, table.alloc(5 * (size_t)n));
+		LB200_CUDA(ctx, relative.alloc(7 * (size_t)n));
+		const uint32_t* cols[5] = {attached, parent, system, instance, bone};
+		for (int c = 0; c < 5; ++c) LB200_CUDA(ctx, cudaMemcpyAsync(table.get() + (size_t)c * n, cols[c], sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+		LB200_CUDA(ctx, cudaMemcpyAsync(relative, relative7, sizeof(float) * 7 * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
+	}
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the old table may still be read by the stream
+	h->d_att_table = std::move(table);
+	h->d_att_relative = std::move(relative);
+	h->att_count = n;
+	h->att_max_node = max_node;
+	std::swap(h->att_slots, slots);
+	h->att_rounds_valid = false;
+	h->att_round_start.clear();
+	h->att_round_level.clear();
+	return LB200_OK;
+}
+
+int lb200_hierarchy_propagate_attached(lb200_hierarchy* h, lb200_animation* const* systems, const uint8_t* posed, uint32_t n_systems,
+	const float* bounding_radius, lb200_hierarchy_moved* out, uint32_t* out_count)
+{
+	if (!h || !out || (n_systems && !systems)) return LB200_ERR_INVALID;
+	lb200_range range("transform hierarchy + bone attachments + moved list"); // World::setTransform, world.cpp:337-342 + onModelInstanceMoved, render_module.cpp:1544-1566
+	lb200_ctx* ctx = h->ctx;
+	const uint32_t count = h->att_count;
+	if (!count) { // propagate_moved, whatever systems are passed
+		LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+		return movedFrame(h, bounding_radius, out, out_count, [&] { return propagateLevels<true>(h); });
+	}
+	if (h->att_max_node >= h->n) {
+		lb200_set_error(ctx, "propagate_attached: the attachment table names node %u, the hierarchy has %u nodes (set the attachments again)", h->att_max_node, h->n);
+		return LB200_ERR_STATE;
+	}
+	if (h->att_slots.back().slot >= n_systems) {
+		lb200_set_error(ctx, "propagate_attached: the attachment table names system slot %u, %u systems given", h->att_slots.back().slot, n_systems);
+		return LB200_ERR_INVALID;
+	}
+	h->att_systems.resize(n_systems);
+	const lb200_hierarchy::SlotUse* use = h->att_slots.data(); // the next slot the table names (all of them are < n_systems)
+	for (uint32_t k = 0; k < n_systems; ++k) {
+		AnimationPoses p;
+		if (!systems[k]) { lb200_set_error(ctx, "propagate_attached: system %u is NULL", k); return LB200_ERR_STATE; }
+		if (lb200_animation_internal_poses(systems[k], &p)) { lb200_set_error(ctx, "propagate_attached: system %u has no absolute poses (update with LB200_PALETTE_POSE)", k); return LB200_ERR_STATE; }
+		if (p.ctx != ctx) { lb200_set_error(ctx, "propagate_attached: system %u belongs to another context", k); return LB200_ERR_STATE; }
+		if (use != h->att_slots.data() + h->att_slots.size() && use->slot == k) {
+			if (use->max_instance >= p.n_instances || use->max_bone >= p.bone_count) {
+				lb200_set_error(ctx, "propagate_attached: system %u: instance %u / bone %u out of range (%u instances, %u bones)", k, use->max_instance, use->max_bone,
+					p.n_instances, p.bone_count);
+				return LB200_ERR_INVALID;
+			}
+			++use;
+		}
+		h->att_systems[k] = AttachSystem{p.pos, p.rot, p.bone_count, posed ? (uint32_t)(posed[k] != 0) : 1u};
+	}
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	if (!h->att_rounds_valid) {
+		const int rc = buildRounds(h);
+		if (rc) return rc;
+	}
+	if (h->d_att_systems.size() < n_systems) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+		LB200_CUDA(ctx, h->d_att_systems.alloc(n_systems));
+	}
+	LB200_CUDA(ctx, cudaMemcpyAsync(h->d_att_systems, h->att_systems.data(), sizeof(AttachSystem) * n_systems, cudaMemcpyHostToDevice, ctx->stream));
+	return movedFrame(h, bounding_radius, out, out_count, [&] { return attachedLevels(h); });
+}
+
+int lb200_hierarchy_get_attachment_rounds(lb200_hierarchy* h, uint32_t* rounds, uint32_t* n_rounds) {
+	if (!h || !n_rounds) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = h->ctx;
+	if (h->att_round_start.empty()) { lb200_set_error(ctx, "get_attachment_rounds: no rounds built since the last set_attachments"); return LB200_ERR_STATE; }
+	*n_rounds = (uint32_t)h->att_round_start.size() - 1;
+	if (rounds) {
+		LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+		LB200_CUDA(ctx, cudaMemcpyAsync(rounds, h->d_att_round, sizeof(uint32_t) * h->att_count, cudaMemcpyDeviceToHost, ctx->stream));
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	}
 	return LB200_OK;
 }

@@ -177,6 +177,14 @@ struct CullViewsResult {
 int lb200_culling_internal_views(lb200_culling* cs, CullViewsResult* out);
 // culling.cu: 1 + the largest entity id ever added (0 if none): every id a cull of cs can emit is below it
 uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs);
+// animation.cu: the absolute poses of the last update with LB200_PALETTE_POSE (pos: 3 floats, rot: 4 floats per bone, instance-major) for
+// lb200_hierarchy_propagate_attached; LB200_ERR_STATE (out untouched) while the system has none
+struct AnimationPoses {
+	lb200_ctx* ctx;
+	const float *pos, *rot;
+	uint32_t bone_count, n_instances;
+};
+int lb200_animation_internal_poses(const lb200_animation* a, AnimationPoses* out);
 // context.cu: *out = blocks of a cooperative kernel that can be co-resident on the context's device (threads per block, dynamic smem)
 int lb200_coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out);
 // radix_sort.cu: scratch for sorts of up to min(blocks, co-resident blocks) blocks; on failure `out` is left as it was

@@ -128,6 +128,15 @@ LB_HD Rigid rmul(Rigid a, Rigid b) {
 	return r;
 }
 
+// Transform::compose(const LocalRigidTransform&), math.cpp:763: pos + rot.rotate(rhs.pos * scale) in fp32, added to the fp64 position;
+// rotation rot * rhs.rot.  RenderModuleImpl::updateBoneAttachment (render_module.cpp:399-403) composes the parent entity's transform with
+// bone * relative this way and keeps the attached entity's own scale.
+LB_HD void compose_rigid(D3 ppos, Q4 prot, V3 pscale, Rigid local, D3& pos, Q4& rot) {
+	const V3 rotated = rotate(prot, mul(local.pos, pscale));
+	rot = qmul(prot, local.rot);
+	pos = d3(LB_DADD(ppos.x, (double)rotated.x), LB_DADD(ppos.y, (double)rotated.y), LB_DADD(ppos.z, (double)rotated.z));
+}
+
 } // namespace lb
 
 namespace lb {

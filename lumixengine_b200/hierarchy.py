@@ -38,6 +38,7 @@ class Hierarchy:
         self.ctx = ctx
         p = np.ascontiguousarray(parents, np.int32)
         self.n = len(p)
+        self.n_attachments = 0
         h = vp()
         check(self.L.lb200_hierarchy_create(ctx.h, ptr(p), C.c_uint32(self.n), C.byref(h)), ctx.h)
         self.h = h
@@ -166,6 +167,40 @@ class Hierarchy:
         k = C.c_uint32()
         check(self.L.lb200_hierarchy_propagate_moved(self.h, ptr(b) if b is not None else None, C.byref(out), C.byref(k) if read_count else None), self.ctx.h)
         return MovedList(out.entities, out.transforms, out.pos3, out.radius, out.count, k.value if read_count else None)
+
+    def setAttachments(self, attached, parent, system, instance, bone, relative7):
+        """RenderModuleImpl::m_bone_attachments held by the hierarchy: node attached[k] follows bone bone[k] of instance instance[k] of the
+        system in slot system[k] of propagateAttached's list, parent node parent[k], relative7[k] = (pos xyz, rot xyzw).  Empty arrays remove
+        the table.  A node >= n, a node attached to itself or attached twice raises and leaves the table as it was."""
+        cols = [np.ascontiguousarray(a, np.uint32).reshape(-1) for a in (attached, parent, system, instance, bone)]
+        rel = np.ascontiguousarray(relative7, np.float32).reshape(-1, 7)
+        k = len(cols[0])
+        assert all(len(c) == k for c in cols) and len(rel) == k
+        check(self.L.lb200_hierarchy_set_attachments(self.h, C.c_uint32(k), *[ptr(c) for c in cols], ptr(rel)), self.ctx.h)
+        self.n_attachments = k
+
+    def propagateAttached(self, systems, posed=None, bounding_radius=None, read_count=True):
+        """propagateMoved + every round of the attachments (lb200_hierarchy_propagate_attached): one MovedList.  systems: the
+        AnimationSystems the table's slots index; posed[s] true: system s was updated this frame (None: all were)."""
+        handles = (C.c_void_p * max(1, len(systems)))(*[s.h for s in systems])
+        ps = None if posed is None else np.ascontiguousarray(posed, np.uint8)
+        if ps is not None:
+            assert len(ps) == len(systems)
+        b = None if bounding_radius is None else np.ascontiguousarray(bounding_radius, np.float32)
+        if b is not None:
+            assert len(b) == self.n
+        out = _Moved()
+        k = C.c_uint32()
+        check(self.L.lb200_hierarchy_propagate_attached(self.h, handles, ptr(ps), C.c_uint32(len(systems)), ptr(b), C.byref(out),
+                                                        C.byref(k) if read_count else None), self.ctx.h)
+        return MovedList(out.entities, out.transforms, out.pos3, out.radius, out.count, k.value if read_count else None)
+
+    def attachmentRounds(self):
+        """(round of every attachment, 1-based in table order, number of rounds) as the last round build made them."""
+        nr = C.c_uint32()
+        rounds = np.empty(self.n_attachments, np.uint32)
+        check(self.L.lb200_hierarchy_get_attachment_rounds(self.h, ptr(rounds), C.byref(nr)), self.ctx.h)
+        return rounds, int(nr.value)
 
     def getRelativeMatrices(self, base_pos):
         """World::getRelativeMatrix(entity, base_pos) (world.cpp:370-377) for every node: float32[n,16], column-major."""
