@@ -637,6 +637,21 @@ LB200_API int lb200_animation_set_instances(lb200_animation* a, const uint32_t* 
  * palettes in HBM, then step the time as :458-469 do: time_delta > 0: (time + dt) % length; otherwise (rewind, and zero):
  * (time + length - (-dt % length)) % length — a time already below the clip length is left alone by a zero step. */
 LB200_API int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t palette_flags);
+/* lb200_animation_update of every listed system in one device pass: the frame's updateAnimables over all its skeletons (one system per
+ * Model), launched as one grid of up to 64 systems (longer lists run as consecutive launches on the context stream).
+ * - Results: bit for bit what lb200_animation_update(systems[k], time_delta, palette_flags) gives for every k — dual quaternions,
+ *   matrices, absolute poses and advanced times, in each system's own buffers.  Systems are independent, so the order does not
+ *   matter.  A system with 0 instances is skipped, as update skips it.
+ * - Execution: asynchronous on the context stream, no synchronisation and no read-back, inside the NVTX range "update animables".
+ * - n = 0 returns LB200_OK before any other check and launches nothing.
+ * - LB200_ERR_INVALID, with nothing changed and nothing launched: systems == NULL with n > 0, a NULL entry, a system listed twice
+ *   (its time would advance twice), systems of different contexts.
+ * - Palette and pose buffers are allocated per system, as update allocates them, before anything is launched; a failed allocation
+ *   returns LB200_ERR_CUDA with nothing launched.
+ * - Lanes per instance: one G serves the whole call.  If every listed system with instances would choose the same G on its own
+ *   (its set_launch value, then LB200_POSE_LANES, then 8) that G runs, otherwise 8; 4 lanes fall back to 8 when the call's largest
+ *   skeleton has more than 192 bones.  get_launch on each of these systems reports the G that ran.  Results do not depend on G. */
+LB200_API int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, float time_delta, uint32_t palette_flags);
 /* evaluateSkin (model.cpp:103-109) for every vertex of every instance from the matrix palette; output stays in HBM. */
 LB200_API int lb200_animation_skin(lb200_animation* a);
 /* Launch shape of later updates and skins, for tests and tuning.  pose_lanes = lanes per instance of the pose kernel (4, 8, 16 or 32);

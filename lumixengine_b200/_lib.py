@@ -107,7 +107,7 @@ SYMBOLS = [
     "lb200_hierarchy_propagate", "lb200_hierarchy_get_globals", "lb200_hierarchy_get_spheres", "lb200_hierarchy_refresh_spheres", "lb200_hierarchy_get_relative_matrices", "lb200_hierarchy_set_globals", "lb200_hierarchy_compute_locals", "lb200_hierarchy_get_locals", "lb200_hierarchy_algorithmic_bytes",
     "lb200_hierarchy_set_entities", "lb200_hierarchy_mark_moved", "lb200_hierarchy_propagate_moved",
     "lb200_hierarchy_set_attachments", "lb200_hierarchy_propagate_attached", "lb200_hierarchy_get_attachment_rounds",
-    "lb200_animation_create", "lb200_animation_destroy", "lb200_animation_set_instances", "lb200_animation_update", "lb200_animation_skin",
+    "lb200_animation_create", "lb200_animation_destroy", "lb200_animation_set_instances", "lb200_animation_update", "lb200_animation_update_many", "lb200_animation_skin",
     "lb200_animation_set_launch", "lb200_animation_get_launch",
     "lb200_animation_get_dual_quats", "lb200_animation_get_matrices", "lb200_animation_get_pose", "lb200_animation_get_times", "lb200_animation_set_layers", "lb200_animation_bone_attachments", "lb200_animation_compute_relative", "lb200_animation_get_relative_pose", "lb200_animation_blend_pose",
     "lb200_animation_get_skinned", "lb200_animation_skinned_checksum", "lb200_animation_algorithmic_bytes",
@@ -183,6 +183,7 @@ def lib():
     L.lb200_culling_destroy.restype = None
     L.lb200_hierarchy_destroy.restype = None
     L.lb200_animation_destroy.restype = None
+    L.lb200_animation_update_many.argtypes = [C.POINTER(vp), C.c_uint32, C.c_float, C.c_uint32]
     L.lb200_comm_destroy.restype = None
     L.lb200_frustum_perspective.restype = None
     L.lb200_frustum_ortho.restype = None

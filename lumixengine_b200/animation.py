@@ -325,6 +325,16 @@ class AnimationSystem:
     def update(self, time_delta, palette=PALETTE_DUAL_QUAT):
         check(self.L.lb200_animation_update(self.h, C.c_float(time_delta), C.c_uint32(palette)), self.ctx.h)
 
+    @staticmethod
+    def updateMany(systems, time_delta, palette=PALETTE_DUAL_QUAT):
+        """update(time_delta, palette) of every system in one device pass (lb200_animation_update_many): same results, one launch per
+        64 systems.  Entries may be None (refused, as the C call refuses a NULL entry); an empty list launches nothing."""
+        L = _lib.lib()
+        systems = list(systems)
+        arr = (vp * max(len(systems), 1))(*[None if s is None else s.h for s in systems])
+        ctx = next((s.ctx.h for s in systems if s is not None), None)
+        check(L.lb200_animation_update_many(arr, C.c_uint32(len(systems)), C.c_float(time_delta), C.c_uint32(palette)), ctx)
+
     def skin(self):
         check(self.L.lb200_animation_skin(self.h), self.ctx.h)
 

@@ -14,6 +14,7 @@
 #include "lb200_internal.h"
 #include "lb200_math.cuh"
 
+#include <algorithm>
 #include <memory>
 #include <new>
 #include <vector>
@@ -230,11 +231,47 @@ __global__ void __launch_bounds__(256) decode_clips_kernel(const __grid_constant
 
 constexpr int POSE_THREADS = 128;
 
-// G lanes cooperate on one instance (32 / G instances per warp): per-bone phases stride the bones by G, the absolute pass
-// walks depth levels with up to G bones of a level in flight.  G is 8 unless LB200_POSE_LANES or lb200_animation_set_launch asks
-// for another (lb200_animation_update).
-template <int G>
-__global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimParams P) {
+// The fields of AnimParams that differ from system to system, for pose_palette_many_kernel: the pose kernel reads no other table
+// of a system (the bit streams and track descriptors are only read by decode_clips_kernel).
+struct AnimSysParams {
+	const DevClip* clips;
+	const float4* key_pos; const float4* key_rot;
+	const unsigned char* key_flags;
+	const float4* inv_bind_pos; const float4* inv_bind_rot;
+	const short* parents;
+	const unsigned char* level_bones;
+	const uint32_t* level_start;
+	uint32_t bone_count;
+	uint32_t max_level;
+	uint32_t n_instances;
+	uint32_t n_layers;
+	const uint32_t* clip_index;
+	uint32_t* time_ticks;
+	float* out_dq; float* out_mtx; float* out_pos; float* out_rot; // null where the palette flags do not ask for the output
+	const uint32_t* layer_clip;
+	const uint32_t* layer_time;
+	const float* layer_weight;
+};
+static_assert(sizeof(AnimSysParams) == 160, "");
+
+// Systems per pose_palette_many_kernel launch (DESIGN.md §4.3): the parameter block is 16 + 164 x cap bytes, 10.5 KB at 64;
+// longer lists run as consecutive launches on the context stream.
+constexpr uint32_t POSE_MANY_CAP = 64;
+
+struct AnimManyParams {
+	uint32_t dt_ticks;   // as AnimParams: one time step for every system
+	int dt_negative;
+	int advance;
+	uint32_t n_systems;
+	uint32_t block_end[POSE_MANY_CAP]; // inclusive prefix of block counts: system s owns blocks [block_end[s - 1], block_end[s])
+	AnimSysParams sys[POSE_MANY_CAP];
+};
+
+// One instance group of G lanes: sample, blend layers, computeAbsolute, palettes and the time advance of every instance of block
+// `block` of a system.  P holds the system's tables (AnimParams or AnimSysParams), A the time step (dt_ticks, dt_negative, advance).
+// pose_palette_kernel and pose_palette_many_kernel both run it, so the reference arithmetic exists once.
+template <int G, class SP, class AP>
+__device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, const uint32_t block) {
 	extern __shared__ float4 smem4[];
 	constexpr int INST_PER_BLOCK = POSE_THREADS / G;
 	const int lane = threadIdx.x & 31;
@@ -262,7 +299,7 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid
 	// per instance: rot[Bp] (float4) then pos[Bp] (float4, w unused): 128-bit shared accesses, conflict-free per quarter warp
 	float4* s_rot = inst_base + (size_t)grp * Bp * 2;
 	float4* s_pos = s_rot + Bp;
-	const uint32_t inst = blockIdx.x * INST_PER_BLOCK + grp;
+	const uint32_t inst = block * INST_PER_BLOCK + grp;
 	const bool valid = inst < P.n_instances;
 	// the lanes of one group share a mask so that __syncwarp only joins what must be joined
 	const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (lane & ~(G - 1)));
@@ -406,14 +443,37 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid
 		}
 
 		// animation_module.cpp:458-469
-		if (P.advance && sub == 0) {
+		if (A.advance && sub == 0) {
 			const uint32_t l = clip.length_ticks;
 			uint32_t nt;
-			if (!P.dt_negative) nt = (ticks + P.dt_ticks) % l;
-			else nt = (ticks + l - (P.dt_ticks % l)) % l;
+			if (!A.dt_negative) nt = (ticks + A.dt_ticks) % l;
+			else nt = (ticks + l - (A.dt_ticks % l)) % l;
 			P.time_ticks[inst] = nt;
 		}
 	}
+}
+
+// G lanes cooperate on one instance (32 / G instances per warp): per-bone phases stride the bones by G, the absolute pass
+// walks depth levels with up to G bones of a level in flight.  G is 8 unless LB200_POSE_LANES or lb200_animation_set_launch asks
+// for another (lb200_animation_update).
+template <int G>
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimParams P) {
+	pose_palette_body<G>(P, P, blockIdx.x);
+}
+
+// The same for up to POSE_MANY_CAP systems in one grid (lb200_animation_update_many): each block finds its system by a binary search
+// over the prefix of block counts (uniform across the block, once per block) and runs the system's block as pose_palette_kernel would.
+// Dynamic shared memory is sized for the launch's largest skeleton.
+template <int G>
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const __grid_constant__ AnimManyParams M) {
+	uint32_t lo = 0, hi = M.n_systems - 1;
+	while (lo < hi) {
+		const uint32_t mid = (lo + hi) >> 1;
+		if (blockIdx.x < M.block_end[mid]) hi = mid;
+		else lo = mid + 1;
+	}
+	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
+	pose_palette_body<G>(M.sys[lo], M, blockIdx.x - first_block);
 }
 
 // ---- skinning ------------------------------------------------------------------------------------------------
@@ -755,6 +815,10 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 	}
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * 196 * 3 * sizeof(float4))));
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(8 * 196 * 3 * sizeof(float4))));
@@ -783,12 +847,12 @@ int lb200_animation_set_instances(lb200_animation* a, const uint32_t* clip_index
 	return LB200_OK;
 }
 
-int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags) {
-	lb200_range range("update animables"); // animation_module.cpp:743
-	if (!a) return LB200_ERR_INVALID;
+} // extern "C"
+
+namespace {
+// the palette and pose buffers `flags` asks for, allocated once per system at max_instances
+int allocOutputs(lb200_animation* a, uint32_t flags) {
 	lb200_ctx* ctx = a->ctx;
-	if (!a->n_instances) return LB200_OK;
-	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	const size_t nb = (size_t)a->max_instances * a->bone_count;
 	if ((flags & LB200_PALETTE_DUAL_QUAT) && !a->d_dq) LB200_CUDA(ctx, a->d_dq.alloc(8 * nb));
 	if ((flags & LB200_PALETTE_MATRIX) && !a->d_mtx) LB200_CUDA(ctx, a->d_mtx.alloc(16 * nb));
@@ -796,6 +860,42 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 		const int rc = allocPosePair(ctx, a->d_pos, a->d_rot, nb);
 		if (rc) return rc;
 	}
+	return LB200_OK;
+}
+
+// lanes per instance a system asks for: its set_launch value, then LB200_POSE_LANES, then its default (8)
+int requestedLanes(const lb200_animation* a) {
+	static const int g_env = [] { const char* e = getenv("LB200_POSE_LANES"); const int v = e ? atoi(e) : 0; return (v == 4 || v == 8 || v == 16 || v == 32) ? v : 0; }();
+	return a->pose_lanes ? a->pose_lanes : g_env ? g_env : a->lanes_per_instance;
+}
+
+// 4 lanes = 32 instances per block: only while their poses of the largest skeleton fit in shared memory
+int fitLanes(int G, uint32_t bone_count) {
+	if (G == 4) {
+		const uint32_t bp = (bone_count + 3u) & ~3u;
+		if (sizeof(float4) * (2 * (size_t)bp * (POSE_THREADS / 4) + 2 * bp + 128) > 200 * 1024) G = 8;
+	}
+	return G;
+}
+
+// dynamic shared memory of one block of the pose kernel: inverse bind + topology, then per_block poses
+size_t poseSmemBytes(const lb200_animation* a, unsigned per_block) {
+	const uint32_t Bp_ = (a->bone_count + 3u) & ~3u;
+	const uint32_t n_ls_ = (a->max_level + 2u + 3u) & ~3u;
+	const size_t shared_words16 = 2 * Bp_ + (n_ls_ * 4 + Bp_ * 2 + Bp_ + 15) / 16; // in float4 units
+	return sizeof(float4) * (shared_words16 + 2 * (size_t)Bp_ * per_block);
+}
+
+// Time::fromSeconds: u32(time * ONE_SECOND), animation.h:21-24 (:462 uses -time_delta for rewinds)
+// animation_module.cpp:458 `if (time_delta > 0) ... else ...`: zero takes the rewind branch too, which leaves a time below the clip
+// length alone and wraps one at or beyond it (time % length), exactly as the reference does on every update
+template <class T> void setTimeStep(T& A, float time_delta) {
+	A.dt_negative = !(time_delta > 0);
+	A.dt_ticks = (uint32_t)((A.dt_negative ? -time_delta : time_delta) * (float)(1 << 15));
+	A.advance = 1;
+}
+// pose_palette_kernel<G> over one system's instances (the caller checks the launch)
+void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flags) {
 	AnimParams P;
 	P.clips = a->d_clips; P.tracks = a->d_tracks; P.const_t = a->d_const_t; P.const_r_value = a->d_const_r_value; P.const_r_bone = a->d_const_r_bone; P.stream = a->d_stream;
 	P.key_pos = a->d_key_pos; P.key_rot = a->d_key_rot; P.key_flags = a->d_key_flags;
@@ -807,30 +907,106 @@ int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags)
 	P.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
 	P.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
 	P.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
-	// Time::fromSeconds: u32(time * ONE_SECOND), animation.h:21-24 (:462 uses -time_delta for rewinds)
-	// animation_module.cpp:458 `if (time_delta > 0) ... else ...`: zero takes the rewind branch too, which leaves a time below the clip
-	// length alone and wraps one at or beyond it (time % length), exactly as the reference does on every update
-	P.dt_negative = !(time_delta > 0);
-	P.dt_ticks = (uint32_t)((P.dt_negative ? -time_delta : time_delta) * (float)(1 << 15));
-	P.advance = 1;
-	static const int g_env = [] { const char* e = getenv("LB200_POSE_LANES"); const int v = e ? atoi(e) : 0; return (v == 4 || v == 8 || v == 16 || v == 32) ? v : 0; }();
-	int G = a->pose_lanes ? a->pose_lanes : g_env ? g_env : a->lanes_per_instance;
-	if (G == 4) { // 32 instances per block: only while their poses fit in shared memory
-		const uint32_t bp = (a->bone_count + 3u) & ~3u;
-		if (sizeof(float4) * (2 * (size_t)bp * (POSE_THREADS / 4) + 2 * bp + 128) > 200 * 1024) G = 8;
-	}
+	setTimeStep(P, time_delta);
 	const unsigned per_block = POSE_THREADS / G;
 	const unsigned blocks = (a->n_instances + per_block - 1) / per_block;
-	const uint32_t Bp_ = (a->bone_count + 3u) & ~3u;
-	const uint32_t n_ls_ = (a->max_level + 2u + 3u) & ~3u;
-	const size_t shared_words16 = 2 * Bp_ + (n_ls_ * 4 + Bp_ * 2 + Bp_ + 15) / 16; // inverse bind + topology, in float4 units
-	const size_t smem = sizeof(float4) * (shared_words16 + 2 * (size_t)Bp_ * per_block);
-	if (G == 4) pose_palette_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
-	else if (G == 8) pose_palette_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
-	else if (G == 16) pose_palette_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
-	else pose_palette_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(P);
+	const size_t smem = poseSmemBytes(a, per_block);
+	cudaStream_t st = a->ctx->stream;
+	if (G == 4) pose_palette_kernel<4><<<blocks, POSE_THREADS, smem, st>>>(P);
+	else if (G == 8) pose_palette_kernel<8><<<blocks, POSE_THREADS, smem, st>>>(P);
+	else if (G == 16) pose_palette_kernel<16><<<blocks, POSE_THREADS, smem, st>>>(P);
+	else pose_palette_kernel<32><<<blocks, POSE_THREADS, smem, st>>>(P);
+}
+} // namespace
+
+extern "C" {
+
+int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags) {
+	lb200_range range("update animables"); // animation_module.cpp:743
+	if (!a) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = a->ctx;
+	if (!a->n_instances) return LB200_OK;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	const int rc = allocOutputs(a, flags);
+	if (rc) return rc;
+	const int G = fitLanes(requestedLanes(a), a->bone_count);
+	launchPose(a, G, time_delta, flags);
 	LB200_CHECK_LAUNCH(ctx);
 	a->last_pose_lanes = G;
+	return LB200_OK;
+}
+
+int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, float time_delta, uint32_t flags) {
+	lb200_range range("update animables"); // animation_module.cpp:743, one range for the frame's systems
+	if (!n) return LB200_OK;
+	if (!systems) return LB200_ERR_INVALID;
+	for (uint32_t k = 0; k < n; ++k) if (!systems[k]) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = systems[0]->ctx;
+	for (uint32_t k = 1; k < n; ++k) {
+		if (systems[k]->ctx != ctx) { lb200_set_error(ctx, "update_many: system %u belongs to another context", k); return LB200_ERR_INVALID; }
+	}
+	{
+		std::vector<const lb200_animation*> sorted(systems, systems + n);
+		std::sort(sorted.begin(), sorted.end());
+		if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) { lb200_set_error(ctx, "update_many: a system is listed twice"); return LB200_ERR_INVALID; }
+	}
+	// systems without instances are skipped, as lb200_animation_update skips them; the others agree on one G or run 8
+	std::vector<lb200_animation*> run;
+	run.reserve(n);
+	uint32_t max_bones = 0;
+	int G = 0;
+	for (uint32_t k = 0; k < n; ++k) {
+		lb200_animation* a = systems[k];
+		if (!a->n_instances) continue;
+		const int g = requestedLanes(a);
+		G = run.empty() ? g : (G == g ? G : 8);
+		max_bones = std::max(max_bones, a->bone_count);
+		run.push_back(a);
+	}
+	if (run.empty()) return LB200_OK;
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	for (lb200_animation* a : run) { // every buffer before the first launch
+		const int rc = allocOutputs(a, flags);
+		if (rc) return rc;
+	}
+	G = fitLanes(G, max_bones);
+	const unsigned per_block = POSE_THREADS / G;
+	AnimManyParams M;
+	setTimeStep(M, time_delta);
+	for (size_t first = 0; first < run.size(); first += POSE_MANY_CAP) {
+		const uint32_t count = (uint32_t)std::min<size_t>(POSE_MANY_CAP, run.size() - first);
+		if (count == 1) { // a launch of one system is the per-system kernel: no search, parameters read at fixed offsets
+			launchPose(run[first], G, time_delta, flags);
+			LB200_CHECK_LAUNCH(ctx);
+			continue;
+		}
+		M.n_systems = count;
+		uint32_t blocks = 0;
+		size_t smem = 0;
+		for (uint32_t s = 0; s < count; ++s) {
+			const lb200_animation* a = run[first + s];
+			AnimSysParams& S = M.sys[s];
+			S.clips = a->d_clips; S.key_pos = a->d_key_pos; S.key_rot = a->d_key_rot; S.key_flags = a->d_key_flags;
+			S.inv_bind_pos = a->d_bind + 2 * a->bone_count; S.inv_bind_rot = a->d_bind + 3 * a->bone_count;
+			S.parents = a->d_parents; S.level_bones = a->d_level_bones; S.level_start = a->d_level_start;
+			S.bone_count = a->bone_count; S.max_level = a->max_level; S.n_instances = a->n_instances;
+			S.n_layers = a->n_layers; S.layer_clip = a->d_layer_clip; S.layer_time = a->d_layer_time; S.layer_weight = a->d_layer_weight;
+			S.clip_index = a->d_clip_index; S.time_ticks = a->d_time;
+			S.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
+			S.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
+			S.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
+			S.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
+			blocks += (a->n_instances + per_block - 1) / per_block;
+			M.block_end[s] = blocks;
+			smem = std::max(smem, poseSmemBytes(a, per_block));
+		}
+		if (G == 4) pose_palette_many_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		else if (G == 8) pose_palette_many_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		else if (G == 16) pose_palette_many_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		else pose_palette_many_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	for (lb200_animation* a : run) a->last_pose_lanes = G;
 	return LB200_OK;
 }
 
