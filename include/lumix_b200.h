@@ -635,7 +635,8 @@ LB200_API void lb200_animation_destroy(lb200_animation* a);
 LB200_API int lb200_animation_set_instances(lb200_animation* a, const uint32_t* clip_index, const uint32_t* time_ticks, uint32_t n);
 /* One updateAnimables pass (animation_module.cpp:737-749) for all instances: evaluate at the current time, build the requested
  * palettes in HBM, then step the time as :458-469 do: time_delta > 0: (time + dt) % length; otherwise (rewind, and zero):
- * (time + length - (-dt % length)) % length — a time already below the clip length is left alone by a zero step. */
+ * (time + length - (-dt % length)) % length — a time already below the clip length is left alone by a zero step.  A system in
+ * sample-list mode (lb200_animation_set_samples) evaluates its lists and steps no time. */
 LB200_API int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t palette_flags);
 /* lb200_animation_update of every listed system in one device pass: the frame's updateAnimables over all its skeletons (one system per
  * Model), launched as one grid of up to 64 systems (longer lists run as consecutive launches on the context stream).
@@ -671,6 +672,23 @@ LB200_API int lb200_animation_get_pose(lb200_animation* a, uint32_t first, uint3
  * are replaced otherwise; other bones keep their pose.  Layer times are the caller's (not advanced by update).  n_layers = 0 removes
  * the layers; lb200_animation_set_instances also does.  Up to 16 layers. */
 LB200_API int lb200_animation_set_layers(lb200_animation* a, uint32_t n_layers, const uint32_t* clip_index, const uint32_t* time_ticks, const float* weight);
+/* One SAMPLE instruction of an animator's blend stack (controller.cpp:267-293 -> getPose :142-157): clip index, time in ticks, weight,
+ * looped (0 = clamped).  16 bytes, read by the pose kernel as one 128-bit load. */
+typedef struct { uint32_t clip; uint32_t time_ticks; float weight; uint32_t looped; } lb200_sample;
+/* Sample lists: the SAMPLE part of each animator's evalBlendStack, one list per instance (CSR: instance i owns
+ * samples[offsets[i] .. offsets[i+1])).  Instance i starts from the bind pose (Model::getRelativePose, model.cpp:226-237) and applies its
+ * samples in order, each with Animation::getRelativePose's arithmetic for its weight (animation.cpp:117-204, 294-311): bones the clip
+ * tracks are replaced at weight >= 0.9999 and moved by lerp / simd_nlerp below it, other bones keep their pose.  A sample is taken at
+ * time % length when looped and at min(time, length) otherwise, length = Animation::getLength().  Any count per instance, 0 included
+ * (the bind pose).  Then computeAbsolute and the requested palettes / pose, as update always does.
+ * - Mode: set_samples puts the system in sample-list mode with n_instances instances; set_instances puts it back in clip mode.  In
+ *   sample-list mode update and update_many step no time (the animator's controller owns it), and get_times and set_layers return
+ *   LB200_ERR_INVALID.  update_many takes clip-mode and sample-list systems in one call.
+ * - LB200_ERR_INVALID, with nothing changed: n_instances > max_instances, NULL offsets, NULL samples with offsets[n_instances] > 0,
+ *   offsets[0] != 0, decreasing offsets, a clip index out of range.  (Clips of length 0 are refused by create, so a looped sample never
+ *   divides by 0.)
+ * - The lists are copied before the call returns. */
+LB200_API int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples);
 /* Pose::computeRelative (src/renderer/pose.cpp:136-146) of every instance's absolute pose (needs an update with LB200_PALETTE_POSE):
  * the parent-relative poses IK / ragdoll consumers start from (controller.cpp).  Kept in HBM next to the absolute ones. */
 LB200_API int lb200_animation_compute_relative(lb200_animation* a);

@@ -22,6 +22,8 @@ TRACK_DTYPE = np.dtype([("bone_index", np.uint16), ("offset_bits", np.uint16), (
 CONST_T_DTYPE = np.dtype([("bone_index", np.uint16), ("pad", np.uint16), ("value", np.float32, 3)])
 CONST_R_DTYPE = np.dtype([("bone_index", np.uint16), ("pad", np.uint16), ("value", np.float32, 4)])
 assert TRACK_DTYPE.itemsize == 32 and CONST_T_DTYPE.itemsize == 16 and CONST_R_DTYPE.itemsize == 20
+SAMPLE_DTYPE = np.dtype([("clip", np.uint32), ("time_ticks", np.uint32), ("weight", np.float32), ("looped", np.uint32)])  # lb200_sample
+assert SAMPLE_DTYPE.itemsize == 16
 
 
 def _pack_frames(per_track_values, bits_per_track):
@@ -379,6 +381,17 @@ class AnimationSystem:
         w = np.ascontiguousarray(weight, np.float32).reshape(self.n, -1)
         assert ci.shape == tt.shape == w.shape
         check(self.L.lb200_animation_set_layers(self.h, C.c_uint32(ci.shape[1]), ptr(ci), ptr(tt), ptr(w)), self.ctx.h)
+
+    def setSamples(self, offsets, clip, time_ticks, weight, looped):
+        """Sample lists (lb200_animation_set_samples): instance i starts from the bind pose and applies samples offsets[i] .. offsets[i+1]
+        in order, each (clip, time in ticks, weight, looped) as the SAMPLE instruction of an animator's blend stack
+        (controller.cpp:142-157, 267-293).  len(offsets) - 1 instances; the system is in sample-list mode until setInstances."""
+        off = np.ascontiguousarray(offsets, np.uint32)
+        assert off.ndim == 1 and len(off) >= 1
+        s = np.empty(len(np.atleast_1d(clip)), SAMPLE_DTYPE)
+        s["clip"], s["time_ticks"], s["weight"], s["looped"] = clip, time_ticks, weight, looped
+        check(self.L.lb200_animation_set_samples(self.h, C.c_uint32(len(off) - 1), ptr(off), ptr(s) if len(s) else None), self.ctx.h)
+        self.n = len(off) - 1
 
     def boneAttachments(self, instance, bone, relative7, parent_transforms, original_scale3):
         """updateBoneAttachment (render_module.cpp:377-405) for a batch: world Transforms of entities attached to posed bones."""

@@ -75,7 +75,7 @@ struct AnimParams {
 	uint32_t bone_count;
 	uint32_t max_level;
 	uint32_t n_instances;
-	const uint32_t* clip_index;
+	union { const uint32_t* clip_index; const uint32_t* sample_offsets; }; // sample lists: [n_instances + 1] CSR offsets
 	uint32_t* time_ticks;
 	float* out_dq;    // n * B * 8 or null
 	float* out_mtx;   // n * B * 16 or null
@@ -84,12 +84,16 @@ struct AnimParams {
 	uint32_t dt_ticks;   // |time_delta| in ticks
 	int dt_negative;
 	int advance;
-	// blend layers on top of the base clip (lb200_animation_set_layers): [instance][n_layers]
+	// blend layers on top of the base clip (lb200_animation_set_layers): [instance][n_layers]; n_layers == SAMPLE_LISTS: the system is
+	// in sample-list mode (lb200_animation_set_samples) and the layer fields hold the lists and the bind pose instead
 	uint32_t n_layers;
-	const uint32_t* layer_clip;
-	const uint32_t* layer_time;
+	union { const uint32_t* layer_clip; const uint4* samples; };     // sample lists: lb200_sample entries
+	union { const uint32_t* layer_time; const float4* bind_pose; };  // sample lists: bind pos[B], then bind rot[B]
 	const float* layer_weight;
 };
+
+// AnimParams::n_layers of a system in sample-list mode (set_layers allows at most 16 layers)
+constexpr uint32_t SAMPLE_LISTS = 0xffffffffu;
 
 // unaligned little-endian u64 at byte address `byte` of a word-addressed stream (the reference memcpy's 8 bytes, animation.cpp:44)
 __device__ __forceinline__ unsigned long long load_u64_unaligned(const uint32_t* __restrict__ words, uint32_t byte) {
@@ -244,12 +248,12 @@ struct AnimSysParams {
 	uint32_t bone_count;
 	uint32_t max_level;
 	uint32_t n_instances;
-	uint32_t n_layers;
-	const uint32_t* clip_index;
+	uint32_t n_layers;   // SAMPLE_LISTS: sample-list mode, the unions hold what AnimParams' unions hold
+	union { const uint32_t* clip_index; const uint32_t* sample_offsets; };
 	uint32_t* time_ticks;
 	float* out_dq; float* out_mtx; float* out_pos; float* out_rot; // null where the palette flags do not ask for the output
-	const uint32_t* layer_clip;
-	const uint32_t* layer_time;
+	union { const uint32_t* layer_clip; const uint4* samples; };
+	union { const uint32_t* layer_time; const float4* bind_pose; };
 	const float* layer_weight;
 };
 static_assert(sizeof(AnimSysParams) == 160, "");
@@ -270,7 +274,11 @@ struct AnimManyParams {
 // One instance group of G lanes: sample, blend layers, computeAbsolute, palettes and the time advance of every instance of block
 // `block` of a system.  P holds the system's tables (AnimParams or AnimSysParams), A the time step (dt_ticks, dt_negative, advance).
 // pose_palette_kernel and pose_palette_many_kernel both run it, so the reference arithmetic exists once.
-template <int G, class SP, class AP>
+// Which start and sample source the body compiles: POSE_EITHER reads the mode of each system (pose_palette_many_kernel); the per-system
+// kernel compiles one mode per instantiation, so that clip mode runs the code it ran before sample lists existed.
+enum PoseMode { POSE_CLIPS, POSE_LISTS, POSE_EITHER };
+
+template <int G, int MODE, class SP, class AP>
 __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, const uint32_t block) {
 	extern __shared__ float4 smem4[];
 	constexpr int INST_PER_BLOCK = POSE_THREADS / G;
@@ -305,53 +313,80 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 	const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (lane & ~(G - 1)));
 
 	if (valid) {
-		const DevClip clip = P.clips[P.clip_index[inst]];
-		const uint32_t ticks = P.time_ticks[inst];
-
-		// animation.h:27 toFrame: float(value / double(ONE_SECOND) * fps); animation.cpp:131-133
-		const float frame = __double2float_rn(LB_DMUL(__uint2double_rn(ticks) / 32768.0, (double)clip.fps));
-		const float hi = LB_FSUB(__uint2float_rn(clip.frame_count), 0.00001f);
-		float sample = frame > 0.f ? frame : 0.f; // maximum(value, min): value > min ? value : min
-		sample = sample < hi ? sample : hi;       // minimum(x, max)
-		const uint32_t sample_idx = (uint32_t)sample;
-		const float t = LB_FSUB(sample, __uint2float_rn(sample_idx));
-
-		// Model::getRelativePose (model.cpp:226-237) + Animation::getRelativePose (animation.cpp:117-204) from the decoded keyframes:
-		// the two frames of a track do not depend on the instance, so they were unpacked once per clip (decode_clips_kernel) with the
-		// reference's arithmetic; here only the per-instance part remains: lerp (math.cpp:194-201) / simd_nlerp (simd_math.h:107-123)
-		// for animated tracks, plain copy for constant tracks and untracked bones (which keep the bind pose).
-		const float4* k0p = P.key_pos + clip.key_off + (size_t)sample_idx * Bp;
-		const float4* k0r = P.key_rot + clip.key_off + (size_t)sample_idx * Bp;
-		const unsigned char* kf = P.key_flags + clip.flag_off;
-		for (uint32_t b = sub; b < B; b += G) {
-			const uint32_t fl = kf[b];
-			float4 p = __ldg(k0p + b);
-			float4 r = __ldg(k0r + b);
-			if (fl & 1u) {
-				const float4 p1 = __ldg(k0p + Bp + b);
-				const V3 v = lerp(v3(p.x, p.y, p.z), v3(p1.x, p1.y, p1.z), t);
-				p = make_float4(v.x, v.y, v.z, 0.f);
+		// the instance's start pose, then its samples [k_begin, k_end): the layers after the base clip in clip mode, the instance's
+		// list after the bind pose in sample-list mode
+		const bool lists = MODE == POSE_EITHER ? P.n_layers == SAMPLE_LISTS : MODE == POSE_LISTS;
+		size_t k_begin, k_end;
+		uint32_t ticks = 0, length = 0; // clip mode: the base clip's time and length, for the time step
+		if (lists) {
+			k_begin = P.sample_offsets[inst];
+			k_end = P.sample_offsets[inst + 1];
+			for (uint32_t b = sub; b < B; b += G) { // Model::getRelativePose, model.cpp:226-237
+				s_pos[b] = __ldg(P.bind_pose + b);
+				s_rot[b] = __ldg(P.bind_pose + B + b);
 			}
-			if (fl & 2u) {
-				const float4 r1 = __ldg(k0r + Bp + b);
-				const Q4 q = simd_nlerp(q4(r.x, r.y, r.z, r.w), q4(r1.x, r1.y, r1.z, r1.w), t);
-				r = make_float4(q.x, q.y, q.z, q.w);
+		}
+		else {
+			const DevClip clip = P.clips[P.clip_index[inst]];
+			ticks = P.time_ticks[inst];
+			length = clip.length_ticks;
+			k_begin = (size_t)inst * P.n_layers;
+			k_end = k_begin + P.n_layers;
+
+			// animation.h:27 toFrame: float(value / double(ONE_SECOND) * fps); animation.cpp:131-133
+			const float frame = __double2float_rn(LB_DMUL(__uint2double_rn(ticks) / 32768.0, (double)clip.fps));
+			const float hi = LB_FSUB(__uint2float_rn(clip.frame_count), 0.00001f);
+			float sample = frame > 0.f ? frame : 0.f; // maximum(value, min): value > min ? value : min
+			sample = sample < hi ? sample : hi;       // minimum(x, max)
+			const uint32_t sample_idx = (uint32_t)sample;
+			const float t = LB_FSUB(sample, __uint2float_rn(sample_idx));
+
+			// Model::getRelativePose (model.cpp:226-237) + Animation::getRelativePose (animation.cpp:117-204) from the decoded keyframes:
+			// the two frames of a track do not depend on the instance, so they were unpacked once per clip (decode_clips_kernel) with the
+			// reference's arithmetic; here only the per-instance part remains: lerp (math.cpp:194-201) / simd_nlerp (simd_math.h:107-123)
+			// for animated tracks, plain copy for constant tracks and untracked bones (which keep the bind pose).
+			const float4* k0p = P.key_pos + clip.key_off + (size_t)sample_idx * Bp;
+			const float4* k0r = P.key_rot + clip.key_off + (size_t)sample_idx * Bp;
+			const unsigned char* kf = P.key_flags + clip.flag_off;
+			for (uint32_t b = sub; b < B; b += G) {
+				const uint32_t fl = kf[b];
+				float4 p = __ldg(k0p + b);
+				float4 r = __ldg(k0r + b);
+				if (fl & 1u) {
+					const float4 p1 = __ldg(k0p + Bp + b);
+					const V3 v = lerp(v3(p.x, p.y, p.z), v3(p1.x, p1.y, p1.z), t);
+					p = make_float4(v.x, v.y, v.z, 0.f);
+				}
+				if (fl & 2u) {
+					const float4 r1 = __ldg(k0r + Bp + b);
+					const Q4 q = simd_nlerp(q4(r.x, r.y, r.z, r.w), q4(r1.x, r1.y, r1.z, r1.w), t);
+					r = make_float4(q.x, q.y, q.z, q.w);
+				}
+				s_pos[b] = p;
+				s_rot[b] = r;
 			}
-			s_pos[b] = p;
-			s_rot[b] = r;
 		}
 		__syncwarp(gmask);
 
-		// Blend layers (the animator's stack of weighted samples, controller.cpp:267-292 -> Animation::getRelativePose with
-		// ctx.weight): every bone the layer's clip has a track for — constant or animated — moves towards the layer's sample,
-		// lerp (math.cpp:194-201) for positions and simd_nlerp for rotations when weight < 0.9999 (animation.cpp:294-311), plain
-		// replacement otherwise; bones without a track are left alone (animation.cpp:136-203).  Bones are independent: no sync inside.
-		for (uint32_t layer = 0; layer < P.n_layers; ++layer) {
-			const size_t li = (size_t)inst * P.n_layers + layer;
-			const DevClip lclip = P.clips[P.layer_clip[li]];
-			const float w = P.layer_weight[li];
+		// Blend layers and sample lists (the animator's stack of weighted samples, controller.cpp:267-292 -> Animation::getRelativePose
+		// with ctx.weight): every bone the sample's clip has a track for — constant or animated — moves towards the sample, lerp
+		// (math.cpp:194-201) for positions and simd_nlerp for rotations when weight < 0.9999 (animation.cpp:294-311), plain replacement
+		// otherwise; bones without a track are left alone (animation.cpp:136-203).  Bones are independent: no sync inside.
+		for (size_t li = k_begin; li < k_end; ++li) {
+			uint32_t lc, ltime;
+			float w;
+			if (lists) {
+				const uint4 e = __ldg(P.samples + li);
+				lc = e.x; w = __uint_as_float(e.z);
+				const uint32_t len = P.clips[lc].length_ticks;
+				ltime = e.w ? e.y % len : (e.y < len ? e.y : len); // getPose, controller.cpp:148
+			}
+			else {
+				lc = P.layer_clip[li]; ltime = P.layer_time[li]; w = P.layer_weight[li];
+			}
+			const DevClip lclip = P.clips[lc];
 			const bool use_weight = w < 0.9999f;
-			const float lframe = __double2float_rn(LB_DMUL(__uint2double_rn(P.layer_time[li]) / 32768.0, (double)lclip.fps));
+			const float lframe = __double2float_rn(LB_DMUL(__uint2double_rn(ltime) / 32768.0, (double)lclip.fps));
 			const float lhi = LB_FSUB(__uint2float_rn(lclip.frame_count), 0.00001f);
 			float ls = lframe > 0.f ? lframe : 0.f;
 			ls = ls < lhi ? ls : lhi;
@@ -443,8 +478,8 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 		}
 
 		// animation_module.cpp:458-469
-		if (A.advance && sub == 0) {
-			const uint32_t l = clip.length_ticks;
+		if (A.advance && !lists && sub == 0) {
+			const uint32_t l = length;
 			uint32_t nt;
 			if (!A.dt_negative) nt = (ticks + A.dt_ticks) % l;
 			else nt = (ticks + l - (A.dt_ticks % l)) % l;
@@ -456,9 +491,9 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 // G lanes cooperate on one instance (32 / G instances per warp): per-bone phases stride the bones by G, the absolute pass
 // walks depth levels with up to G bones of a level in flight.  G is 8 unless LB200_POSE_LANES or lb200_animation_set_launch asks
 // for another (lb200_animation_update).
-template <int G>
+template <int G, bool LISTS>
 __global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimParams P) {
-	pose_palette_body<G>(P, P, blockIdx.x);
+	pose_palette_body<G, LISTS ? POSE_LISTS : POSE_CLIPS>(P, P, blockIdx.x);
 }
 
 // The same for up to POSE_MANY_CAP systems in one grid (lb200_animation_update_many): each block finds its system by a binary search
@@ -473,7 +508,7 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const _
 		else lo = mid + 1;
 	}
 	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
-	pose_palette_body<G>(M.sys[lo], M, blockIdx.x - first_block);
+	pose_palette_body<G, POSE_EITHER>(M.sys[lo], M, blockIdx.x - first_block);
 }
 
 // ---- skinning ------------------------------------------------------------------------------------------------
@@ -627,6 +662,9 @@ struct lb200_animation {
 	int last_pose_lanes = 0, last_skin_group = 0;
 	DeviceArray<uint32_t> d_clip_index, d_time;
 	uint32_t n_layers = 0; DeviceArray<uint32_t> d_layer_clip, d_layer_time; DeviceArray<float> d_layer_weight; // all three or none
+	// sample-list mode (lb200_animation_set_samples): CSR offsets [max_instances + 1] and the samples, grown to the largest list set
+	bool sample_lists = false;
+	DeviceArray<uint32_t> d_sample_offsets; DeviceArray<lb200_sample> d_samples;
 	// palettes and poses, allocated by the first update that asks for them; d_pos / d_rot and d_rel_pos / d_rel_rot go in pairs
 	DeviceArray<float> d_dq, d_mtx, d_pos, d_rot;
 	DeviceArray<float> d_rel_pos, d_rel_rot; // Pose::computeRelative of d_pos / d_rot
@@ -811,10 +849,12 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 	{
 		const int smem_max = (int)(sizeof(float4) * (2 * 196 * (POSE_THREADS / 8) + 2 * 196 + 128));
 		const int smem_max4 = (int)std::min<size_t>(220 * 1024, sizeof(float4) * (2 * 196 * (POSE_THREADS / 4) + 2 * 196 + 128));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		for (int lists = 0; lists < 2; ++lists) {
+			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<4, true> : pose_palette_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
+			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<8, true> : pose_palette_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<16, true> : pose_palette_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<32, true> : pose_palette_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		}
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
@@ -844,6 +884,36 @@ int lb200_animation_set_instances(lb200_animation* a, const uint32_t* clip_index
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	a->n_instances = n;
 	a->n_layers = 0; // layer tables are per instance: set them again after changing the instances
+	a->sample_lists = false;
+	return LB200_OK;
+}
+
+int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples) {
+	if (!a || !offsets || n_instances > a->max_instances) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = a->ctx;
+	if (offsets[0] != 0) { lb200_set_error(ctx, "set_samples: offsets[0] is %u, not 0", offsets[0]); return LB200_ERR_INVALID; }
+	for (uint32_t i = 0; i < n_instances; ++i) {
+		if (offsets[i + 1] < offsets[i]) { lb200_set_error(ctx, "set_samples: offsets decrease at instance %u", i); return LB200_ERR_INVALID; }
+	}
+	const uint32_t total = offsets[n_instances];
+	if (total && !samples) return LB200_ERR_INVALID;
+	for (uint32_t k = 0; k < total; ++k) {
+		if (samples[k].clip >= a->n_clips) { lb200_set_error(ctx, "set_samples: sample %u: clip %u out of range", k, samples[k].clip); return LB200_ERR_INVALID; }
+	}
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	if (!a->d_sample_offsets) LB200_CUDA(ctx, a->d_sample_offsets.alloc((size_t)a->max_instances + 1));
+	if (a->d_samples.size() < total) { // allocated before the old list goes, so a failed allocation leaves the system as it was
+		DeviceArray<lb200_sample> grown;
+		LB200_CUDA(ctx, grown.alloc(std::max<size_t>(total, 2 * a->d_samples.size())));
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // an update still reading the old list
+		a->d_samples = std::move(grown);
+	}
+	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_sample_offsets, offsets, sizeof(uint32_t) * ((size_t)n_instances + 1), cudaMemcpyHostToDevice, ctx->stream));
+	if (total) LB200_CUDA(ctx, cudaMemcpyAsync(a->d_samples, samples, sizeof(lb200_sample) * total, cudaMemcpyHostToDevice, ctx->stream));
+	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+	a->n_instances = n_instances;
+	a->n_layers = 0;
+	a->sample_lists = true;
 	return LB200_OK;
 }
 
@@ -894,6 +964,18 @@ template <class T> void setTimeStep(T& A, float time_delta) {
 	A.dt_ticks = (uint32_t)((A.dt_negative ? -time_delta : time_delta) * (float)(1 << 15));
 	A.advance = 1;
 }
+// what the pose body samples: the base clips and layers of clip mode, or the sample lists and the bind pose (AnimParams' unions)
+template <class T> void setSources(T& P, const lb200_animation* a) {
+	P.layer_weight = a->d_layer_weight;
+	if (a->sample_lists) {
+		P.n_layers = SAMPLE_LISTS;
+		P.sample_offsets = a->d_sample_offsets; P.samples = reinterpret_cast<const uint4*>(a->d_samples.get()); P.bind_pose = a->d_bind;
+	}
+	else {
+		P.n_layers = a->n_layers;
+		P.clip_index = a->d_clip_index; P.layer_clip = a->d_layer_clip; P.layer_time = a->d_layer_time;
+	}
+}
 // pose_palette_kernel<G> over one system's instances (the caller checks the launch)
 void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flags) {
 	AnimParams P;
@@ -901,8 +983,8 @@ void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flag
 	P.key_pos = a->d_key_pos; P.key_rot = a->d_key_rot; P.key_flags = a->d_key_flags;
 	P.bind_pos = a->d_bind; P.bind_rot = a->d_bind + a->bone_count; P.inv_bind_pos = a->d_bind + 2 * a->bone_count; P.inv_bind_rot = a->d_bind + 3 * a->bone_count; P.parents = a->d_parents; P.level_bones = a->d_level_bones; P.level_start = a->d_level_start;
 	P.bone_count = a->bone_count; P.max_level = a->max_level; P.n_instances = a->n_instances;
-	P.clip_index = a->d_clip_index; P.time_ticks = a->d_time;
-	P.n_layers = a->n_layers; P.layer_clip = a->d_layer_clip; P.layer_time = a->d_layer_time; P.layer_weight = a->d_layer_weight;
+	P.time_ticks = a->d_time;
+	setSources(P, a);
 	P.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
 	P.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
 	P.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
@@ -912,10 +994,11 @@ void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flag
 	const unsigned blocks = (a->n_instances + per_block - 1) / per_block;
 	const size_t smem = poseSmemBytes(a, per_block);
 	cudaStream_t st = a->ctx->stream;
-	if (G == 4) pose_palette_kernel<4><<<blocks, POSE_THREADS, smem, st>>>(P);
-	else if (G == 8) pose_palette_kernel<8><<<blocks, POSE_THREADS, smem, st>>>(P);
-	else if (G == 16) pose_palette_kernel<16><<<blocks, POSE_THREADS, smem, st>>>(P);
-	else pose_palette_kernel<32><<<blocks, POSE_THREADS, smem, st>>>(P);
+	const bool lists = a->sample_lists;
+	if (G == 4) (lists ? pose_palette_kernel<4, true> : pose_palette_kernel<4, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
+	else if (G == 8) (lists ? pose_palette_kernel<8, true> : pose_palette_kernel<8, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
+	else if (G == 16) (lists ? pose_palette_kernel<16, true> : pose_palette_kernel<16, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
+	else (lists ? pose_palette_kernel<32, true> : pose_palette_kernel<32, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
 }
 } // namespace
 
@@ -990,8 +1073,8 @@ int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, flo
 			S.inv_bind_pos = a->d_bind + 2 * a->bone_count; S.inv_bind_rot = a->d_bind + 3 * a->bone_count;
 			S.parents = a->d_parents; S.level_bones = a->d_level_bones; S.level_start = a->d_level_start;
 			S.bone_count = a->bone_count; S.max_level = a->max_level; S.n_instances = a->n_instances;
-			S.n_layers = a->n_layers; S.layer_clip = a->d_layer_clip; S.layer_time = a->d_layer_time; S.layer_weight = a->d_layer_weight;
-			S.clip_index = a->d_clip_index; S.time_ticks = a->d_time;
+			S.time_ticks = a->d_time;
+			setSources(S, a);
 			S.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
 			S.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
 			S.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
@@ -1077,6 +1160,7 @@ int lb200_animation_get_pose(lb200_animation* a, uint32_t first, uint32_t count,
 int lb200_animation_set_layers(lb200_animation* a, uint32_t n_layers, const uint32_t* clip_index, const uint32_t* time_ticks, const float* weight) {
 	if (!a || n_layers > 16) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = a->ctx;
+	if (a->sample_lists) { lb200_set_error(ctx, "set_layers: the system is in sample-list mode"); return LB200_ERR_INVALID; }
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	if (n_layers == 0) { a->n_layers = 0; return LB200_OK; }
 	if (!clip_index || !time_ticks || !weight || !a->n_instances) return LB200_ERR_INVALID;
@@ -1191,6 +1275,7 @@ int lb200_animation_blend_pose(lb200_animation* a, const lb200_animation* b, flo
 }
 
 int lb200_animation_get_times(lb200_animation* a, uint32_t first, uint32_t count, uint32_t* out_ticks) {
+	if (a && a->sample_lists) { lb200_set_error(a->ctx, "get_times: the system is in sample-list mode, its times are the caller's"); return LB200_ERR_INVALID; }
 	return readBack(a, a ? a->d_time.get() : nullptr, sizeof(uint32_t), first, count, out_ticks);
 }
 int lb200_animation_get_skinned(lb200_animation* a, uint32_t first, uint32_t count, float* out_pos3) {
