@@ -687,8 +687,33 @@ typedef struct { uint32_t clip; uint32_t time_ticks; float weight; uint32_t loop
  * - LB200_ERR_INVALID, with nothing changed: n_instances > max_instances, NULL offsets, NULL samples with offsets[n_instances] > 0,
  *   offsets[0] != 0, decreasing offsets, a clip index out of range.  (Clips of length 0 are refused by create, so a looped sample never
  *   divides by 0.)
- * - The lists are copied before the call returns. */
+ * - The lists are copied before the call returns.
+ * - set_samples(a, n, offsets, samples) is set_stacks(a, n, offsets, samples, NULL, NULL): it drops the IK ops of an earlier set_stacks. */
 LB200_API int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples);
+/* One IK instruction of an animator's blend stack (controller.cpp:275-281).  32 bytes, read by the pose kernel as two 128-bit loads. */
+typedef struct {
+	uint32_t after;      /* how many of the instance's samples run before it: 0 = on the bind pose, list length = after all of them */
+	uint32_t leaf_bone;  /* bone index (Model::getBoneIndex of the instruction's BoneNameHash) */
+	uint32_t bone_count; /* bones of the chain, 1 .. 32, the leaf and its bone_count - 1 nearest ancestors */
+	float alpha;         /* what evalIK receives: the instruction's alpha * ctx.weight */
+	float target[3];     /* model space */
+	uint32_t reserved;
+} lb200_ik;
+/* Blend stacks: set_samples plus one CSR list of IK ops per instance (instance i owns iks[ik_offsets[i] .. ik_offsets[i+1])), each run
+ * between the instance's samples where its `after` puts it, as evalBlendStack runs the stack's instructions in order.  Ops of one
+ * instance have non-decreasing `after`; ops with the same `after` run in list order.  An op is evalIK (controller.cpp:166-265) on the
+ * relative pose at that point: nothing below alpha 0.001, otherwise the chain from the leaf up goes to model space, an unreachable
+ * target is pulled onto the chain's reach, 5 FABRIK iterations move the joints, Quat::vec3ToVec3 turns the moves into rotations, and
+ * the pose moves towards the result by lerp and the scalar nlerp with alpha.  Bit for bit what the reference computes, except where
+ * it computes a NaN (two coincident joints), whose payload may differ.
+ * - ik_offsets == NULL: no IK ops (set_samples).  Systems with IK ops run their own kernels; the others run the same code as before.
+ * - LB200_ERR_INVALID, with nothing changed: every refusal of set_samples, ik_offsets[0] != 0, decreasing ik_offsets, NULL iks with
+ *   ik_offsets[n_instances] > 0, `after` greater than the instance's sample count or smaller than the op before it in the instance,
+ *   leaf_bone >= the skeleton's bone count, bone_count 0 or above 32, a chain that leaves the skeleton (walking bone_count - 1
+ *   parents from the leaf reaches -1), which the reference meets with an ASSERT or undefined behaviour.
+ * - The ops are copied before the call returns; the chains are resolved from the skeleton then. */
+LB200_API int lb200_animation_set_stacks(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples,
+	const uint32_t* ik_offsets, const lb200_ik* iks);
 /* Pose::computeRelative (src/renderer/pose.cpp:136-146) of every instance's absolute pose (needs an update with LB200_PALETTE_POSE):
  * the parent-relative poses IK / ragdoll consumers start from (controller.cpp).  Kept in HBM next to the absolute ones. */
 LB200_API int lb200_animation_compute_relative(lb200_animation* a);

@@ -24,6 +24,9 @@ CONST_R_DTYPE = np.dtype([("bone_index", np.uint16), ("pad", np.uint16), ("value
 assert TRACK_DTYPE.itemsize == 32 and CONST_T_DTYPE.itemsize == 16 and CONST_R_DTYPE.itemsize == 20
 SAMPLE_DTYPE = np.dtype([("clip", np.uint32), ("time_ticks", np.uint32), ("weight", np.float32), ("looped", np.uint32)])  # lb200_sample
 assert SAMPLE_DTYPE.itemsize == 16
+IK_DTYPE = np.dtype([("after", np.uint32), ("leaf_bone", np.uint32), ("bone_count", np.uint32), ("alpha", np.float32), ("target", np.float32, 3),
+                     ("reserved", np.uint32)])  # lb200_ik
+assert IK_DTYPE.itemsize == 32
 
 
 def _pack_frames(per_track_values, bits_per_track):
@@ -391,6 +394,23 @@ class AnimationSystem:
         s = np.empty(len(np.atleast_1d(clip)), SAMPLE_DTYPE)
         s["clip"], s["time_ticks"], s["weight"], s["looped"] = clip, time_ticks, weight, looped
         check(self.L.lb200_animation_set_samples(self.h, C.c_uint32(len(off) - 1), ptr(off), ptr(s) if len(s) else None), self.ctx.h)
+        self.n = len(off) - 1
+
+    def setStacks(self, offsets, clip, time_ticks, weight, looped, ik_offsets, ik_after, ik_leaf, ik_bones, ik_alpha, ik_target):
+        """Blend stacks (lb200_animation_set_stacks): setSamples plus IK ops per instance (CSR ik_offsets), op k running evalIK
+        (controller.cpp:166-265) with (leaf bone index, bone count, alpha, model-space target [3]) after the first ik_after[k] samples of
+        its instance.  Ops of an instance have non-decreasing ik_after; equal ones run in list order."""
+        off = np.ascontiguousarray(offsets, np.uint32)
+        assert off.ndim == 1 and len(off) >= 1
+        s = np.empty(len(np.atleast_1d(clip)), SAMPLE_DTYPE)
+        s["clip"], s["time_ticks"], s["weight"], s["looped"] = clip, time_ticks, weight, looped
+        ik_off = np.ascontiguousarray(ik_offsets, np.uint32)
+        assert ik_off.shape == off.shape
+        ik = np.zeros(len(np.atleast_1d(ik_after)), IK_DTYPE)
+        ik["after"], ik["leaf_bone"], ik["bone_count"], ik["alpha"] = ik_after, ik_leaf, ik_bones, ik_alpha
+        ik["target"] = np.asarray(ik_target, np.float32).reshape(-1, 3)
+        check(self.L.lb200_animation_set_stacks(self.h, C.c_uint32(len(off) - 1), ptr(off), ptr(s) if len(s) else None, ptr(ik_off),
+                                                ptr(ik) if len(ik) else None), self.ctx.h)
         self.n = len(off) - 1
 
     def boneAttachments(self, instance, bone, relative7, parent_transforms, original_scale3):

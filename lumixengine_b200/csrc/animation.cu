@@ -76,7 +76,7 @@ struct AnimParams {
 	uint32_t max_level;
 	uint32_t n_instances;
 	union { const uint32_t* clip_index; const uint32_t* sample_offsets; }; // sample lists: [n_instances + 1] CSR offsets
-	uint32_t* time_ticks;
+	union { uint32_t* time_ticks; const uint32_t* ik_offsets; };           // sample lists: [n_instances + 1] CSR offsets of the IK ops, or null
 	float* out_dq;    // n * B * 8 or null
 	float* out_mtx;   // n * B * 16 or null
 	float* out_pos;   // n * B * 3 or null
@@ -89,11 +89,122 @@ struct AnimParams {
 	uint32_t n_layers;
 	union { const uint32_t* layer_clip; const uint4* samples; };     // sample lists: lb200_sample entries
 	union { const uint32_t* layer_time; const float4* bind_pose; };  // sample lists: bind pos[B], then bind rot[B]
-	const float* layer_weight;
+	union { const float* layer_weight; const uint4* iks; };          // sample lists: the IK ops (IkOp) and their bone paths
 };
 
 // AnimParams::n_layers of a system in sample-list mode (set_layers allows at most 16 layers)
 constexpr uint32_t SAMPLE_LISTS = 0xffffffffu;
+
+// The device form of one lb200_ik, two 128-bit loads: {after, path_len, bone_count, alpha} {target xyz, path_off}.  path_off is the byte
+// offset, from the start of the op table, of the root-to-leaf path of the leaf bone (path_len bone indices, one byte each, first the bone
+// whose parent is -1): the chain is its last bone_count entries and getAbsolutePosition of the chain's first parent folds the entries
+// before them.  lb200_animation_set_stacks resolves it from the skeleton, once per distinct leaf.
+constexpr uint32_t IK_MAX_BONES = 32; // controller.cpp:171 MAX_BONES_COUNT
+
+// evalIK (controller.cpp:166-265) of op `op` on one instance's relative pose in shared memory, run by one lane of the instance group.
+// The chain's working arrays live in that lane's local memory (L1): 1.3 KB that only one lane in G ever touches, which would cost every
+// block of the IK kernels that much shared memory per instance for a path most instances of a frame do not take.
+__device__ __noinline__ void eval_ik(float4* s_pos, float4* s_rot, const uint4* __restrict__ iks, uint32_t op) {
+	const uint4 a = __ldg(iks + 2 * op), b = __ldg(iks + 2 * op + 1);
+	const float alpha = __uint_as_float(a.w);
+	if (alpha < 0.001f) return;                                 // :167
+	const uint32_t n = a.z, path_len = a.y, first = path_len - n; // chain = path[first .. path_len), :184-187
+	const unsigned char* path = reinterpret_cast<const unsigned char*>(iks) + b.w;
+	V3 target = v3(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z));
+	unsigned char idx[IK_MAX_BONES];
+	Rigid tr[IK_MAX_BONES];
+	V3 old_pos[IK_MAX_BONES];
+	float len[IK_MAX_BONES - 1];
+	for (uint32_t i = 0; i < n; ++i) idx[i] = __ldg(path + first + i);
+	auto bone = [&](uint32_t j) {
+		const float4 p = s_pos[j], r = s_rot[j];
+		Rigid t;
+		t.pos = v3(p.x, p.y, p.z);
+		t.rot = q4(r.x, r.y, r.z, r.w);
+		return t;
+	};
+	// :190-198 getAbsolutePosition of the first bone's parent (:159-164): the left fold of the relative transforms from the root down
+	Rigid roots_parent;
+	if (first > 0) {
+		roots_parent = bone(__ldg(path));
+		for (uint32_t j = 1; j < first; ++j) roots_parent = rmul(roots_parent, bone(__ldg(path + j)));
+	}
+	else {
+		roots_parent.pos = v3(0, 0, 0);
+		roots_parent.rot = q4(0, 0, 0, 1);
+	}
+	// :200-210 bone space -> object space, bone lengths
+	float len_sum = 0;
+	Rigid parent_tr = roots_parent;
+	for (uint32_t i = 0; i < n; ++i) {
+		tr[i] = rmul(parent_tr, bone(idx[i]));
+		old_pos[i] = tr[i].pos;
+		if (i > 0) {
+			len[i - 1] = length(sub(tr[i].pos, tr[i - 1].pos));
+			len_sum = LB_FADD(len_sum, len[i - 1]);
+		}
+		parent_tr = tr[i];
+	}
+	// :212-216 an unreachable target moves onto the sphere the chain reaches
+	V3 to_target = sub(target, tr[0].pos);
+	if (LB_FMUL(len_sum, len_sum) < squared_length(to_target)) {
+		to_target = normalize(to_target);
+		target = add(tr[0].pos, muls(to_target, len_sum));
+	}
+	// :218-230 five FABRIK sweeps
+	for (uint32_t iteration = 0; iteration < 5; ++iteration) {
+		tr[n - 1].pos = target;
+		for (int i = (int)n - 1; i > 1; --i) {
+			const V3 dir = normalize(sub(tr[i - 1].pos, tr[i].pos));
+			tr[i - 1].pos = add(tr[i].pos, muls(dir, len[i - 1]));
+		}
+		for (uint32_t i = 1; i < n; ++i) {
+			const V3 dir = normalize(sub(tr[i].pos, tr[i - 1].pos));
+			tr[i].pos = add(tr[i - 1].pos, muls(dir, len[i - 1]));
+		}
+	}
+	// :233-239 rotations from the new positions
+	for (int i = (int)n - 2; i >= 0; --i) {
+		const Q4 rel_rot = vec3_to_vec3(sub(old_pos[i + 1], old_pos[i]), sub(tr[i + 1].pos, tr[i].pos));
+		tr[i].rot = qmul(rel_rot, tr[i].rot);
+	}
+	// :243-246 object space -> bone space; tr[i] then holds ik_out[i] for 0 < i < n (its rotation too for i < n - 1, :247-249)
+	for (int i = (int)n - 1; i > 0; --i) tr[i] = rmul(rinverted(tr[i - 1]), tr[i]);
+	// :250-264: ik_out[0] keeps the pose position, ik_out[n - 1] the pose rotation (with n == 1 the rotation of :253-257 wins); the pose
+	// moves towards ik_out by lerp and the scalar nlerp
+	for (uint32_t i = 0; i < n; ++i) {
+		const uint32_t j = idx[i];
+		const float4 p = s_pos[j], r = s_rot[j];
+		const V3 pose_pos = v3(p.x, p.y, p.z);
+		const Q4 pose_rot = q4(r.x, r.y, r.z, r.w);
+		V3 out_pos;
+		Q4 out_rot;
+		if (i == 0) {
+			out_pos = pose_pos;
+			out_rot = first > 0 ? qmul(conjugated(roots_parent.rot), tr[0].rot) : tr[0].rot;
+		}
+		else {
+			out_pos = tr[i].pos;
+			out_rot = i == n - 1 ? pose_rot : tr[i].rot;
+		}
+		const V3 np = lerp(pose_pos, out_pos, alpha);
+		const Q4 nr = nlerp(pose_rot, out_rot, alpha);
+		s_pos[j] = make_float4(np.x, np.y, np.z, 0.f);
+		s_rot[j] = make_float4(nr.x, nr.y, nr.z, nr.w);
+	}
+}
+
+// the IK ops of the instance whose `after` is `at` (the number of its samples applied so far), in list order, [ik, ik_end) advancing:
+// the group joins, one lane solves on the shared pose, the group joins again before any lane reads the pose
+template <class SP>
+__device__ __forceinline__ void run_ik_ops(const SP& P, float4* s_pos, float4* s_rot, uint32_t at, uint32_t& ik, uint32_t ik_end, int sub, unsigned gmask) {
+	while (ik < ik_end && __ldg(reinterpret_cast<const uint32_t*>(P.iks + 2 * ik)) == at) {
+		__syncwarp(gmask);
+		if (sub == 0) eval_ik(s_pos, s_rot, P.iks, ik);
+		__syncwarp(gmask);
+		++ik;
+	}
+}
 
 // unaligned little-endian u64 at byte address `byte` of a word-addressed stream (the reference memcpy's 8 bytes, animation.cpp:44)
 __device__ __forceinline__ unsigned long long load_u64_unaligned(const uint32_t* __restrict__ words, uint32_t byte) {
@@ -250,11 +361,11 @@ struct AnimSysParams {
 	uint32_t n_instances;
 	uint32_t n_layers;   // SAMPLE_LISTS: sample-list mode, the unions hold what AnimParams' unions hold
 	union { const uint32_t* clip_index; const uint32_t* sample_offsets; };
-	uint32_t* time_ticks;
+	union { uint32_t* time_ticks; const uint32_t* ik_offsets; };
 	float* out_dq; float* out_mtx; float* out_pos; float* out_rot; // null where the palette flags do not ask for the output
 	union { const uint32_t* layer_clip; const uint4* samples; };
 	union { const uint32_t* layer_time; const float4* bind_pose; };
-	const float* layer_weight;
+	union { const float* layer_weight; const uint4* iks; };
 };
 static_assert(sizeof(AnimSysParams) == 160, "");
 
@@ -275,10 +386,11 @@ struct AnimManyParams {
 // `block` of a system.  P holds the system's tables (AnimParams or AnimSysParams), A the time step (dt_ticks, dt_negative, advance).
 // pose_palette_kernel and pose_palette_many_kernel both run it, so the reference arithmetic exists once.
 // Which start and sample source the body compiles: POSE_EITHER reads the mode of each system (pose_palette_many_kernel); the per-system
-// kernel compiles one mode per instantiation, so that clip mode runs the code it ran before sample lists existed.
+// kernel compiles one mode per instantiation, so that clip mode runs the code it ran before sample lists existed.  IK compiles the
+// IK ops of sample lists in (pose_palette_ik_kernel, pose_palette_many_ik_kernel); the kernels without it run the code they ran before.
 enum PoseMode { POSE_CLIPS, POSE_LISTS, POSE_EITHER };
 
-template <int G, int MODE, class SP, class AP>
+template <int G, int MODE, class SP, class AP, bool IK = false>
 __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, const uint32_t block) {
 	extern __shared__ float4 smem4[];
 	constexpr int INST_PER_BLOCK = POSE_THREADS / G;
@@ -372,7 +484,11 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 		// with ctx.weight): every bone the sample's clip has a track for — constant or animated — moves towards the sample, lerp
 		// (math.cpp:194-201) for positions and simd_nlerp for rotations when weight < 0.9999 (animation.cpp:294-311), plain replacement
 		// otherwise; bones without a track are left alone (animation.cpp:136-203).  Bones are independent: no sync inside.
+		// With IK, the instance's IK ops run between the samples where their `after` puts them (evalBlendStack's instruction order).
+		uint32_t ik = 0, ik_end = 0;
+		if (IK && lists && P.ik_offsets) { ik = P.ik_offsets[inst]; ik_end = P.ik_offsets[inst + 1]; }
 		for (size_t li = k_begin; li < k_end; ++li) {
+			if (IK) run_ik_ops(P, s_pos, s_rot, (uint32_t)(li - k_begin), ik, ik_end, sub, gmask);
 			uint32_t lc, ltime;
 			float w;
 			if (lists) {
@@ -425,6 +541,7 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 				}
 			}
 		}
+		if (IK) run_ik_ops(P, s_pos, s_rot, (uint32_t)(k_end - k_begin), ik, ik_end, sub, gmask);
 		__syncwarp(gmask);
 
 		// Pose::computeAbsolute, pose.cpp:66-133: bones of one depth level are independent (the reference's 4-wide path
@@ -509,6 +626,25 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const _
 	}
 	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
 	pose_palette_body<G, POSE_EITHER>(M.sys[lo], M, blockIdx.x - first_block);
+}
+
+// pose_palette_kernel<G, true> with the IK ops of the lists (lb200_animation_set_stacks): chosen only for a system that has IK ops
+template <int G>
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_ik_kernel(const __grid_constant__ AnimParams P) {
+	pose_palette_body<G, POSE_LISTS, AnimParams, AnimParams, true>(P, P, blockIdx.x);
+}
+
+// pose_palette_many_kernel<G> with the IK ops: chosen only for a launch in which some system has IK ops
+template <int G>
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_ik_kernel(const __grid_constant__ AnimManyParams M) {
+	uint32_t lo = 0, hi = M.n_systems - 1;
+	while (lo < hi) {
+		const uint32_t mid = (lo + hi) >> 1;
+		if (blockIdx.x < M.block_end[mid]) hi = mid;
+		else lo = mid + 1;
+	}
+	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
+	pose_palette_body<G, POSE_EITHER, AnimSysParams, AnimManyParams, true>(M.sys[lo], M, blockIdx.x - first_block);
 }
 
 // ---- skinning ------------------------------------------------------------------------------------------------
@@ -665,6 +801,11 @@ struct lb200_animation {
 	// sample-list mode (lb200_animation_set_samples): CSR offsets [max_instances + 1] and the samples, grown to the largest list set
 	bool sample_lists = false;
 	DeviceArray<uint32_t> d_sample_offsets; DeviceArray<lb200_sample> d_samples;
+	// IK ops of the lists (lb200_animation_set_stacks): CSR offsets [max_instances + 1], the op table (IkOp pairs, then the leaves' bone
+	// paths) grown like the samples; n_ik = ops of the current lists (0: the IK-free kernels run)
+	uint32_t n_ik = 0;
+	DeviceArray<uint32_t> d_ik_offsets; DeviceArray<uint4> d_iks;
+	std::vector<short> parents; // Model::getBoneParent, for resolving IK chains
 	// palettes and poses, allocated by the first update that asks for them; d_pos / d_rot and d_rel_pos / d_rel_rot go in pairs
 	DeviceArray<float> d_dq, d_mtx, d_pos, d_rot;
 	DeviceArray<float> d_rel_pos, d_rel_rot; // Pose::computeRelative of d_pos / d_rot
@@ -782,6 +923,7 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 	if (!a) return LB200_ERR_CUDA;
 	a->ctx = ctx; a->bone_count = B; a->max_level = max_level; a->n_clips = n_clips; a->max_instances = max_instances;
 	a->first_nonroot = first;
+	a->parents.assign(sk->parents, sk->parents + B);
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	LB200_CUDA(ctx, a->d_clips.alloc(n_clips, TABLE_MIN_BYTES));
 	LB200_CUDA(ctx, a->d_tracks.alloc(tracks.size(), TABLE_MIN_BYTES));
@@ -859,6 +1001,14 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
 	}
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * 196 * 3 * sizeof(float4))));
 	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(8 * 196 * 3 * sizeof(float4))));
@@ -885,10 +1035,13 @@ int lb200_animation_set_instances(lb200_animation* a, const uint32_t* clip_index
 	a->n_instances = n;
 	a->n_layers = 0; // layer tables are per instance: set them again after changing the instances
 	a->sample_lists = false;
+	a->n_ik = 0;
 	return LB200_OK;
 }
 
-int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples) {
+int lb200_animation_set_stacks(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples,
+	const uint32_t* ik_offsets, const lb200_ik* iks)
+{
 	if (!a || !offsets || n_instances > a->max_instances) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = a->ctx;
 	if (offsets[0] != 0) { lb200_set_error(ctx, "set_samples: offsets[0] is %u, not 0", offsets[0]); return LB200_ERR_INVALID; }
@@ -900,21 +1053,84 @@ int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const 
 	for (uint32_t k = 0; k < total; ++k) {
 		if (samples[k].clip >= a->n_clips) { lb200_set_error(ctx, "set_samples: sample %u: clip %u out of range", k, samples[k].clip); return LB200_ERR_INVALID; }
 	}
+	// IK ops: validated, then put in their device form (IkOp) with the root-to-leaf path of each distinct leaf after the ops
+	const uint32_t n_ik = ik_offsets ? ik_offsets[n_instances] : 0;
+	std::vector<uint4> table;
+	if (ik_offsets) {
+		if (ik_offsets[0] != 0) { lb200_set_error(ctx, "set_stacks: ik_offsets[0] is %u, not 0", ik_offsets[0]); return LB200_ERR_INVALID; }
+		for (uint32_t i = 0; i < n_instances; ++i) {
+			if (ik_offsets[i + 1] < ik_offsets[i]) { lb200_set_error(ctx, "set_stacks: ik_offsets decrease at instance %u", i); return LB200_ERR_INVALID; }
+		}
+		if (n_ik && !iks) return LB200_ERR_INVALID;
+		const uint32_t B = a->bone_count;
+		std::vector<unsigned char> paths;
+		std::vector<int64_t> leaf_path(B, -1); // byte offset of the leaf's path inside `paths`
+		std::vector<uint32_t> path_len(B, 0);
+		table.resize(2 * (size_t)n_ik);
+		for (uint32_t i = 0; i < n_instances; ++i) {
+			const uint32_t list_len = offsets[i + 1] - offsets[i];
+			for (uint32_t k = ik_offsets[i]; k < ik_offsets[i + 1]; ++k) {
+				const lb200_ik& op = iks[k];
+				if (op.after > list_len || (k > ik_offsets[i] && op.after < iks[k - 1].after)) {
+					lb200_set_error(ctx, "set_stacks: IK op %u: after %u is past the instance's %u samples or before the op it follows", k, op.after, list_len);
+					return LB200_ERR_INVALID;
+				}
+				if (op.leaf_bone >= B || op.bone_count == 0 || op.bone_count > IK_MAX_BONES) {
+					lb200_set_error(ctx, "set_stacks: IK op %u: leaf bone %u / bone count %u out of range", k, op.leaf_bone, op.bone_count);
+					return LB200_ERR_INVALID;
+				}
+				if (leaf_path[op.leaf_bone] < 0) { // Model::getBoneParent walk from the leaf to the bone whose parent is -1
+					std::vector<unsigned char> up;
+					for (int b = (int)op.leaf_bone; b >= 0; b = a->parents[b]) {
+						if ((uint32_t)b >= B || up.size() == B) { lb200_set_error(ctx, "set_stacks: bone %u: its parents leave the skeleton or loop", op.leaf_bone); return LB200_ERR_INVALID; }
+						up.push_back((unsigned char)b);
+					}
+					leaf_path[op.leaf_bone] = (int64_t)paths.size();
+					path_len[op.leaf_bone] = (uint32_t)up.size();
+					paths.insert(paths.end(), up.rbegin(), up.rend());
+				}
+				if (op.bone_count > path_len[op.leaf_bone]) { // controller.cpp:185-186 would read bone -1
+					lb200_set_error(ctx, "set_stacks: IK op %u: a chain of %u bones from bone %u leaves the skeleton", k, op.bone_count, op.leaf_bone);
+					return LB200_ERR_INVALID;
+				}
+				table[2 * (size_t)k] = make_uint4(op.after, path_len[op.leaf_bone], op.bone_count, __builtin_bit_cast(uint32_t, op.alpha));
+				table[2 * (size_t)k + 1] = make_uint4(__builtin_bit_cast(uint32_t, op.target[0]), __builtin_bit_cast(uint32_t, op.target[1]),
+					__builtin_bit_cast(uint32_t, op.target[2]), (uint32_t)(sizeof(uint4) * table.size() + leaf_path[op.leaf_bone]));
+			}
+		}
+		const size_t ops_words = table.size();
+		table.resize(ops_words + (paths.size() + 15) / 16, make_uint4(0, 0, 0, 0));
+		if (!paths.empty()) memcpy(table.data() + ops_words, paths.data(), paths.size());
+	}
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	// every allocation before anything is replaced, so that a failed one leaves the system as it was
 	if (!a->d_sample_offsets) LB200_CUDA(ctx, a->d_sample_offsets.alloc((size_t)a->max_instances + 1));
-	if (a->d_samples.size() < total) { // allocated before the old list goes, so a failed allocation leaves the system as it was
-		DeviceArray<lb200_sample> grown;
-		LB200_CUDA(ctx, grown.alloc(std::max<size_t>(total, 2 * a->d_samples.size())));
-		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // an update still reading the old list
-		a->d_samples = std::move(grown);
+	if (n_ik && !a->d_ik_offsets) LB200_CUDA(ctx, a->d_ik_offsets.alloc((size_t)a->max_instances + 1));
+	DeviceArray<lb200_sample> grown;
+	DeviceArray<uint4> grown_iks;
+	if (a->d_samples.size() < total) LB200_CUDA(ctx, grown.alloc(std::max<size_t>(total, 2 * a->d_samples.size())));
+	if (a->d_iks.size() < table.size()) LB200_CUDA(ctx, grown_iks.alloc(std::max<size_t>(table.size(), 2 * a->d_iks.size())));
+	if (grown || grown_iks) {
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // an update still reading the old lists
+		if (grown) a->d_samples = std::move(grown);
+		if (grown_iks) a->d_iks = std::move(grown_iks);
 	}
 	LB200_CUDA(ctx, cudaMemcpyAsync(a->d_sample_offsets, offsets, sizeof(uint32_t) * ((size_t)n_instances + 1), cudaMemcpyHostToDevice, ctx->stream));
 	if (total) LB200_CUDA(ctx, cudaMemcpyAsync(a->d_samples, samples, sizeof(lb200_sample) * total, cudaMemcpyHostToDevice, ctx->stream));
+	if (n_ik) {
+		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_ik_offsets, ik_offsets, sizeof(uint32_t) * ((size_t)n_instances + 1), cudaMemcpyHostToDevice, ctx->stream));
+		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_iks, table.data(), sizeof(uint4) * table.size(), cudaMemcpyHostToDevice, ctx->stream));
+	}
 	LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
 	a->n_instances = n_instances;
 	a->n_layers = 0;
 	a->sample_lists = true;
+	a->n_ik = n_ik;
 	return LB200_OK;
+}
+
+int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples) {
+	return lb200_animation_set_stacks(a, n_instances, offsets, samples, nullptr, nullptr);
 }
 
 } // extern "C"
@@ -970,13 +1186,16 @@ template <class T> void setSources(T& P, const lb200_animation* a) {
 	if (a->sample_lists) {
 		P.n_layers = SAMPLE_LISTS;
 		P.sample_offsets = a->d_sample_offsets; P.samples = reinterpret_cast<const uint4*>(a->d_samples.get()); P.bind_pose = a->d_bind;
+		P.ik_offsets = a->n_ik ? a->d_ik_offsets.get() : nullptr; P.iks = a->d_iks; // over time_ticks and layer_weight, which lists do not read
 	}
 	else {
 		P.n_layers = a->n_layers;
 		P.clip_index = a->d_clip_index; P.layer_clip = a->d_layer_clip; P.layer_time = a->d_layer_time;
 	}
 }
-// pose_palette_kernel<G> over one system's instances (the caller checks the launch)
+// whether a system runs the IK kernels: sample lists with IK ops
+bool hasIk(const lb200_animation* a) { return a->sample_lists && a->n_ik; }
+// pose_palette_kernel<G> (pose_palette_ik_kernel<G> for a system with IK ops) over one system's instances (the caller checks the launch)
 void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flags) {
 	AnimParams P;
 	P.clips = a->d_clips; P.tracks = a->d_tracks; P.const_t = a->d_const_t; P.const_r_value = a->d_const_r_value; P.const_r_bone = a->d_const_r_bone; P.stream = a->d_stream;
@@ -995,6 +1214,13 @@ void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flag
 	const size_t smem = poseSmemBytes(a, per_block);
 	cudaStream_t st = a->ctx->stream;
 	const bool lists = a->sample_lists;
+	if (hasIk(a)) {
+		if (G == 4) pose_palette_ik_kernel<4><<<blocks, POSE_THREADS, smem, st>>>(P);
+		else if (G == 8) pose_palette_ik_kernel<8><<<blocks, POSE_THREADS, smem, st>>>(P);
+		else if (G == 16) pose_palette_ik_kernel<16><<<blocks, POSE_THREADS, smem, st>>>(P);
+		else pose_palette_ik_kernel<32><<<blocks, POSE_THREADS, smem, st>>>(P);
+		return;
+	}
 	if (G == 4) (lists ? pose_palette_kernel<4, true> : pose_palette_kernel<4, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
 	else if (G == 8) (lists ? pose_palette_kernel<8, true> : pose_palette_kernel<8, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
 	else if (G == 16) (lists ? pose_palette_kernel<16, true> : pose_palette_kernel<16, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
@@ -1066,8 +1292,10 @@ int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, flo
 		M.n_systems = count;
 		uint32_t blocks = 0;
 		size_t smem = 0;
+		bool ik = false; // some system of the launch has IK ops: pose_palette_many_ik_kernel
 		for (uint32_t s = 0; s < count; ++s) {
 			const lb200_animation* a = run[first + s];
+			ik = ik || hasIk(a);
 			AnimSysParams& S = M.sys[s];
 			S.clips = a->d_clips; S.key_pos = a->d_key_pos; S.key_rot = a->d_key_rot; S.key_flags = a->d_key_flags;
 			S.inv_bind_pos = a->d_bind + 2 * a->bone_count; S.inv_bind_rot = a->d_bind + 3 * a->bone_count;
@@ -1083,7 +1311,13 @@ int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, flo
 			M.block_end[s] = blocks;
 			smem = std::max(smem, poseSmemBytes(a, per_block));
 		}
-		if (G == 4) pose_palette_many_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		if (ik) {
+			if (G == 4) pose_palette_many_ik_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+			else if (G == 8) pose_palette_many_ik_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+			else if (G == 16) pose_palette_many_ik_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+			else pose_palette_many_ik_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		}
+		else if (G == 4) pose_palette_many_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
 		else if (G == 8) pose_palette_many_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
 		else if (G == 16) pose_palette_many_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
 		else pose_palette_many_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);

@@ -128,6 +128,56 @@ LB_HD Rigid rmul(Rigid a, Rigid b) {
 	return r;
 }
 
+// math.cpp:395 squaredLength(Vec3): (x*x + y*y) + z*z
+LB_HD float squared_length(V3 v) { return LB_FADD(LB_FADD(LB_FMUL(v.x, v.x), LB_FMUL(v.y, v.y)), LB_FMUL(v.z, v.z)); }
+// math.cpp:392 length(Vec3): sqrtf of the same sum
+LB_HD float length(V3 v) { return LB_FSQRT(squared_length(v)); }
+
+// math.cpp:664-667 Quat::conjugated
+LB_HD Q4 conjugated(Q4 q) { return q4(q.x, q.y, q.z, -q.w); }
+
+// math.cpp:836-841 LocalRigidTransform::inverted: rot' = rot.conjugated(), pos' = rot'.rotate(-pos)
+LB_HD Rigid rinverted(Rigid a) {
+	Rigid r;
+	r.rot = conjugated(a.rot);
+	r.pos = rotate(r.rot, neg(a.pos));
+	return r;
+}
+
+// math.cpp:677-691 nlerp(Quat, Quat, float), the scalar form: dot and length summed ((x+y)+z)+w, t negated for a negative dot,
+// normalised with 1 / sqrtf
+LB_HD Q4 nlerp(Q4 q1, Q4 q2, float t) {
+	const float inv = LB_FSUB(1.0f, t);
+	const float d = LB_FADD(LB_FADD(LB_FADD(LB_FMUL(q1.x, q2.x), LB_FMUL(q1.y, q2.y)), LB_FMUL(q1.z, q2.z)), LB_FMUL(q1.w, q2.w));
+	if (d < 0) t = -t;
+	const Q4 q = q4(LB_FADD(LB_FMUL(q1.x, inv), LB_FMUL(q2.x, t)), LB_FADD(LB_FMUL(q1.y, inv), LB_FMUL(q2.y, t)),
+		LB_FADD(LB_FMUL(q1.z, inv), LB_FMUL(q2.z, t)), LB_FADD(LB_FMUL(q1.w, inv), LB_FMUL(q2.w, t)));
+	const float len2 = LB_FADD(LB_FADD(LB_FADD(LB_FMUL(q.x, q.x), LB_FMUL(q.y, q.y)), LB_FMUL(q.z, q.z)), LB_FMUL(q.w, q.w));
+	const float l = LB_FDIV(1.0f, LB_FSQRT(len2));
+	return q4(LB_FMUL(q.x, l), LB_FMUL(q.y, l), LB_FMUL(q.z, l), LB_FMUL(q.w, l));
+}
+
+// Quat(axis, PI) (math.cpp:570-578): sinf / cosf of PI * 0.5f (math.h:404) as the reference's x86 libm returns them, 1 and
+// -4.37113883e-08 (tests/golden/ik_kat.npz pins them)
+constexpr float IK_SIN_HALF_PI = 1.0f;
+constexpr float IK_COS_HALF_PI = -0x1.777a5cp-25f;
+
+// math.cpp:581-606 Quat::vec3ToVec3.  The antiparallel branch's squaredLength(n) < 0.01 compares a float with a double.
+LB_HD Q4 vec3_to_vec3(V3 v0, V3 v1) {
+	const V3 from = normalize(v0);
+	const V3 to = normalize(v1);
+	const float cos_angle = dot(from, to);
+	if (cos_angle > -1.0005f && cos_angle < -0.9995f) {
+		V3 n = v3(0, from.z, -from.y);
+		if ((double)squared_length(n) < 0.01) n = v3(from.y, -from.x, 0);
+		n = normalize(n);
+		return q4(LB_FMUL(n.x, IK_SIN_HALF_PI), LB_FMUL(n.y, IK_SIN_HALF_PI), LB_FMUL(n.z, IK_SIN_HALF_PI), IK_COS_HALF_PI);
+	}
+	const V3 half = normalize(add(from, to));
+	return q4(LB_FSUB(LB_FMUL(from.y, half.z), LB_FMUL(from.z, half.y)), LB_FSUB(LB_FMUL(from.z, half.x), LB_FMUL(from.x, half.z)),
+		LB_FSUB(LB_FMUL(from.x, half.y), LB_FMUL(from.y, half.x)), dot(from, half));
+}
+
 // Transform::compose(const LocalRigidTransform&), math.cpp:763: pos + rot.rotate(rhs.pos * scale) in fp32, added to the fp64 position;
 // rotation rot * rhs.rot.  RenderModuleImpl::updateBoneAttachment (render_module.cpp:399-403) composes the parent entity's transform with
 // bone * relative this way and keeps the attached entity's own scale.
