@@ -588,10 +588,10 @@ typedef struct {
 typedef struct { uint16_t bone_index; uint16_t pad; float value[3]; } lb200_const_translation; /* animation.h:86-90 */
 typedef struct { uint16_t bone_index; uint16_t pad; float value[4]; } lb200_const_rotation;    /* animation.h:100-104 */
 
-/* struct Animation, animation.h:158-170 (in-memory form after Animation::load, animation.cpp:397-493).  Root motion is NOT part of this struct:
- * for a clip with root-motion tracks the reference substitutes m_root_motion.pose_translations / pose_rotations for the root bone's tracks
- * (animation.cpp:33-37, 321); the library would sample the packed tracks instead, so such clips must stay on the engine's own path — the
- * engine binding (host/animation_b200.inl) leaves their animables to updateAnimable. */
+/* struct Animation, animation.h:158-170 (in-memory form after Animation::load, animation.cpp:397-493).  Root motion is not part of this
+ * struct: lb200_animation_set_root_motion gives a system's clips the flags and root-motion tracks Animation::setRootMotionBone resolved,
+ * and the system then samples those tracks as the reference does (m_root_motion.pose_translations / pose_rotations, animation.cpp:33-37,
+ * 321). */
 typedef struct {
 	float fps;
 	uint32_t frame_count;
@@ -714,6 +714,29 @@ typedef struct {
  * - The ops are copied before the call returns; the chains are resolved from the skeleton then. */
 LB200_API int lb200_animation_set_stacks(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples,
 	const uint32_t* ik_offsets, const lb200_ik* iks);
+/* Root motion of one clip, as Animation::setRootMotionBone (animation.cpp:214-270) resolved it for the skeleton's root-motion bone.
+ * 12 bytes. */
+typedef struct {
+	uint32_t flags;            /* Animation::Flags (animation.h:73-78): Y_ROOT_TRANSLATION 1, XZ_ROOT_TRANSLATION 2, ROOT_ROTATION 4 */
+	int32_t translation_track; /* index into the clip's lb200_clip.translations (the bone's first animated translation track), or -1 */
+	int32_t rotation_track;    /* index into the clip's lb200_clip.rotations, or -1 */
+} lb200_root_motion;
+/* Root motion per clip (per_clip[c] for clip c of create): afterwards every pose, palette and consumer of the system samples clip c as the
+ * reference samples an Animation on which setRootMotionBone ran once, freshly loaded, with those flags and tracks.  For every frame f of
+ * 0 .. frame_count, the tracks' values tmp (Animation::getTranslation / getRotation; a missing track gives 0 / identity) are masked by
+ * maskRootMotion (animation.cpp:97-115) to rm, rm0 is the masked value of frame 0 (0 / identity where the flags leave the translation /
+ * rotation out), and the tracks sample rm0 * rm.inverted() * tmp in place of their packed values.  A track whose part of the motion the
+ * flags leave out is replaced too, as the reference replaces it.
+ * - An entry with flags 0, or with both tracks -1, leaves the clip as create decoded it.  A later call replaces an earlier one: clips
+ *   with root motion before are decoded again from their packed tracks first, so an entry reset to flags 0 / tracks -1 samples bit for bit
+ *   as a system that never had root motion.
+ * - The tables are built on the device (one thread per clip and frame) and the call returns after they are; times, instances, layers
+ *   and lists are kept.  Only the clips' decoded keyframes change: every update runs the same kernels as without root motion.
+ * - The module's entity-transform step (animation_module.cpp:630-635, Animation::getRootMotion) is not part of this: the library keeps
+ *   no root-motion deltas.
+ * - LB200_ERR_INVALID, with nothing changed: NULL per_clip with n_clips > 0, n_clips other than the system's clip count, a track index
+ *   below -1 or at / past the clip's track count, flag bits outside ANY_ROOT_MOTION (7). */
+LB200_API int lb200_animation_set_root_motion(lb200_animation* a, uint32_t n_clips, const lb200_root_motion* per_clip);
 /* Pose::computeRelative (src/renderer/pose.cpp:136-146) of every instance's absolute pose (needs an update with LB200_PALETTE_POSE):
  * the parent-relative poses IK / ragdoll consumers start from (controller.cpp).  Kept in HBM next to the absolute ones. */
 LB200_API int lb200_animation_compute_relative(lb200_animation* a);

@@ -109,7 +109,7 @@ SYMBOLS = [
     "lb200_hierarchy_set_attachments", "lb200_hierarchy_propagate_attached", "lb200_hierarchy_get_attachment_rounds",
     "lb200_animation_create", "lb200_animation_destroy", "lb200_animation_set_instances", "lb200_animation_update", "lb200_animation_update_many", "lb200_animation_skin",
     "lb200_animation_set_launch", "lb200_animation_get_launch",
-    "lb200_animation_get_dual_quats", "lb200_animation_get_matrices", "lb200_animation_get_pose", "lb200_animation_get_times", "lb200_animation_set_layers", "lb200_animation_set_samples", "lb200_animation_set_stacks", "lb200_animation_bone_attachments", "lb200_animation_compute_relative", "lb200_animation_get_relative_pose", "lb200_animation_blend_pose",
+    "lb200_animation_get_dual_quats", "lb200_animation_get_matrices", "lb200_animation_get_pose", "lb200_animation_get_times", "lb200_animation_set_layers", "lb200_animation_set_samples", "lb200_animation_set_stacks", "lb200_animation_set_root_motion", "lb200_animation_bone_attachments", "lb200_animation_compute_relative", "lb200_animation_get_relative_pose", "lb200_animation_blend_pose",
     "lb200_animation_get_skinned", "lb200_animation_skinned_checksum", "lb200_animation_algorithmic_bytes",
 ]
 

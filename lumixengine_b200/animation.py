@@ -27,6 +27,9 @@ assert SAMPLE_DTYPE.itemsize == 16
 IK_DTYPE = np.dtype([("after", np.uint32), ("leaf_bone", np.uint32), ("bone_count", np.uint32), ("alpha", np.float32), ("target", np.float32, 3),
                      ("reserved", np.uint32)])  # lb200_ik
 assert IK_DTYPE.itemsize == 32
+ROOT_MOTION_DTYPE = np.dtype([("flags", np.uint32), ("translation_track", np.int32), ("rotation_track", np.int32)])  # lb200_root_motion
+assert ROOT_MOTION_DTYPE.itemsize == 12
+Y_ROOT_TRANSLATION, XZ_ROOT_TRANSLATION, ROOT_ROTATION = 1, 2, 4  # Animation::Flags, animation.h:73-78
 
 
 def _pack_frames(per_track_values, bits_per_track):
@@ -49,7 +52,7 @@ def _pack_frames(per_track_values, bits_per_track):
 
 class AnimationClip:
     def __init__(self, fps, frame_count, translations, const_translations, rotations, const_rotations, translation_stream, rotation_stream,
-                 translations_frame_size_bits, rotations_frame_size_bits):
+                 translations_frame_size_bits, rotations_frame_size_bits, flags=0):
         self.fps = float(np.float32(fps))
         self.frame_count = int(frame_count)
         self.translations = np.ascontiguousarray(translations, TRACK_DTYPE)
@@ -60,11 +63,19 @@ class AnimationClip:
         self.rotation_stream = np.ascontiguousarray(rotation_stream, np.uint8)
         self.translations_frame_size_bits = int(translations_frame_size_bits)
         self.rotations_frame_size_bits = int(rotations_frame_size_bits)
+        self.flags = int(flags)  # Animation::m_flags: the root-motion bits of the compiled file's header
 
     @property
     def length_ticks(self):
         # Animation::getLength(): Time::fromSeconds(m_frame_count / m_fps), animation.h:21-24,128
         return int(np.uint32(np.float32(np.float32(self.frame_count) / np.float32(self.fps)) * np.float32(ONE_SECOND)))
+
+    def rootMotionTracks(self, bone):
+        """(translation track, rotation track) of `bone` as Animation::setRootMotionBone resolves them (animation.cpp:223-237): the index of
+        the bone's first animated (non-constant) track in `translations` / `rotations`, or -1."""
+        t = np.nonzero(self.translations["bone_index"] == bone)[0]
+        r = np.nonzero(self.rotations["bone_index"] == bone)[0]
+        return (int(t[0]) if len(t) else -1, int(r[0]) if len(r) else -1)
 
     @staticmethod
     def encode(fps, positions, rotations, pos_bits=(16, 16, 16), rot_bits=(15, 15, 15), const_eps=0.0):
@@ -172,7 +183,7 @@ class AnimationClip:
         if version <= 6 or version > 7:
             raise ValueError(f"animation version {version} not supported (7 = SKELETON without an embedded path)")
         pos = 8
-        fps, frame_count, _flags = struct.unpack_from("<fII", data, pos); pos += 12
+        fps, frame_count, flags = struct.unpack_from("<fII", data, pos); pos += 12
         (n_tr,) = struct.unpack_from("<I", data, pos); pos += 4
         T, CT, t_bits = [], [], 0
         for _ in range(n_tr):
@@ -198,7 +209,7 @@ class AnimationClip:
         n = (r_bits * (frame_count + 1) + 7) // 8
         r_stream = np.zeros(n + 8, np.uint8); r_stream[:n] = np.frombuffer(data, np.uint8, min(n, len(data) - pos), pos)[:n]
         return AnimationClip(fps, frame_count, np.array(T, TRACK_DTYPE), np.array(CT, CONST_T_DTYPE), np.array(R, TRACK_DTYPE), np.array(CR, CONST_R_DTYPE),
-                             t_stream, r_stream, t_bits, r_bits)
+                             t_stream, r_stream, t_bits, r_bits, flags)
 
     def as_struct(self, struct_cls):
         """Fill a ctypes clip struct (lumix_b200 `Clip` or any struct with the same field names); keeps the arrays alive through self."""
@@ -412,6 +423,14 @@ class AnimationSystem:
         check(self.L.lb200_animation_set_stacks(self.h, C.c_uint32(len(off) - 1), ptr(off), ptr(s) if len(s) else None, ptr(ik_off),
                                                 ptr(ik) if len(ik) else None), self.ctx.h)
         self.n = len(off) - 1
+
+    def setRootMotion(self, flags, translation_track, rotation_track):
+        """Root motion per clip (lb200_animation_set_root_motion), one entry per clip of the system: Animation::Flags and the clip's
+        root-motion tracks (AnimationClip.rootMotionTracks, -1 for none).  The clips are then sampled as the reference samples them after
+        Animation::setRootMotionBone; flags 0 or both tracks -1 leave a clip as decoded."""
+        rm = np.zeros(len(np.atleast_1d(flags)), ROOT_MOTION_DTYPE)
+        rm["flags"], rm["translation_track"], rm["rotation_track"] = flags, translation_track, rotation_track
+        check(self.L.lb200_animation_set_root_motion(self.h, C.c_uint32(len(rm)), ptr(rm) if len(rm) else None), self.ctx.h)
 
     def boneAttachments(self, instance, bone, relative7, parent_transforms, original_scale3):
         """updateBoneAttachment (render_module.cpp:377-405) for a batch: world Transforms of entities attached to posed bones."""

@@ -8,6 +8,8 @@
 //   computeSkeletonDualQuats (src/renderer/pipeline.cpp:2680-2745) / computeSkinMatrices (src/renderer/model.cpp:132-137)
 //     palette[j] = toDualQuat / toMatrix ({pos[j], rot[j]} * inverse_bind[j]) written once, coalesced
 //   time advance of updateAnimable (src/animation/animation_module.cpp:458-469)
+// root_motion_tables_kernel — Animation::setRootMotionBone (src/animation/animation.cpp:214-270): the root-motion tracks' rows of the
+//   decoded keyframes replaced by pose_translations / pose_rotations (lb200_animation_set_root_motion), which the pose kernels then sample
 // skin_kernel — evaluateSkin (model.cpp:103-109): palette of each instance staged in shared memory as 3x4 rows,
 //   one thread per vertex, vertex data kept in registers across the instances of a group.
 // Clips, skeleton and mesh are shared by all instances (L2-resident); HBM traffic is the per-instance output.
@@ -223,11 +225,7 @@ __device__ __forceinline__ uint32_t shr64_lo32(unsigned long long v, uint32_t s)
 }
 __device__ __forceinline__ uint32_t mask32(uint32_t bits) { return bits >= 32u ? 0xffffffffu : ((1u << bits) - 1u); }
 
-// animation.cpp:313-316 unpackChannel: float(min + to_float_range * double(val & mask))
-__device__ __forceinline__ float unpack_channel(unsigned long long val, float mn, float range, uint32_t bits) {
-	const unsigned long long mask = (1ull << bits) - 1ull;
-	return __double2float_rn(LB_DADD((double)mn, LB_DMUL((double)range, __ull2double_rn(val & mask))));
-}
+// unpack_channel (animation.cpp:313-316) of a field known to fit 32 bits
 __device__ __forceinline__ float unpack_channel32(uint32_t field, float mn, float range) {
 	return __double2float_rn(LB_DADD((double)mn, LB_DMUL((double)range, __uint2double_rn(field))));
 }
@@ -342,6 +340,73 @@ __global__ void __launch_bounds__(256) decode_clips_kernel(const __grid_constant
 		kr[tr.bone_index] = make_float4(q.x, q.y, q.z, q.w);
 		if (frame == 0) atomicOr(reinterpret_cast<unsigned int*>(kf + (tr.bone_index & ~3u)), 2u << (8u * (tr.bone_index & 3u)));
 	}
+}
+
+// Animation::setRootMotionBone (animation.cpp:214-270) for the clips with root motion, one thread per (clip, frame): the frame's
+// pose_translations / pose_rotations entry replaces the decoded keyframe of the tracks' bones, which is what the sampler reads for those
+// tracks (animation.cpp:33-37, 321).  Runs after decode_clips_kernel has decoded the clip's rows from its packed tracks.
+struct RootMotionParams {
+	const DevClip* clips;
+	const DevTrack* tracks;
+	const uint32_t* stream;
+	const int4* root_motion;     // per clip: flags, translation track, rotation track (indices into the clip's tracks, or -1), unused
+	const uint32_t* frame_clip;  // thread -> clip
+	const uint32_t* frame_index; // thread -> frame inside the clip
+	uint32_t n;
+	uint32_t bone_count;
+	float4* key_pos; float4* key_rot;
+};
+
+constexpr uint32_t RM_Y = 1u, RM_XZ = 2u, RM_ROT = 4u; // Animation::Flags, animation.h:73-78
+
+__global__ void __launch_bounds__(128) root_motion_tables_kernel(const __grid_constant__ RootMotionParams P) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P.n) return;
+	const uint32_t c = P.frame_clip[i], frame = P.frame_index[i];
+	const DevClip clip = P.clips[c];
+	const int4 rm = P.root_motion[c];
+	const uint32_t flags = (uint32_t)rm.x;
+	const bool has_t = rm.y >= 0, has_r = rm.z >= 0;
+	Track tt = {}, rt = {};
+	if (has_t) tt = load_track(P.tracks + clip.t_off + rm.y);
+	if (has_r) rt = load_track(P.tracks + clip.r_off + rm.z);
+	// :249-251 tmp: Animation::getTranslation / getRotation (unpackChannel through double) of the tracks, 0 / identity without one
+	auto sample = [&](uint32_t f) {
+		Rigid t;
+		t.pos = has_t ? get_translation(P.stream + (clip.t_stream >> 2), clip.t_bits, f, tt) : v3(0, 0, 0);
+		t.rot = q4(0, 0, 0, 1);
+		if (has_r) {
+			const uint32_t offset = clip.r_bits * f + rt.offset_bits;
+			const unsigned long long p = load_u64_unaligned(P.stream + (clip.r_stream >> 2), offset >> 3) >> (offset & 7u);
+			t.rot = unpack_rotation_d(p, rt.min, rt.to_range, rt.bitsizes, rt.skipped_channel);
+		}
+		return t;
+	};
+	// :97-115 maskRootMotion
+	auto mask = [&](const Rigid& t) {
+		Rigid m;
+		m.pos = v3(0, 0, 0);
+		m.rot = q4(0, 0, 0, 1);
+		if (flags & RM_Y) m.pos.y = t.pos.y;
+		if (flags & RM_XZ) { m.pos.x = t.pos.x; m.pos.z = t.pos.z; }
+		if (flags & RM_ROT) {
+			m.rot.y = t.rot.y;
+			m.rot.w = t.rot.w;
+			m.rot = normalize(m.rot);
+		}
+		return m;
+	};
+	const Rigid tmp = sample(frame);
+	const Rigid rmf = mask(tmp);
+	// :254-255 rm0: the masked frame 0 where m_root_motion.translations / rotations were filled (:240-246), else 0 / identity
+	const Rigid m0 = mask(sample(0));
+	Rigid rm0;
+	rm0.pos = has_t && (flags & (RM_Y | RM_XZ)) ? m0.pos : v3(0, 0, 0);
+	rm0.rot = has_r && (flags & RM_ROT) ? m0.rot : q4(0, 0, 0, 1);
+	const Rigid out = rmul(rmul(rm0, rinverted(rmf)), tmp); // :257 rm0 * rm.inverted() * tmp
+	const size_t row = clip.key_off + (size_t)frame * ((P.bone_count + 3u) & ~3u);
+	if (has_t) P.key_pos[row + tt.bone_index] = make_float4(out.pos.x, out.pos.y, out.pos.z, 0.f);
+	if (has_r) P.key_rot[row + rt.bone_index] = make_float4(out.rot.x, out.rot.y, out.rot.z, out.rot.w);
 }
 
 constexpr int POSE_THREADS = 128;
@@ -791,6 +856,8 @@ struct lb200_animation {
 	DeviceArray<uint32_t> d_stream;
 	DeviceArray<float4> d_bind; // bind_pos[B], bind_rot[B], inv_bind_pos[B], inv_bind_rot[B]
 	DeviceArray<float4> d_key_pos, d_key_rot; DeviceArray<unsigned char> d_key_flags;
+	std::vector<DevClip> clips;                // host copy of d_clips
+	std::vector<lb200_root_motion> root_motion; // per clip, lb200_animation_set_root_motion; flags 0 or both tracks -1: none
 	DeviceArray<short> d_parents; DeviceArray<unsigned char> d_level_bones; DeviceArray<uint32_t> d_level_start;
 	int lanes_per_instance = 8;
 	// lb200_animation_set_launch (0 = environment switch, else the default) and what the last update / skin launched
@@ -824,6 +891,62 @@ int allocPosePair(lb200_ctx* ctx, DeviceArray<float>& pos, DeviceArray<float>& r
 	LB200_CUDA(ctx, p.alloc(3 * nb));
 	LB200_CUDA(ctx, r.alloc(4 * nb));
 	pos = std::move(p); rot = std::move(r);
+	return LB200_OK;
+}
+
+bool hasRootMotion(const lb200_root_motion& rm) { return rm.flags && (rm.translation_track >= 0 || rm.rotation_track >= 0); }
+
+// The decoded keyframes of the listed clips: decode_clips_kernel from the packed tracks, then root_motion_tables_kernel for those of them
+// with root motion.  Waits for both, so that the frame lists can go.
+int decodeClips(lb200_animation* a, const std::vector<uint32_t>& list) {
+	lb200_ctx* ctx = a->ctx;
+	std::vector<uint32_t> frame_clip, frame_index, rm_clip, rm_frame;
+	for (uint32_t c : list) {
+		const bool rm = hasRootMotion(a->root_motion[c]);
+		for (uint32_t f = 0; f <= a->clips[c].frame_count; ++f) {
+			frame_clip.push_back(c); frame_index.push_back(f);
+			if (rm) { rm_clip.push_back(c); rm_frame.push_back(f); }
+		}
+	}
+	if (frame_clip.empty()) return LB200_OK;
+	cudaStream_t st = ctx->stream;
+	const uint32_t B = a->bone_count;
+	DeviceArray<uint32_t> d_fc, d_fi;
+	LB200_CUDA(ctx, d_fc.alloc(frame_clip.size()));
+	LB200_CUDA(ctx, d_fi.alloc(frame_index.size()));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_fc, frame_clip.data(), sizeof(uint32_t) * frame_clip.size(), cudaMemcpyHostToDevice, st));
+	LB200_CUDA(ctx, cudaMemcpyAsync(d_fi, frame_index.data(), sizeof(uint32_t) * frame_index.size(), cudaMemcpyHostToDevice, st));
+	DeviceArray<uint32_t> d_rc, d_rf;
+	DeviceArray<int4> d_rm;
+	if (!rm_clip.empty()) {
+		std::vector<int4> rm(a->n_clips);
+		for (uint32_t c = 0; c < a->n_clips; ++c) {
+			const lb200_root_motion& r = a->root_motion[c];
+			rm[c] = make_int4((int)r.flags, r.translation_track, r.rotation_track, 0);
+		}
+		LB200_CUDA(ctx, d_rc.alloc(rm_clip.size()));
+		LB200_CUDA(ctx, d_rf.alloc(rm_frame.size()));
+		LB200_CUDA(ctx, d_rm.alloc(rm.size()));
+		LB200_CUDA(ctx, cudaMemcpyAsync(d_rc, rm_clip.data(), sizeof(uint32_t) * rm_clip.size(), cudaMemcpyHostToDevice, st));
+		LB200_CUDA(ctx, cudaMemcpyAsync(d_rf, rm_frame.data(), sizeof(uint32_t) * rm_frame.size(), cudaMemcpyHostToDevice, st));
+		LB200_CUDA(ctx, cudaMemcpyAsync(d_rm, rm.data(), sizeof(int4) * rm.size(), cudaMemcpyHostToDevice, st));
+	}
+	DecodeParams D;
+	D.clips = a->d_clips; D.tracks = a->d_tracks; D.const_t = a->d_const_t; D.const_r_value = a->d_const_r_value; D.const_r_bone = a->d_const_r_bone;
+	D.stream = a->d_stream; D.bind_pos = a->d_bind; D.bind_rot = a->d_bind + B;
+	D.key_pos = a->d_key_pos; D.key_rot = a->d_key_rot; D.key_flags = a->d_key_flags;
+	D.frame_clip = d_fc; D.frame_index = d_fi; D.bone_count = B;
+	decode_clips_kernel<<<(unsigned)frame_clip.size(), 256, 0, st>>>(D);
+	LB200_CHECK_LAUNCH(ctx);
+	if (!rm_clip.empty()) {
+		RootMotionParams R;
+		R.clips = a->d_clips; R.tracks = a->d_tracks; R.stream = a->d_stream; R.root_motion = d_rm;
+		R.frame_clip = d_rc; R.frame_index = d_rf; R.n = (uint32_t)rm_clip.size(); R.bone_count = B;
+		R.key_pos = a->d_key_pos; R.key_rot = a->d_key_rot;
+		root_motion_tables_kernel<<<(R.n + 127) / 128, 128, 0, st>>>(R);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	LB200_CUDA(ctx, cudaStreamSynchronize(st)); // before the frame lists are freed
 	return LB200_OK;
 }
 } // namespace
@@ -908,12 +1031,10 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 	}
 	// decoded keyframe tables: (frame_count + 1) frames x Bp bones per clip
 	const uint32_t Bp = (B + 3u) & ~3u;
-	std::vector<uint32_t> frame_clip, frame_index;
 	size_t key_entries = 0;
 	for (uint32_t c = 0; c < n_clips; ++c) {
 		dc[c].key_off = (uint32_t)key_entries;
 		dc[c].flag_off = c * Bp;
-		for (uint32_t f = 0; f <= dc[c].frame_count; ++f) { frame_clip.push_back(c); frame_index.push_back(f); }
 		key_entries += (size_t)(dc[c].frame_count + 1) * Bp;
 		if (key_entries > 0x7fffffffull) { lb200_set_error(ctx, "decoded clips exceed 2^31 keyframe entries"); return LB200_ERR_INVALID; }
 	}
@@ -973,19 +1094,12 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		LB200_CUDA(ctx, a->d_key_pos.alloc(key_entries, TABLE_MIN_BYTES));
 		LB200_CUDA(ctx, a->d_key_rot.alloc(key_entries, TABLE_MIN_BYTES));
 		LB200_CUDA(ctx, a->d_key_flags.alloc((size_t)n_clips * Bp, TABLE_MIN_BYTES));
-		DeviceArray<uint32_t> d_fc, d_fi;
-		LB200_CUDA(ctx, d_fc.alloc(frame_clip.size(), TABLE_MIN_BYTES));
-		LB200_CUDA(ctx, d_fi.alloc(frame_index.size(), TABLE_MIN_BYTES));
-		LB200_CUDA(ctx, cudaMemcpyAsync(d_fc, frame_clip.data(), sizeof(uint32_t) * frame_clip.size(), cudaMemcpyHostToDevice, st));
-		LB200_CUDA(ctx, cudaMemcpyAsync(d_fi, frame_index.data(), sizeof(uint32_t) * frame_index.size(), cudaMemcpyHostToDevice, st));
-		DecodeParams D;
-		D.clips = a->d_clips; D.tracks = a->d_tracks; D.const_t = a->d_const_t; D.const_r_value = a->d_const_r_value; D.const_r_bone = a->d_const_r_bone;
-		D.stream = a->d_stream; D.bind_pos = a->d_bind; D.bind_rot = a->d_bind + B;
-		D.key_pos = a->d_key_pos; D.key_rot = a->d_key_rot; D.key_flags = a->d_key_flags;
-		D.frame_clip = d_fc; D.frame_index = d_fi; D.bone_count = B;
-		decode_clips_kernel<<<(unsigned)frame_clip.size(), 256, 0, st>>>(D);
-		LB200_CHECK_LAUNCH(ctx);
-		LB200_CUDA(ctx, cudaStreamSynchronize(st)); // before d_fc / d_fi are freed
+		a->clips = dc;
+		a->root_motion.assign(n_clips, lb200_root_motion{0u, -1, -1});
+		std::vector<uint32_t> all(n_clips);
+		for (uint32_t c = 0; c < n_clips; ++c) all[c] = c;
+		const int rc = decodeClips(a.get(), all);
+		if (rc) return rc;
 	}
 	LB200_CUDA(ctx, cudaStreamSynchronize(st));
 	{
@@ -1131,6 +1245,28 @@ int lb200_animation_set_stacks(lb200_animation* a, uint32_t n_instances, const u
 
 int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const uint32_t* offsets, const lb200_sample* samples) {
 	return lb200_animation_set_stacks(a, n_instances, offsets, samples, nullptr, nullptr);
+}
+
+int lb200_animation_set_root_motion(lb200_animation* a, uint32_t n_clips, const lb200_root_motion* per_clip) {
+	if (!a || (n_clips && !per_clip)) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = a->ctx;
+	if (n_clips != a->n_clips) { lb200_set_error(ctx, "set_root_motion: %u entries for %u clips", n_clips, a->n_clips); return LB200_ERR_INVALID; }
+	for (uint32_t c = 0; c < n_clips; ++c) {
+		const lb200_root_motion& r = per_clip[c];
+		if (r.flags & ~(RM_Y | RM_XZ | RM_ROT)) { lb200_set_error(ctx, "set_root_motion: clip %u: flags 0x%x outside ANY_ROOT_MOTION", c, r.flags); return LB200_ERR_INVALID; }
+		if (r.translation_track < -1 || r.translation_track >= (int64_t)a->clips[c].n_t || r.rotation_track < -1 || r.rotation_track >= (int64_t)a->clips[c].n_r) {
+			lb200_set_error(ctx, "set_root_motion: clip %u: track %d / %d out of range", c, r.translation_track, r.rotation_track);
+			return LB200_ERR_INVALID;
+		}
+	}
+	// clips with root motion before or after: decoded again, then given their new tables
+	std::vector<uint32_t> list;
+	for (uint32_t c = 0; c < n_clips; ++c) {
+		if (hasRootMotion(a->root_motion[c]) || hasRootMotion(per_clip[c])) list.push_back(c);
+		a->root_motion[c] = per_clip[c];
+	}
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	return decodeClips(a, list);
 }
 
 } // extern "C"

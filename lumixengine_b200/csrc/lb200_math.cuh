@@ -21,6 +21,7 @@
 #define LB_DDIV(a, b) __ddiv_rn((a), (b))
 #define LB_FSQRT(a) __fsqrt_rn((a))
 #define LB_FDIV(a, b) __fdiv_rn((a), (b))
+#define LB_U64_TO_D(a) __ull2double_rn((a))
 #else
 #define LB_HD inline
 #define LB_FMUL(a, b) ((a) * (b))
@@ -32,6 +33,7 @@
 #define LB_DDIV(a, b) ((a) / (b))
 #define LB_FSQRT(a) sqrtf((a))
 #define LB_FDIV(a, b) ((a) / (b))
+#define LB_U64_TO_D(a) ((double)(a))
 #endif
 
 namespace lb {
@@ -176,6 +178,40 @@ LB_HD Q4 vec3_to_vec3(V3 v0, V3 v1) {
 	const V3 half = normalize(add(from, to));
 	return q4(LB_FSUB(LB_FMUL(from.y, half.z), LB_FMUL(from.z, half.y)), LB_FSUB(LB_FMUL(from.z, half.x), LB_FMUL(from.x, half.z)),
 		LB_FSUB(LB_FMUL(from.x, half.y), LB_FMUL(from.y, half.x)), dot(from, half));
+}
+
+// math.cpp:378-389 normalize(Quat): 1 / sqrtf of the sum ((x*x + y*y) + z*z) + w*w, then four products
+LB_HD Q4 normalize(Q4 q) {
+	const float len2 = LB_FADD(LB_FADD(LB_FADD(LB_FMUL(q.x, q.x), LB_FMUL(q.y, q.y)), LB_FMUL(q.z, q.z)), LB_FMUL(q.w, q.w));
+	const float inv_len = LB_FDIV(1.0f, LB_FSQRT(len2));
+	return q4(LB_FMUL(q.x, inv_len), LB_FMUL(q.y, inv_len), LB_FMUL(q.z, inv_len), LB_FMUL(q.w, inv_len));
+}
+
+// animation.cpp:313-316 unpackChannel: float(min + to_float_range * double(val & mask))
+LB_HD float unpack_channel(unsigned long long val, float mn, float range, uint32_t bits) {
+	const unsigned long long mask = (1ull << bits) - 1ull;
+	return (float)LB_DADD((double)mn, LB_DMUL((double)range, LB_U64_TO_D(val & mask)));
+}
+
+// animation.cpp:336-364 Animation::getRotation of one packed sample (already shifted to its first bit): the three channels through
+// unpackChannel (double), unlike the float form of AnimationSampler::getRotation (:71-77), then the smallest-three reconstruction
+LB_HD Q4 unpack_rotation_d(unsigned long long packed, const float* mn, const float* range, const uint32_t* bits, uint32_t skipped_channel) {
+	const bool is_negative = (packed & 1ull) != 0;
+	packed >>= 1;
+	V3 v;
+	v.x = unpack_channel(packed, mn[0], range[0], bits[0]);
+	packed >>= bits[0];
+	v.y = unpack_channel(packed, mn[1], range[1], bits[1]);
+	packed >>= bits[1];
+	v.z = unpack_channel(packed, mn[2], range[2], bits[2]);
+	const float rem = LB_FSUB(1.0f, dot(v, v));
+	const float skipped = LB_FMUL(LB_FSQRT(0.f > rem ? 0.f : rem), is_negative ? -1.0f : 1.0f); // maximum(0.f, x), math.h
+	switch (skipped_channel) {
+		case 0: return q4(skipped, v.x, v.y, v.z);
+		case 1: return q4(v.x, skipped, v.y, v.z);
+		case 2: return q4(v.x, v.y, skipped, v.z);
+		default: return q4(v.x, v.y, v.z, skipped);
+	}
 }
 
 // Transform::compose(const LocalRigidTransform&), math.cpp:763: pos + rot.rotate(rhs.pos * scale) in fp32, added to the fp64 position;
