@@ -764,6 +764,41 @@ LB200_API int lb200_animation_get_skinned(lb200_animation* a, uint32_t first, ui
 LB200_API int lb200_animation_skinned_checksum(lb200_animation* a, uint64_t* out);
 LB200_API uint64_t lb200_animation_algorithmic_bytes(const lb200_animation* a, uint32_t palette_flags, int skin);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Skinning palettes of the instances createSortKeys claims — PoseProcessor::push + computeSkeletonDualQuats
+ * (src/renderer/pipeline.cpp:3730-3787, 2680-2745) on the device, for the pose lists lb200_sortkeys_create_keys[_views] left in HBM.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* The entity each instance poses: entity_of_instance[i] = EntityRef::index of the ModelInstance whose Pose instance i writes, negative =
+ * none.  Host array, copied before the call returns; instances at or past n have no entity.  set_instances, set_samples and set_stacks
+ * leave the table alone.  LB200_ERR_INVALID, with nothing changed: n > max_instances, NULL entity_of_instance with n > 0, a
+ * non-negative id listed twice.  Precedent: lb200_hierarchy_set_entities. */
+LB200_API int lb200_animation_set_entities(lb200_animation* a, const int32_t* entity_of_instance, uint32_t n);
+typedef struct {
+	const float* dual_quats;  /* DualQuat per bone (r xyzw, d xyzw: 32 B), the slices of every palette the build wrote */
+	const uint32_t* offset;   /* per entity, max_entities long: first bone of its slice in dual_quats, 0xffffffff = listed, no instance */
+	const uint32_t* n_bones;  /* bones written (one word) */
+} lb200_sk_palettes;
+/* For every entity e of the pose list of the latest create_keys (views == 0), or of every view's pose list of the latest create_keys_views
+ * (views == 1), in one pass: the instance of `systems` whose entity id is e (lb200_animation_set_entities; if several are, one of them)
+ * writes its bone_count dual quaternions to_dual_quat(pose_abs[b] * inv_bind[b]) into a slice of one palette buffer, and offset[e] = the
+ * slice's first bone.  The draw stage reads the palette of a DRAW_SKINNED value's entity e at dual_quats + 8 * offset[e].
+ * - Bits: exactly what lb200_animation_update(..., LB200_PALETTE_DUAL_QUAT) writes for that instance from the same poses.
+ * - A listed entity no instance lists gets offset 0xffffffff and nothing is written: a skinned model without an animation component
+ *   keeps Model::getPose's palette, which stays on the host.  Entities not listed keep the offset they had.
+ * - Slices are disjoint and contiguous (32-byte aligned) and *n_bones is their sum; their order is not specified.  The buffer holds the
+ *   bones of every instance with an entity id, so a build cannot run out of room.
+ * - Execution: asynchronous on the context stream, no read-back; the list lengths are read on the device, clamped to the lists'
+ *   capacity.  Host work grows with the number of systems, not of instances.  One launch maps entities to instances and one builds
+ *   palettes per 64 systems (one build launch for an empty list).
+ * - Buffers are allocated or grown before anything is launched (a build that grows the palette buffer waits for the stream first); a
+ *   failed allocation returns LB200_ERR_CUDA with the earlier outputs intact.  The pointers stay valid until the next build_palettes;
+ *   a spawn that grows max_entities grows `offset` too, keeping its contents, and makes pointers handed out before it stale.
+ * - Refused, with the earlier outputs as they were: LB200_ERR_INVALID for NULL out, NULL systems with n_systems > 0, a NULL entry, a
+ *   system listed twice, a system of another context, views other than 0 / 1; LB200_ERR_STATE for a system with instances that have
+ *   entity ids but no absolute poses yet (no update with LB200_PALETTE_POSE), views == 1 before any create_keys_views and views == 0
+ *   before any create_keys. */
+LB200_API int lb200_sortkeys_build_palettes(lb200_sortkeys* sk, lb200_animation* const* systems, uint32_t n_systems, int views, lb200_sk_palettes* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -79,6 +79,11 @@ class Skeleton(C.Structure):
     _fields_ = [("bone_count", C.c_uint32), ("first_nonroot_bone_index", C.c_int32), ("parents", vp), ("bind_relative7", vp), ("inverse_bind7", vp)]
 
 
+class SkPalettes(C.Structure):
+    """lb200_sk_palettes: device pointers of the latest lb200_sortkeys_build_palettes."""
+    _fields_ = [("dual_quats", vp), ("offset", vp), ("n_bones", vp)]
+
+
 class Mesh(C.Structure):
     _fields_ = [("n_vertices", C.c_uint32), ("positions3", vp), ("weights4", vp), ("indices4", vp)]
 
@@ -102,6 +107,7 @@ SYMBOLS = [
     "lb200_sortkeys_view_outputs",
     "lb200_sortkeys_move_device", "lb200_sortkeys_end_frame", "lb200_sortkeys_prev_transforms", "lb200_sortkeys_moved_list", "lb200_sortkeys_max_entities",
     "lb200_sortkeys_spawn_instances_device", "lb200_sortkeys_spawn_decals_device", "lb200_sortkeys_clear_dirty_device", "lb200_radix_sort_device", "lb200_animation_bone_attachments_device",
+    "lb200_animation_set_entities", "lb200_sortkeys_build_palettes",
     "lb200_hierarchy_create", "lb200_hierarchy_destroy", "lb200_hierarchy_depth",
     "lb200_hierarchy_set_parents", "lb200_hierarchy_set_parents_device", "lb200_hierarchy_get_level_order", "lb200_hierarchy_set_locals", "lb200_hierarchy_set_root_globals", "lb200_hierarchy_set_subset",
     "lb200_hierarchy_propagate", "lb200_hierarchy_get_globals", "lb200_hierarchy_get_spheres", "lb200_hierarchy_refresh_spheres", "lb200_hierarchy_get_relative_matrices", "lb200_hierarchy_set_globals", "lb200_hierarchy_compute_locals", "lb200_hierarchy_get_locals", "lb200_hierarchy_algorithmic_bytes",
@@ -184,6 +190,8 @@ def lib():
     L.lb200_hierarchy_destroy.restype = None
     L.lb200_animation_destroy.restype = None
     L.lb200_animation_update_many.argtypes = [C.POINTER(vp), C.c_uint32, C.c_float, C.c_uint32]
+    L.lb200_animation_set_entities.argtypes = [vp, vp, C.c_uint32]
+    L.lb200_sortkeys_build_palettes.argtypes = [vp, C.POINTER(vp), C.c_uint32, C.c_int, C.POINTER(SkPalettes)]
     L.lb200_comm_destroy.restype = None
     L.lb200_frustum_perspective.restype = None
     L.lb200_frustum_ortho.restype = None

@@ -338,6 +338,12 @@ class AnimationSystem:
         check(self.L.lb200_animation_set_instances(self.h, ptr(c), ptr(t), C.c_uint32(len(c))), self.ctx.h)
         self.n = len(c)
 
+    def setEntities(self, ids):
+        """EntityRef::index of the model instance each instance poses (lb200_animation_set_entities): ids[i] for instance i, negative = none;
+        instances at or past len(ids) have none.  SortKeys.buildPalettes finds an entity's pose through this table."""
+        e = np.ascontiguousarray(ids, np.int32)
+        check(self.L.lb200_animation_set_entities(self.h, ptr(e) if len(e) else None, C.c_uint32(len(e))), self.ctx.h)
+
     def update(self, time_delta, palette=PALETTE_DUAL_QUAT):
         check(self.L.lb200_animation_update(self.h, C.c_float(time_delta), C.c_uint32(palette)), self.ctx.h)
 

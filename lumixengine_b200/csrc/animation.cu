@@ -880,6 +880,9 @@ struct lb200_animation {
 	DeviceArray<float> d_mesh_pos; DeviceArray<float4> d_mesh_w; DeviceArray<short> d_mesh_idx;
 	DeviceArray<float> d_skinned;
 	DeviceArray<unsigned long long> d_checksum;
+	// lb200_animation_set_entities: EntityRef::index per instance [0, n_entities) (max_instances allocated by the first call), < 0 = none
+	DeviceArray<int32_t> d_entity;
+	uint32_t n_entities = 0;
 };
 
 namespace {
@@ -1247,6 +1250,27 @@ int lb200_animation_set_samples(lb200_animation* a, uint32_t n_instances, const 
 	return lb200_animation_set_stacks(a, n_instances, offsets, samples, nullptr, nullptr);
 }
 
+int lb200_animation_set_entities(lb200_animation* a, const int32_t* entity_of_instance, uint32_t n) {
+	if (!a) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = a->ctx;
+	if (n > a->max_instances || (n && !entity_of_instance)) { lb200_set_error(ctx, "set_entities: %u ids for %u instances at most, or no array", n, a->max_instances); return LB200_ERR_INVALID; }
+	{
+		std::vector<int32_t> ids(entity_of_instance, entity_of_instance + n);
+		std::sort(ids.begin(), ids.end());
+		for (uint32_t i = 1; i < n; ++i) {
+			if (ids[i] >= 0 && ids[i] == ids[i - 1]) { lb200_set_error(ctx, "set_entities: entity %d is listed twice", ids[i]); return LB200_ERR_INVALID; }
+		}
+	}
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	if (!a->d_entity) LB200_CUDA(ctx, a->d_entity.alloc(a->max_instances));
+	if (n) {
+		LB200_CUDA(ctx, cudaMemcpyAsync(a->d_entity, entity_of_instance, sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
+		LB200_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // a build still reading the old ids, and the caller's array
+	}
+	a->n_entities = n;
+	return LB200_OK;
+}
+
 int lb200_animation_set_root_motion(lb200_animation* a, uint32_t n_clips, const lb200_root_motion* per_clip) {
 	if (!a || (n_clips && !per_clip)) return LB200_ERR_INVALID;
 	lb200_ctx* ctx = a->ctx;
@@ -1602,6 +1626,11 @@ int lb200_animation_internal_poses(const lb200_animation* a, AnimationPoses* out
 	if (!a->d_pos || !a->n_instances) return LB200_ERR_STATE;
 	*out = AnimationPoses{a->ctx, a->d_pos, a->d_rot, a->bone_count, a->n_instances};
 	return LB200_OK;
+}
+
+void lb200_animation_internal_palette_source(const lb200_animation* a, AnimationPaletteSource* out) {
+	*out = AnimationPaletteSource{a->ctx, a->d_pos, a->d_rot, a->d_bind + 2 * a->bone_count, a->d_bind + 3 * a->bone_count, a->d_entity, a->bone_count,
+		std::min(a->n_instances, a->n_entities)};
 }
 
 extern "C" {

@@ -185,6 +185,17 @@ struct AnimationPoses {
 	uint32_t bone_count, n_instances;
 };
 int lb200_animation_internal_poses(const lb200_animation* a, AnimationPoses* out);
+// animation.cu: what lb200_sortkeys_build_palettes reads of a system: its absolute poses (null before an update with LB200_PALETTE_POSE),
+// inverse bind pose (float4 pos[bone_count], rot[bone_count]) and the entity ids of instances [0, n_listed), n_listed = min(instance
+// count, ids set by lb200_animation_set_entities)
+struct AnimationPaletteSource {
+	lb200_ctx* ctx;
+	const float *pos, *rot;
+	const float4 *inv_bind_pos, *inv_bind_rot;
+	const int32_t* entity;
+	uint32_t bone_count, n_listed;
+};
+void lb200_animation_internal_palette_source(const lb200_animation* a, AnimationPaletteSource* out);
 // context.cu: *out = blocks of a cooperative kernel that can be co-resident on the context's device (threads per block, dynamic smem)
 int lb200_coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out);
 // radix_sort.cu: scratch for sorts of up to min(blocks, co-resident blocks) blocks; on failure `out` is left as it was

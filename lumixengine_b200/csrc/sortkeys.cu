@@ -33,6 +33,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <new>
+#include <vector>
 
 namespace {
 
@@ -564,6 +565,7 @@ struct OutputSet {
 	DeviceArray<uint32_t> group_count, group_offset, group_cursor; // [n_views][max_groups]; a launch's views lie n_groups apart
 	DeviceArray<uint64_t> group_renderables; DeviceArray<float4> instance_data; // [n_views][cap_recs], [n_views][3 cap_recs]
 	DeviceArray<uint32_t> pose_list, dirty_list;                   // [n_views][max_entities]
+	uint32_t pose_cap = 0; // capacity of each pose list when create_keys last filled the set (0 = never): entries past it were not written
 };
 } // namespace
 
@@ -603,6 +605,11 @@ struct lb200_sortkeys {
 	int launch_blocks = 0, launch_prefetch = -1;
 	uint32_t last_grid = 0, last_prefetch = 0;
 	int last_in_smem = 0;
+	// lb200_sortkeys_build_palettes, allocated by the first build: the palette buffer (2 float4 = one dual quaternion per bone, grown to the
+	// largest capacity a build needed), per entity the first bone of its slice, the bones written; per entity the instance that lists it,
+	// as (number << 32 | stamp of the build that wrote it); the build sequence the stamps come from
+	DeviceArray<float4> d_pal_dq; DeviceArray<uint32_t> d_pal_offset, d_pal_n_bones; DeviceArray<unsigned long long> d_pal_map;
+	uint32_t pal_seq = 0;
 };
 
 namespace {
@@ -728,6 +735,7 @@ int launch_keys(lb200_sortkeys* sk, const CullViewsResult& cv, const lb200_sk_vi
 	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)create_keys_kernel, dim3(grid), dim3(SK_THREADS), args, smem, s));
 	LB200_CHECK_LAUNCH(ctx);
 	sk->last_grid = grid; sk->last_in_smem = in_smem ? 1 : 0; sk->last_prefetch = EP.prefetch_ahead;
+	out.pose_cap = EP.cap_pose;
 	if (sort) {
 		lb200_range r2("radixSort"); // pipeline.cpp:4101
 		for (uint32_t v = 0; v < n; ++v) { // every view: whether a view has keys is known on the device only
@@ -815,6 +823,7 @@ int grow_entities(lb200_sortkeys* sk, size_t cap, DeviceArray<uint32_t>& stamp) 
 	LB200_CHECK_LAUNCH(ctx);
 	DeviceArray<uint32_t> decal_sort_key, stash, moved_list, pose_frame, plain_pose, plain_dirty, views_pose, views_dirty;
 	DeviceArray<uint8_t> decal_layer; DeviceArray<float4> stash4; DeviceArray<lb200_transform> prev; DeviceArray<float> lod;
+	DeviceArray<uint32_t> pal_offset; DeviceArray<unsigned long long> pal_map;
 	int rc = grow_copy(ctx, sk->d_decal_sort_key, old, cap, 0, decal_sort_key);
 	if (!rc) rc = grow_copy(ctx, sk->d_decal_layer, old, cap, 0, decal_layer);
 	if (rc) return rc;
@@ -829,6 +838,12 @@ int grow_entities(lb200_sortkeys* sk, size_t cap, DeviceArray<uint32_t>& stamp) 
 		LB200_CUDA(ctx, lod.alloc(cap));
 		LB200_CUDA(ctx, pose_frame.alloc(cap));
 	}
+	if (sk->d_pal_offset) { // the palette offsets keep theirs; the entity -> instance map is rebuilt by every build and starts stamp-free
+		rc = grow_copy(ctx, sk->d_pal_offset, old, cap, 0xff, pal_offset);
+		if (rc) return rc;
+		LB200_CUDA(ctx, pal_map.alloc(cap));
+		LB200_CUDA(ctx, cudaMemsetAsync(pal_map, 0, sizeof(unsigned long long) * cap, s));
+	}
 	rc = grow_lists(ctx, sk->plain.pose_list, sk->plain.n_views, (uint32_t)old, (uint32_t)cap, plain_pose);
 	if (!rc) rc = grow_lists(ctx, sk->plain.dirty_list, sk->plain.n_views, (uint32_t)old, (uint32_t)cap, plain_dirty);
 	if (!rc && sk->views.n_views) {
@@ -842,6 +857,7 @@ int grow_entities(lb200_sortkeys* sk, size_t cap, DeviceArray<uint32_t>& stamp) 
 	sk->d_stash = std::move(stash); sk->d_stash4 = std::move(stash4); sk->d_stamp = std::move(stamp);
 	if (sk->d_moved_list) { sk->d_moved_list = std::move(moved_list); sk->d_prev = std::move(prev); }
 	if (sk->d_lod) { sk->d_lod = std::move(lod); sk->d_pose_frame = std::move(pose_frame); }
+	if (sk->d_pal_offset) { sk->d_pal_offset = std::move(pal_offset); sk->d_pal_map = std::move(pal_map); }
 	sk->plain.pose_list = std::move(plain_pose); sk->plain.dirty_list = std::move(plain_dirty);
 	if (sk->views.n_views) { sk->views.pose_list = std::move(views_pose); sk->views.dirty_list = std::move(views_dirty); }
 	sk->max_entities = (uint32_t)cap;
@@ -893,6 +909,114 @@ int spawn_check(lb200_sortkeys* sk, const int32_t* entities, uint32_t n, uint32_
 	const int rc = spawn_result(sk, what, reasons, max_entity);
 	if (rc) return rc;
 	return grow_entities(sk, stamps, grown_stamp);
+}
+
+// ---- PoseProcessor::push + computeSkeletonDualQuats (pipeline.cpp:3730-3787, 2680-2745) for the pose lists create_keys left ----
+// Every build numbers the instances of its systems that have entity ids 0, 1, ... in system order and maps each entity to the number of
+// the instance that lists it (pal_map_kernel: one 64-bit exchange per instance, stamped with the build).  pal_build_kernel then walks the
+// pose lists: the first listing of a mapped entity claims the map entry (stamp -> stamp + 1) and writes the instance's palette into a
+// slice of the build's buffer; a listing of an unmapped entity writes PAL_NONE.  Stale entries carry an older stamp: nothing is cleared.
+constexpr uint32_t PAL_MAX_SYSTEMS = 64; // systems per launch (parameter block of ~3.6 KB); longer lists run as consecutive launches
+constexpr int PAL_THREADS = 256;
+constexpr uint32_t PAL_LANES = 8;        // lanes per listed entity, the bones strided over them
+constexpr uint32_t PAL_NONE = 0xffffffffu;
+
+struct PalSystem {
+	const float* pos; const float4* rot;                // absolute poses, instance-major (what LB200_PALETTE_POSE fills)
+	const float4* inv_bind_pos; const float4* inv_bind_rot;
+	const int32_t* entity;                              // entity id of instances [0, n)
+	uint32_t bone_count, n, base, pad;                  // instance i has number base + i
+};
+struct PalParams {
+	PalSystem sys[PAL_MAX_SYSTEMS];
+	uint32_t n_systems, first, end; // the launch's systems own numbers [first, end)
+	uint32_t stamp;                 // even; an entry this build claimed holds stamp + 1
+	const uint32_t* list[SK_MAX_VIEWS]; const uint32_t* count[SK_MAX_VIEWS]; // the pose lists and their counts (device)
+	uint32_t n_lists, cap_pose, max_entities;
+	uint32_t write_none;            // the first launch of a build: listed entities without an instance get PAL_NONE
+	unsigned long long* map; uint32_t* offset; float4* dq; uint32_t* n_bones;
+};
+
+// blockIdx.y = system of the launch, its instances grid-strided over blockIdx.x
+__global__ void __launch_bounds__(PAL_THREADS) pal_map_kernel(const __grid_constant__ PalParams P) {
+	const PalSystem& S = P.sys[blockIdx.y];
+	for (uint32_t i = blockIdx.x * PAL_THREADS + threadIdx.x; i < S.n; i += gridDim.x * PAL_THREADS) {
+		const int32_t e = S.entity[i];
+		if (e >= 0 && (uint32_t)e < P.max_entities) atomicExch(P.map + e, ((unsigned long long)(S.base + i) << 32) | P.stamp);
+	}
+}
+
+// PAL_LANES lanes per listed entity, the lists of every view as one index space, grid-strided a warp (32 / PAL_LANES entities) at a time.
+// The arithmetic is the pose kernel's palette epilogue: the same rmul + to_dual_quat of the same inputs, so the bits are the same.
+__global__ void __launch_bounds__(PAL_THREADS) pal_build_kernel(const __grid_constant__ PalParams P) {
+	constexpr uint32_t PER_WARP = 32 / PAL_LANES;
+	__shared__ uint32_t s_end[SK_MAX_VIEWS]; // inclusive prefix of the clamped list lengths
+	if (threadIdx.x == 0) {
+		uint32_t total = 0;
+		for (uint32_t v = 0; v < P.n_lists; ++v) { total += min(__ldcg(P.count[v]), P.cap_pose); s_end[v] = total; }
+	}
+	__syncthreads();
+	const uint32_t total = s_end[P.n_lists - 1];
+	const uint32_t lane = threadIdx.x & 31u, sub = lane % PAL_LANES, leader = lane - sub;
+	const uint32_t warps = gridDim.x * (PAL_THREADS / 32);
+	for (uint32_t at = (blockIdx.x * (PAL_THREADS / 32) + threadIdx.x / 32) * PER_WARP; at < total; at += warps * PER_WARP) { // warp-uniform
+		const uint32_t k = at + lane / PAL_LANES;
+		uint32_t e = 0, g = 0, s = 0, bones = 0;
+		if (sub == 0 && k < total) {
+			uint32_t v = 0;
+			while (k >= s_end[v]) ++v;
+			e = __ldcg(P.list[v] + (k - (v ? s_end[v - 1] : 0u)));
+			const unsigned long long w = __ldcg(P.map + e);
+			const uint32_t stamp = (uint32_t)w;
+			g = (uint32_t)(w >> 32);
+			if (stamp == P.stamp) {
+				if (g >= P.first && g < P.end && atomicCAS(P.map + e, w, w + 1) == w) { // the entity's first listing builds it
+					uint32_t lo = 0, hi = P.n_systems - 1; // the last system whose numbers start at or below g
+					while (lo < hi) {
+						const uint32_t mid = (lo + hi + 1) >> 1;
+						if (P.sys[mid].base <= g) lo = mid;
+						else hi = mid - 1;
+					}
+					s = lo;
+					bones = P.sys[s].bone_count;
+				}
+			}
+			else if (stamp != P.stamp + 1 && P.write_none) P.offset[e] = PAL_NONE; // no instance of the build lists e
+		}
+		// the warp's slices with one atomic: inclusive scan of the bones its leaders build
+		uint32_t incl = bones;
+#pragma unroll
+		for (int d = 1; d < 32; d <<= 1) {
+			const uint32_t y = __shfl_up_sync(0xffffffffu, incl, d);
+			if (lane >= (uint32_t)d) incl += y;
+		}
+		uint32_t base = 0;
+		if (lane == 31 && incl) base = atomicAdd(P.n_bones, incl);
+		base = __shfl_sync(0xffffffffu, base, 31);
+		const uint32_t first = __shfl_sync(0xffffffffu, base + incl - bones, leader);
+		e = __shfl_sync(0xffffffffu, e, leader);
+		g = __shfl_sync(0xffffffffu, g, leader);
+		s = __shfl_sync(0xffffffffu, s, leader);
+		bones = __shfl_sync(0xffffffffu, bones, leader);
+		if (!bones) continue;
+		const PalSystem& S = P.sys[s];
+		if (sub == 0) P.offset[e] = first;
+		const size_t src = (size_t)(g - S.base) * bones;
+		float4* out = P.dq + 2 * (size_t)first;
+		for (uint32_t b = sub; b < bones; b += PAL_LANES) {
+			const float* p = S.pos + 3 * (src + b);
+			const float4 r = __ldg(S.rot + src + b);
+			const float4 ip = __ldg(S.inv_bind_pos + b), ir = __ldg(S.inv_bind_rot + b);
+			Rigid pose, inv;
+			pose.pos = v3(__ldg(p), __ldg(p + 1), __ldg(p + 2));
+			pose.rot = q4(r.x, r.y, r.z, r.w);
+			inv.pos = v3(ip.x, ip.y, ip.z);
+			inv.rot = q4(ir.x, ir.y, ir.z, ir.w);
+			const DualQ dq = to_dual_quat(rmul(pose, inv));
+			out[2 * b] = make_float4(dq.r.x, dq.r.y, dq.r.z, dq.r.w);
+			out[2 * b + 1] = make_float4(dq.d.x, dq.d.y, dq.d.z, dq.d.w);
+		}
+	}
 }
 
 } // namespace
@@ -1231,6 +1355,110 @@ int lb200_sortkeys_clear_dirty_device(lb200_sortkeys* sk, const int32_t* dev_ent
 	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
 	clear_dirty_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(sk->d_ent, sk->max_entities, dev_entities, n);
 	LB200_CHECK_LAUNCH(ctx);
+	return LB200_OK;
+}
+
+
+int lb200_sortkeys_build_palettes(lb200_sortkeys* sk, lb200_animation* const* systems, uint32_t n_systems, int views, lb200_sk_palettes* out) {
+	if (!sk) return LB200_ERR_INVALID;
+	lb200_ctx* ctx = sk->ctx;
+	lb200_range range("PoseProcessor"); // pipeline.cpp:3730
+	if (!out || (n_systems && !systems) || (views != 0 && views != 1)) { lb200_set_error(ctx, "build_palettes: no outputs, no system array or views %d not 0 / 1", views); return LB200_ERR_INVALID; }
+	std::vector<AnimationPaletteSource> src(n_systems);
+	for (uint32_t k = 0; k < n_systems; ++k) {
+		if (!systems[k]) { lb200_set_error(ctx, "build_palettes: system %u is NULL", k); return LB200_ERR_INVALID; }
+		lb200_animation_internal_palette_source(systems[k], &src[k]);
+		if (src[k].ctx != ctx) { lb200_set_error(ctx, "build_palettes: system %u belongs to another context", k); return LB200_ERR_INVALID; }
+	}
+	{
+		std::vector<const lb200_animation*> sorted(systems, systems + n_systems);
+		std::sort(sorted.begin(), sorted.end());
+		if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) { lb200_set_error(ctx, "build_palettes: a system is listed twice"); return LB200_ERR_INVALID; }
+	}
+	uint64_t cap = 0; // bones of every instance with an entity id: each feeds one slice at most
+	for (uint32_t k = 0; k < n_systems; ++k) {
+		if (src[k].n_listed && !src[k].pos) { lb200_set_error(ctx, "build_palettes: system %u has no absolute poses (update with LB200_PALETTE_POSE)", k); return LB200_ERR_STATE; }
+		cap += (uint64_t)src[k].n_listed * src[k].bone_count;
+	}
+	const OutputSet& set = views ? sk->views : sk->plain;
+	const uint32_t n_lists = views ? sk->views_n : 1u;
+	if (!n_lists || !set.pose_cap) { lb200_set_error(ctx, "build_palettes needs a preceding %s", views ? "create_keys_views" : "create_keys"); return LB200_ERR_STATE; }
+	if (cap >= PAL_NONE) { lb200_set_error(ctx, "build_palettes: %llu bones do not fit 32-bit offsets", (unsigned long long)cap); return LB200_ERR_INVALID; }
+	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
+	cudaStream_t st = ctx->stream;
+	// every buffer before anything is launched or replaced
+	const size_t E = sk->max_entities;
+	DeviceArray<uint32_t> offset, n_bones; DeviceArray<unsigned long long> map; DeviceArray<float4> dq;
+	if (!sk->d_pal_offset) {
+		LB200_CUDA(ctx, offset.alloc(E));
+		LB200_CUDA(ctx, n_bones.alloc(1));
+		LB200_CUDA(ctx, map.alloc(E));
+	}
+	const size_t have = sk->d_pal_dq.size() / 2;
+	if (!sk->d_pal_dq || have < cap) LB200_CUDA(ctx, dq.alloc(2 * grownCapacity(have, 4096, (size_t)cap)));
+	if (offset) {
+		LB200_CUDA(ctx, cudaMemsetAsync(offset, 0xff, sizeof(uint32_t) * E, st));
+		LB200_CUDA(ctx, cudaMemsetAsync(map, 0, sizeof(unsigned long long) * E, st));
+		sk->d_pal_offset = std::move(offset); sk->d_pal_n_bones = std::move(n_bones); sk->d_pal_map = std::move(map);
+	}
+	if (dq) {
+		if (sk->d_pal_dq) LB200_CUDA(ctx, cudaStreamSynchronize(st)); // nothing enqueued still writes or reads the old buffer
+		sk->d_pal_dq = std::move(dq);
+	}
+	if (++sk->pal_seq == 0x80000000u) { // the stamps would wrap: no entry may hold the new one already
+		LB200_CUDA(ctx, cudaMemsetAsync(sk->d_pal_map, 0, sizeof(unsigned long long) * E, st));
+		sk->pal_seq = 1;
+	}
+	LB200_CUDA(ctx, cudaMemsetAsync(sk->d_pal_n_bones, 0, sizeof(uint32_t), st));
+	PalParams P = {};
+	P.stamp = 2 * sk->pal_seq;
+	P.n_lists = n_lists; P.cap_pose = set.pose_cap; P.max_entities = sk->max_entities;
+	for (uint32_t v = 0; v < n_lists; ++v) {
+		P.list[v] = set.pose_list + (size_t)v * sk->max_entities;
+		P.count[v] = set.counts + (size_t)v * CNT_WORDS + CNT_POSE;
+	}
+	P.map = sk->d_pal_map; P.offset = sk->d_pal_offset; P.dq = sk->d_pal_dq; P.n_bones = sk->d_pal_n_bones;
+	// the launches' systems, numbered in list order; the map of every launch goes in before the first build reads it
+	const uint32_t n_launches = std::max(1u, (n_systems + PAL_MAX_SYSTEMS - 1) / PAL_MAX_SYSTEMS);
+	uint32_t number = 0;
+	std::vector<uint32_t> first_number(n_launches + 1, 0);
+	for (uint32_t l = 0; l < n_launches; ++l) {
+		first_number[l] = number;
+		for (uint32_t k = l * PAL_MAX_SYSTEMS; k < std::min(n_systems, (l + 1) * PAL_MAX_SYSTEMS); ++k) number += src[k].n_listed;
+	}
+	first_number[n_launches] = number;
+	auto fill = [&](uint32_t l) {
+		P.n_systems = 0;
+		uint32_t base = first_number[l], most = 0;
+		for (uint32_t k = l * PAL_MAX_SYSTEMS; k < std::min(n_systems, (l + 1) * PAL_MAX_SYSTEMS); ++k) {
+			const AnimationPaletteSource& a = src[k];
+			PalSystem& S = P.sys[P.n_systems++];
+			S.pos = a.pos; S.rot = reinterpret_cast<const float4*>(a.rot); S.inv_bind_pos = a.inv_bind_pos; S.inv_bind_rot = a.inv_bind_rot; S.entity = a.entity;
+			S.bone_count = a.bone_count; S.n = a.n_listed; S.base = base;
+			base += a.n_listed;
+			most = std::max(most, a.n_listed);
+		}
+		P.first = first_number[l]; P.end = first_number[l + 1];
+		return most;
+	};
+	for (uint32_t l = 0; l < n_launches; ++l) {
+		const uint32_t most = fill(l);
+		if (!most) continue;
+		pal_map_kernel<<<dim3(std::min(256u, (most + PAL_THREADS - 1) / PAL_THREADS), P.n_systems), PAL_THREADS, 0, st>>>(P);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	const uint64_t listed = (uint64_t)n_lists * set.pose_cap; // the lists' capacity: the counts stay on the device
+	const uint32_t per_block = PAL_THREADS / PAL_LANES;
+	const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->sm_count * 8, (listed + per_block - 1) / per_block));
+	for (uint32_t l = 0; l < n_launches; ++l) {
+		fill(l);
+		P.write_none = l == 0;
+		pal_build_kernel<<<grid, PAL_THREADS, 0, st>>>(P);
+		LB200_CHECK_LAUNCH(ctx);
+	}
+	out->dual_quats = reinterpret_cast<const float*>(sk->d_pal_dq.get());
+	out->offset = sk->d_pal_offset;
+	out->n_bones = sk->d_pal_n_bones;
 	return LB200_OK;
 }
 

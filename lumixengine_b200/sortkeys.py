@@ -171,6 +171,27 @@ class SortKeys:
             return np.zeros(self.max_entities, TRANSFORM_DTYPE)
         return self.ctx.copy_to_host(p.value, self.max_entities, TRANSFORM_DTYPE)
 
+    def buildPalettes(self, systems, views=False):
+        """PoseProcessor + computeSkeletonDualQuats for the pose list of the latest createSortKeys (views=False) or every view's pose list of
+        the latest createSortKeysViews (views=True), from the absolute poses of `systems` (AnimationSystem, entity ids from setEntities;
+        entries may be None, which the call refuses).  Asynchronous: nothing is read back.  -> the device pointers (SkPalettes)."""
+        systems = list(systems)
+        arr = (vp * max(len(systems), 1))(*[None if a is None else a.h for a in systems])
+        out = _lib.SkPalettes()
+        self._err(self.L.lb200_sortkeys_build_palettes(self.h, arr, C.c_uint32(len(systems)), C.c_int(1 if views else 0), C.byref(out)))
+        self._palettes = out
+        return out
+
+    def readPalettes(self):
+        """Host copies of what the latest buildPalettes left: offset per entity (u32, 0xffffffff = listed without an instance), n_bones and
+        the dual quaternions of the written bones (f32[n_bones, 8]); entity e's palette is dual_quats[offset[e]:offset[e] + its bone count]."""
+        o = self._palettes
+        cp = self.ctx.copy_to_host
+        n_bones = int(cp(o.n_bones, 1, np.uint32)[0])
+        offset = cp(o.offset, self.max_entities, np.uint32)
+        dq = cp(o.dual_quats, 8 * n_bones, np.float32).reshape(n_bones, 8)
+        return dict(offset=offset, n_bones=n_bones, dual_quats=dq)
+
     def read(self, res):
         """Host copies of everything the last createSortKeys left in HBM."""
         o = SkOutputs()
