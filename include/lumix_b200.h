@@ -628,6 +628,12 @@ typedef struct {
 #define LB200_PALETTE_MATRIX 2u     /* 64 B/bone, model.cpp:132-137 */
 #define LB200_PALETTE_POSE 4u       /* absolute pose write-back (pos 12 B + rot 16 B per bone) for lockPose consumers */
 
+/* Refused with LB200_ERR_INVALID, before anything is allocated: a clip with fps <= 0, no frames or 2^24 frames or more (the sampler's
+ * clamp to frame_count - 0.00001f is computed in fp32 and could pass the last frame from there on); one whose length
+ * (frame_count / fps * 32768, in fp32 as Time::fromSeconds) is below one tick or 2^32 ticks or more; a track whose bone is outside the
+ * skeleton (constant tracks too), with a channel of 64 bits or more (bitsizes[k] >= 64; unpackChannel's mask is undefined there, the importer writes at most 31),
+ * or a rotation track with skipped_channel > 3; a bit stream shorter than (frame_count + 1) frames; clips whose decoded keyframe tables,
+ * (frame_count + 2) rows of bone_count rounded up to 4 entries each, pass 2^31 entries together. */
 LB200_API int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* skeleton, const lb200_clip* clips, uint32_t n_clips,
 	const lb200_mesh* mesh /* may be NULL */, uint32_t max_instances, lb200_animation** out);
 LB200_API void lb200_animation_destroy(lb200_animation* a);

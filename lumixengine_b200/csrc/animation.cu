@@ -33,7 +33,7 @@ struct DevClip {
 	uint32_t t_off, ct_off, r_off, cr_off; // first element in the flat track arrays
 	uint32_t t_stream, r_stream;      // byte offsets of the bit streams inside the stream blob (multiples of 4)
 	uint32_t length_ticks;            // Animation::getLength(), animation.h:128
-	uint32_t key_off;                 // first float4 of this clip's decoded keyframes: [(frame_count + 1)][Bp] entries
+	uint32_t key_off;                 // first float4 of this clip's decoded keyframes: [key_rows(frame_count)][Bp] entries
 	uint32_t flag_off, pad[3];        // first byte of this clip's per-bone track flags
 };
 
@@ -218,9 +218,11 @@ __device__ __forceinline__ unsigned long long load_u64_unaligned(const uint32_t*
 	return ((unsigned long long)hi << 32) | lo;
 }
 
-// low 32 bits of (v >> s), 0 <= s < 64
+// low 32 bits of (v >> s), 0 <= s <= 64: the third channel of a (32, 32, 32) track starts at bit 64, past the 8 bytes the reference
+// reads, and comes out 0 as the reference's two shifts by 32 leave it
 __device__ __forceinline__ uint32_t shr64_lo32(unsigned long long v, uint32_t s) {
 	const uint32_t lo = (uint32_t)v, hi = (uint32_t)(v >> 32);
+	if (s >= 64u) return 0u;
 	return s >= 32u ? (hi >> (s - 32u)) : __funnelshift_r(lo, hi, s);
 }
 __device__ __forceinline__ uint32_t mask32(uint32_t bits) { return bits >= 32u ? 0xffffffffu : ((1u << bits) - 1u); }
@@ -283,9 +285,18 @@ __device__ __forceinline__ Q4 unpack_rotation(unsigned long long packed, const T
 	}
 }
 
-// Unpack every frame of every clip once (clips are shared by all instances): block = (clip, frame), threads over bones / tracks.
+// Unpack every frame of every clip once (clips are shared by all instances): block = (clip, row), threads over bones / tracks.
 // Same arithmetic as the per-sample path of the reference: Animation::getTranslation (animation.cpp:318-334, unpackChannel through
 // double) and the smallest-three reconstruction of AnimationSampler::getRotation (animation.cpp:51-77).
+//
+// A clip has key_rows(frame_count) = frame_count + 2 rows: frames 0 .. frame_count, then frame_count again.  The pose kernels read
+// rows sample_idx and sample_idx + 1, and sample_idx reaches frame_count itself at or past the clip's end once frame_count - 0.00001f
+// rounds to frame_count (frame_count >= 257).  There t == 0, so lerp / simd_nlerp of the last frame with its copy give the last frame,
+// which is what the reference's read of frame_count + 1 yields for any finite value; the extra row keeps that read inside the clip's own
+// table.  That holds because frame_count is at most MAX_FRAME_COUNT (lb200_animation_create refuses more): exact in fp32, so the clamp
+// never rounds above it and sample_idx <= frame_count.  From 2^24 on an odd frame_count can round up and sample_idx pass frame_count + 1.
+inline size_t key_rows(uint32_t frame_count) { return (size_t)frame_count + 2u; }
+constexpr uint32_t MAX_FRAME_COUNT = (1u << 24) - 1u;
 struct DecodeParams {
 	const DevClip* clips;
 	const DevTrack* tracks;
@@ -300,10 +311,11 @@ struct DecodeParams {
 
 __global__ void __launch_bounds__(256) decode_clips_kernel(const __grid_constant__ DecodeParams P) {
 	const uint32_t B = P.bone_count, Bp = (B + 3u) & ~3u;
-	const uint32_t c = P.frame_clip[blockIdx.x], frame = P.frame_index[blockIdx.x];
+	const uint32_t c = P.frame_clip[blockIdx.x], row = P.frame_index[blockIdx.x];
 	const DevClip clip = P.clips[c];
-	float4* kp = P.key_pos + clip.key_off + (size_t)frame * Bp;
-	float4* kr = P.key_rot + clip.key_off + (size_t)frame * Bp;
+	const uint32_t frame = row < clip.frame_count ? row : clip.frame_count; // the last row repeats the last frame
+	float4* kp = P.key_pos + clip.key_off + (size_t)row * Bp;
+	float4* kr = P.key_rot + clip.key_off + (size_t)row * Bp;
 	unsigned char* kf = P.key_flags + clip.flag_off;
 	for (uint32_t b = threadIdx.x; b < Bp; b += blockDim.x) {
 		kp[b] = b < B ? P.bind_pos[b] : make_float4(0, 0, 0, 0);
@@ -362,8 +374,9 @@ constexpr uint32_t RM_Y = 1u, RM_XZ = 2u, RM_ROT = 4u; // Animation::Flags, anim
 __global__ void __launch_bounds__(128) root_motion_tables_kernel(const __grid_constant__ RootMotionParams P) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= P.n) return;
-	const uint32_t c = P.frame_clip[i], frame = P.frame_index[i];
+	const uint32_t c = P.frame_clip[i], row = P.frame_index[i];
 	const DevClip clip = P.clips[c];
+	const uint32_t frame = row < clip.frame_count ? row : clip.frame_count; // key_rows: the last row repeats the last frame
 	const int4 rm = P.root_motion[c];
 	const uint32_t flags = (uint32_t)rm.x;
 	const bool has_t = rm.y >= 0, has_r = rm.z >= 0;
@@ -404,9 +417,9 @@ __global__ void __launch_bounds__(128) root_motion_tables_kernel(const __grid_co
 	rm0.pos = has_t && (flags & (RM_Y | RM_XZ)) ? m0.pos : v3(0, 0, 0);
 	rm0.rot = has_r && (flags & RM_ROT) ? m0.rot : q4(0, 0, 0, 1);
 	const Rigid out = rmul(rmul(rm0, rinverted(rmf)), tmp); // :257 rm0 * rm.inverted() * tmp
-	const size_t row = clip.key_off + (size_t)frame * ((P.bone_count + 3u) & ~3u);
-	if (has_t) P.key_pos[row + tt.bone_index] = make_float4(out.pos.x, out.pos.y, out.pos.z, 0.f);
-	if (has_r) P.key_rot[row + rt.bone_index] = make_float4(out.rot.x, out.rot.y, out.rot.z, out.rot.w);
+	const size_t at = clip.key_off + (size_t)row * ((P.bone_count + 3u) & ~3u);
+	if (has_t) P.key_pos[at + tt.bone_index] = make_float4(out.pos.x, out.pos.y, out.pos.z, 0.f);
+	if (has_r) P.key_rot[at + rt.bone_index] = make_float4(out.rot.x, out.rot.y, out.rot.z, out.rot.w);
 }
 
 constexpr int POSE_THREADS = 128;
@@ -906,7 +919,7 @@ int decodeClips(lb200_animation* a, const std::vector<uint32_t>& list) {
 	std::vector<uint32_t> frame_clip, frame_index, rm_clip, rm_frame;
 	for (uint32_t c : list) {
 		const bool rm = hasRootMotion(a->root_motion[c]);
-		for (uint32_t f = 0; f <= a->clips[c].frame_count; ++f) {
+		for (uint32_t f = 0; f < key_rows(a->clips[c].frame_count); ++f) {
 			frame_clip.push_back(c); frame_index.push_back(f);
 			if (rm) { rm_clip.push_back(c); rm_frame.push_back(f); }
 		}
@@ -998,6 +1011,8 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		d.bits = (uint32_t)t.bitsizes[0] | ((uint32_t)t.bitsizes[1] << 8) | ((uint32_t)t.bitsizes[2] << 16) | ((uint32_t)t.skipped_channel << 24);
 		return d;
 	};
+	// unpackChannel's mask (1 << bitsize) - 1 is defined below 64 bits only (animation.cpp:315); the importer writes at most 31
+	auto channelsFit = [](const lb200_track& t) { return t.bitsizes[0] < 64 && t.bitsizes[1] < 64 && t.bitsizes[2] < 64; };
 	std::vector<uint32_t> stream;
 	auto appendStream = [&](const uint8_t* data, uint32_t bytes) -> uint32_t {
 		const uint32_t off = (uint32_t)stream.size() * 4;
@@ -1011,34 +1026,46 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		const lb200_clip& s = clips[c];
 		DevClip& d = dc[c];
 		if (!(s.fps > 0) || !s.frame_count) { lb200_set_error(ctx, "clip %u: fps/frame_count invalid", c); return LB200_ERR_INVALID; }
+		// the sampler's clamp frame_count - 0.00001f stays at or below frame_count only while frame_count is exact in fp32 (key_rows)
+		if (s.frame_count > MAX_FRAME_COUNT) { lb200_set_error(ctx, "clip %u: %u frames, 2^24 or more", c, s.frame_count); return LB200_ERR_INVALID; }
 		d.fps = s.fps; d.frame_count = s.frame_count;
 		d.t_bits = s.translations_frame_size_bits; d.r_bits = s.rotations_frame_size_bits;
 		d.n_t = s.n_translations; d.n_ct = s.n_const_translations; d.n_r = s.n_rotations; d.n_cr = s.n_const_rotations;
 		d.t_off = (uint32_t)tracks.size();
-		for (uint32_t i = 0; i < s.n_translations; ++i) { if (s.translations[i].bone_index >= B) return LB200_ERR_INVALID; tracks.push_back(packTrack(s.translations[i])); }
+		for (uint32_t i = 0; i < s.n_translations; ++i) {
+			if (s.translations[i].bone_index >= B || !channelsFit(s.translations[i])) { lb200_set_error(ctx, "clip %u: translation track %u: bone or channel width out of range", c, i); return LB200_ERR_INVALID; }
+			tracks.push_back(packTrack(s.translations[i]));
+		}
 		d.r_off = (uint32_t)tracks.size();
-		for (uint32_t i = 0; i < s.n_rotations; ++i) { if (s.rotations[i].bone_index >= B || s.rotations[i].skipped_channel > 3) return LB200_ERR_INVALID; tracks.push_back(packTrack(s.rotations[i])); }
+		for (uint32_t i = 0; i < s.n_rotations; ++i) {
+			if (s.rotations[i].bone_index >= B || s.rotations[i].skipped_channel > 3 || !channelsFit(s.rotations[i])) { lb200_set_error(ctx, "clip %u: rotation track %u: bone, skipped channel or channel width out of range", c, i); return LB200_ERR_INVALID; }
+			tracks.push_back(packTrack(s.rotations[i]));
+		}
 		d.ct_off = (uint32_t)cts.size();
-		for (uint32_t i = 0; i < s.n_const_translations; ++i) { if (s.const_translations[i].bone_index >= B) return LB200_ERR_INVALID; const lb200_const_translation& c0 = s.const_translations[i]; cts.push_back(make_float4(c0.value[0], c0.value[1], c0.value[2], __builtin_bit_cast(float, (uint32_t)c0.bone_index))); }
+		for (uint32_t i = 0; i < s.n_const_translations; ++i) { if (s.const_translations[i].bone_index >= B) { lb200_set_error(ctx, "clip %u: constant translation %u: bone %u out of range", c, i, (unsigned)s.const_translations[i].bone_index); return LB200_ERR_INVALID; } const lb200_const_translation& c0 = s.const_translations[i]; cts.push_back(make_float4(c0.value[0], c0.value[1], c0.value[2], __builtin_bit_cast(float, (uint32_t)c0.bone_index))); }
 		d.cr_off = (uint32_t)cr_values.size();
-		for (uint32_t i = 0; i < s.n_const_rotations; ++i) { if (s.const_rotations[i].bone_index >= B) return LB200_ERR_INVALID; const lb200_const_rotation& c0 = s.const_rotations[i]; cr_values.push_back(make_float4(c0.value[0], c0.value[1], c0.value[2], c0.value[3])); cr_bones.push_back(c0.bone_index); }
+		for (uint32_t i = 0; i < s.n_const_rotations; ++i) { if (s.const_rotations[i].bone_index >= B) { lb200_set_error(ctx, "clip %u: constant rotation %u: bone %u out of range", c, i, (unsigned)s.const_rotations[i].bone_index); return LB200_ERR_INVALID; } const lb200_const_rotation& c0 = s.const_rotations[i]; cr_values.push_back(make_float4(c0.value[0], c0.value[1], c0.value[2], c0.value[3])); cr_bones.push_back(c0.bone_index); }
 		// streams must hold (frame_count + 1) frames + the loader's 8-byte tail (animation.cpp:439)
-		const uint64_t need_t = s.n_translations ? ((uint64_t)d.t_bits * (s.frame_count + 1) + 7) / 8 : 0;
-		const uint64_t need_r = s.n_rotations ? ((uint64_t)d.r_bits * (s.frame_count + 1) + 7) / 8 : 0;
+		const uint64_t need_t = s.n_translations ? ((uint64_t)d.t_bits * ((uint64_t)s.frame_count + 1) + 7) / 8 : 0;
+		const uint64_t need_r = s.n_rotations ? ((uint64_t)d.r_bits * ((uint64_t)s.frame_count + 1) + 7) / 8 : 0;
 		if (s.translation_stream_bytes < need_t || s.rotation_stream_bytes < need_r) { lb200_set_error(ctx, "clip %u: bit stream shorter than (frame_count+1) frames", c); return LB200_ERR_INVALID; }
 		d.t_stream = appendStream(s.translation_stream, s.translation_stream_bytes);
 		d.r_stream = appendStream(s.rotation_stream, s.rotation_stream_bytes);
-		d.length_ticks = (uint32_t)(((float)s.frame_count / s.fps) * (float)(1 << 15)); // Time::fromSeconds(m_frame_count / m_fps)
-		if (!d.length_ticks) return LB200_ERR_INVALID;
+		// Time::fromSeconds(m_frame_count / m_fps): a length that does not fit the u32 ticks would be an undefined conversion
+		const float length = ((float)s.frame_count / s.fps) * (float)(1 << 15);
+		if (!(length < 4294967296.0f)) { lb200_set_error(ctx, "clip %u: %u frames at %g fps last 2^32 ticks or more", c, s.frame_count, (double)s.fps); return LB200_ERR_INVALID; }
+		d.length_ticks = (uint32_t)length;
+		if (!d.length_ticks) { lb200_set_error(ctx, "clip %u: %u frames at %g fps last less than one tick", c, s.frame_count, (double)s.fps); return LB200_ERR_INVALID; }
 		d.pad[0] = d.pad[1] = d.pad[2] = 0;
 	}
-	// decoded keyframe tables: (frame_count + 1) frames x Bp bones per clip
+	// decoded keyframe tables: key_rows (frame_count + 2) rows x Bp bones per clip, refused before anything is allocated when their
+	// offsets would not fit the u32 key_off
 	const uint32_t Bp = (B + 3u) & ~3u;
 	size_t key_entries = 0;
 	for (uint32_t c = 0; c < n_clips; ++c) {
 		dc[c].key_off = (uint32_t)key_entries;
 		dc[c].flag_off = c * Bp;
-		key_entries += (size_t)(dc[c].frame_count + 1) * Bp;
+		key_entries += (size_t)key_rows(dc[c].frame_count) * Bp;
 		if (key_entries > 0x7fffffffull) { lb200_set_error(ctx, "decoded clips exceed 2^31 keyframe entries"); return LB200_ERR_INVALID; }
 	}
 

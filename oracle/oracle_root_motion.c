@@ -221,12 +221,17 @@ int oracle_stack_rm(const OracleSkeleton* sk, const OracleClip* clips, uint32_t 
 	for (uint32_t c = 0; c < n_clips; ++c) {
 		rc[c].clip = &clips[c];
 		rc[c].t = rc[c].r = -1;
-		rc[c].pose_t = (OVec3*)malloc(sizeof(OVec3) * (clips[c].frame_count + 1));
-		rc[c].pose_r = (OQuat*)malloc(sizeof(OQuat) * (clips[c].frame_count + 1));
+		/* one entry past the reference's frame_count + 1: a sample at or past the end of a clip of 257 frames or more reads entry
+		 * frame_count + 1 at t == 0 (see sample()); it repeats the last entry, whose value that lerp / nlerp then gives */
+		const size_t n = (size_t)clips[c].frame_count + 2;
+		rc[c].pose_t = (OVec3*)malloc(sizeof(OVec3) * n);
+		rc[c].pose_r = (OQuat*)malloc(sizeof(OQuat) * n);
 		if (!rc[c].pose_t || !rc[c].pose_r) { status = -1; continue; }
 		if (rm && oracle_root_motion_tables(&clips[c], rm[c].flags, rm[c].translation_track, rm[c].rotation_track, rc[c].pose_t, rc[c].pose_r)) {
 			rc[c].t = rm[c].translation_track; /* :268-269 */
 			rc[c].r = rm[c].rotation_track;
+			rc[c].pose_t[n - 1] = rc[c].pose_t[n - 2];
+			rc[c].pose_r[n - 1] = rc[c].pose_r[n - 2];
 		}
 	}
 	if (status == 0) {
