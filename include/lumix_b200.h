@@ -805,6 +805,114 @@ typedef struct {
  *   before any create_keys. */
 LB200_API int lb200_sortkeys_build_palettes(lb200_sortkeys* sk, lb200_animation* const* systems, uint32_t n_systems, int views, lb200_sk_palettes* out);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Light clusters — PipelineImpl::fillClusters (src/renderer/pipeline.cpp:3327-3684) on the device, for the LOCAL_LIGHT ids a view's
+ * cull left in HBM: the per-light ClusterLight records, the shadow-atlas candidates of AtlasSorter (:2375-2401) and the binning of
+ * lights, environment probes and reflection probes into the 64 px x 64 px x 16 froxel grid (clusters[] and map[]).  The shadow atlas
+ * (allocation, bakeShadow, shadow matrices) and the probe arrays stay with the host, as in the reference.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct lb200_clusters lb200_clusters;
+#define LB200_LIGHT_CAST_SHADOWS 1u   /* PointLight::CAST_SHADOWS */
+#define LB200_LIGHT_DYNAMIC 2u        /* PointLight::DYNAMIC */
+#define LB200_CLUSTERS_LAST_CULL 0xffffffffu /* lb200_cluster_view.view: the last cull of the culling system (a lone cull, or select_view's) */
+#define LB200_CLUSTERS_MAX_ATLAS 64   /* ShadowAtlas::inv_map (pipeline.cpp:267) and AtlasSorter::lights (:2399) hold 64 entries */
+/* The PointLight fields fillClusters reads (render_module.h:156-171).  32 bytes. */
+typedef struct {
+	float color[3];
+	float intensity;
+	float fov;
+	float attenuation_param;
+	float range;
+	uint32_t flags;               /* LB200_LIGHT_* */
+} lb200_point_light;
+/* fillClusters' ClusterLight (:3331-3341), 64 bytes; padding is written as zero. */
+typedef struct {
+	float pos[3];                 /* Vec3(transform.pos - cam_pos): the difference in fp64, each component then rounded to fp32 */
+	float radius;                 /* range */
+	float rot[4];                 /* the transform's rotation */
+	float color[3];               /* color * intensity */
+	float attenuation_param;
+	uint32_t atlas_idx;           /* shadow-atlas entry, 0xffffffff = none */
+	float fov;
+	float padding[2];
+} lb200_cluster_light;
+/* Cluster (:3343-3348): the cluster's entries are map[offset, offset + lights_count + env_probes_count + refl_probes_count), lights
+ * first, then environment probes, then reflection probes, each kind in increasing index. */
+typedef struct { uint32_t offset, lights_count, env_probes_count, refl_probes_count; } lb200_cluster;
+/* ClusterEnvProbe (:3350-3359, 208 bytes) and ClusterReflProbe (:3361-3367, 48 bytes) as the host fills and sorts them (:3497-3538).
+ * The binning reads pos and outer_range / half_extents. */
+typedef struct {
+	float pos[3]; float pad0;
+	float rot[4];
+	float inner_range[3]; float pad1;
+	float outer_range[3]; float pad2;
+	float sh_coefs[9][4];
+} lb200_cluster_env_probe;
+typedef struct {
+	float pos[3]; uint32_t layer;
+	float rot[4];
+	float half_extents[3]; float pad1;
+} lb200_cluster_refl_probe;
+typedef struct {
+	double cam_pos[3];            /* CameraParams::pos */
+	uint32_t w, h;                /* the pipeline's viewport in pixels, 1 .. 4096 each */
+	uint32_t view;                /* view k of the latest lb200_culling_cull_views, or LB200_CLUSTERS_LAST_CULL */
+	uint32_t pad;
+	lb200_shifted_frustum frustum; /* CameraParams::frustum: the planes are built from its points */
+} lb200_cluster_view;
+/* One entry of AtlasSorter::lights. */
+typedef struct { uint32_t light_idx; float priority; int32_t entity; } lb200_shadow_candidate;
+typedef struct {
+	uint32_t n_lights;            /* visible lights = entries of lights[] and light_entities[] */
+	uint32_t n_clusters;          /* size[0] * size[1] * size[2] */
+	uint32_t n_map;               /* entries of map[] */
+	uint32_t size[3];             /* ((w + 63) / 64, (h + 63) / 64, 16) */
+	uint32_t n_shadow;            /* AtlasSorter::count */
+	lb200_shadow_candidate shadow[LB200_CLUSTERS_MAX_ATLAS];
+	uint32_t n_uncast;            /* visible lights without CAST_SHADOWS whose entity has an atlas entry, in light order (:3405-3407) */
+	int32_t uncast[LB200_CLUSTERS_MAX_ATLAS]; /* their entities */
+} lb200_cluster_result;
+typedef struct {                  /* device pointers, valid until the next lb200_clusters_fill */
+	const lb200_cluster_light* lights;  /* n_lights */
+	const lb200_cluster* clusters;      /* n_clusters */
+	const int32_t* map;                 /* n_map */
+	const int32_t* light_entities;      /* n_lights: the entity of light i, in the order of the cull's LOCAL_LIGHT segment */
+} lb200_cluster_outputs;
+/* Per-entity tables for entity ids [0, max_entities): point lights start as all zero, atlas entries as none. */
+LB200_API int lb200_clusters_create(lb200_ctx* ctx, uint32_t max_entities, lb200_clusters** out);
+LB200_API void lb200_clusters_destroy(lb200_clusters* cl);
+/* RenderModule's point lights: records[i] for entity entities[i].  LB200_ERR_INVALID, nothing changed: NULL arrays with n > 0, an entity
+ * outside [0, max_entities) or listed twice. */
+LB200_API int lb200_clusters_set_point_lights(lb200_clusters* cl, const int32_t* entities, const lb200_point_light* records, uint32_t n);
+/* ShadowAtlas::map: entity entities[i] gets entry atlas_idx[i], -1 removes its entry, in list order.  LB200_ERR_INVALID, nothing changed:
+ * NULL arrays with n > 0, an entity outside [0, max_entities), an index outside -1 .. 63, more than LB200_CLUSTERS_MAX_ATLAS entities
+ * with an entry afterwards. */
+LB200_API int lb200_clusters_set_atlas(lb200_clusters* cl, const int32_t* entities, const int32_t* atlas_idx, uint32_t n);
+/* fillClusters up to the host's atlas step, for the LOCAL_LIGHT segment of the chosen cull of cs, on the context stream:
+ *  - lights[i] and light_entities[i] for the i-th id of the segment, transforms from sk's entity records (set_transforms[_device],
+ *    move_device and spawns keep them current);
+ *  - result->shadow: the list AtlasSorter::push leaves after the CAST_SHADOWS lights are pushed in light order with
+ *    computeShadowPriority (:3322-3325), ties and NaN priorities included; result->uncast: what :3405-3407 removes from the atlas;
+ *  - the planes of :3468-3495 (built on the host in fp32, as the reference builds them), range() per axis (:3540-3561) for every light
+ *    (radius = range), env probe (length(outer_range)) and refl probe (length(half_extents)), and clusters[] / map[] exactly as the
+ *    count, offset and scatter passes of :3628-3666 leave them.
+ * Byte for byte the reference's output for the light order of the cull; for a fixed light order every run gives the same bytes.
+ * Kernels: four launches whatever the number of lights (four more when map[] grows).  The call reads back `result` (one copy) and
+ * waits for it.  map[] grows as needed and keeps its capacity; a growth re-runs the call's kernels once.
+ * LB200_ERR_INVALID, with the earlier outputs as they were: NULL view / result, NULL probes with a count > 0, w or h of 0 or above 4096
+ * (xplanes[65] of the reference holds 64 columns), a view index at or past the latest cull_views' count, a culling system whose entity
+ * ids reach past sk's or cl's max_entities, an sk without transforms, an sk or cs of another context.  LB200_ERR_STATE where the chosen
+ * cull does not exist. */
+LB200_API int lb200_clusters_fill(lb200_clusters* cl, lb200_sortkeys* sk, lb200_culling* cs, const lb200_cluster_view* view,
+                                  const lb200_cluster_env_probe* env_probes, uint32_t n_env, const lb200_cluster_refl_probe* refl_probes,
+                                  uint32_t n_refl, lb200_cluster_result* result);
+/* The atlas step's outcome (:3414-3437): lights[light_idx[i]].atlas_idx = atlas_idx[i] on the device, in list order (-1 is written as
+ * 0xffffffff, no entry).  Asynchronous.  LB200_ERR_STATE before a fill; LB200_ERR_INVALID (nothing written) for NULL arrays with n > 0,
+ * a light index at or past the last fill's n_lights or an atlas index outside -1 .. 63. */
+LB200_API int lb200_clusters_patch_atlas(lb200_clusters* cl, const uint32_t* light_idx, const int32_t* atlas_idx, uint32_t n);
+/* Device pointers of the last fill's lights, clusters, map and light entities (LB200_ERR_STATE before a fill). */
+LB200_API int lb200_clusters_outputs(lb200_clusters* cl, lb200_cluster_outputs* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -4,6 +4,7 @@
   hierarchy.Hierarchy        <- src/engine/world.cpp:255-282         (World::transformEntity, batched)
   animation.AnimationSystem  <- src/animation/animation_module.cpp:439-472 + pipeline.cpp:2680-2745 + model.cpp:103-137
   sortkeys.SortKeys          <- src/renderer/pipeline.cpp:3789-4144  (createSortKeys + radixSort: the consumer of the visible list)
+  clusters.Clusters          <- src/renderer/pipeline.cpp:3327-3684  (fillClusters: light records, atlas candidates, froxel binning)
 
 Everything computes in liblumix_b200.so (hand-written sm_90a CUDA behind the C-ABI of include/lumix_b200.h).
 There is no CPU fallback: importing works anywhere, creating a Context without a GPU raises NoDeviceError.
@@ -14,3 +15,4 @@ from .hierarchy import Hierarchy, TRANSFORM_DTYPE  # noqa: F401
 from .animation import AnimationClip, AnimationSystem, SkinnedMesh, Skeleton  # noqa: F401
 from .sortkeys import SortKeys, radix_sort  # noqa: F401
 from . import sortkeys  # noqa: F401
+from .clusters import Clusters  # noqa: F401

@@ -461,6 +461,7 @@ int lb200_culling_internal_last(lb200_culling* cs, const uint32_t** out_ids, con
 // the device re-binning only moves entities the host mirror added, and a device add grows the host's entity -> slot table to its largest
 // id (lb200_culling_add_many_device), so the table spans every id a cull can emit
 uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs) { return (uint32_t)cs->host.entity_to_slot.size(); }
+lb200_ctx* lb200_culling_internal_ctx(const lb200_culling* cs) { return cs->ctx; }
 
 extern "C" {
 

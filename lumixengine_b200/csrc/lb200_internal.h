@@ -177,6 +177,8 @@ struct CullViewsResult {
 int lb200_culling_internal_views(lb200_culling* cs, CullViewsResult* out);
 // culling.cu: 1 + the largest entity id ever added (0 if none): every id a cull of cs can emit is below it
 uint32_t lb200_culling_internal_entity_range(const lb200_culling* cs);
+// culling.cu: the context whose stream cs culls on (null for a host-only culling system)
+lb200_ctx* lb200_culling_internal_ctx(const lb200_culling* cs);
 // animation.cu: the absolute poses of the last update with LB200_PALETTE_POSE (pos: 3 floats, rot: 4 floats per bone, instance-major) for
 // lb200_hierarchy_propagate_attached; LB200_ERR_STATE (out untouched) while the system has none
 struct AnimationPoses {
@@ -196,6 +198,25 @@ struct AnimationPaletteSource {
 	uint32_t bone_count, n_listed;
 };
 void lb200_animation_internal_palette_source(const lb200_animation* a, AnimationPaletteSource* out);
+// sortkeys.cu: the per-entity records of createSortKeys.  One entity = one 64-byte DRAM burst.  Sector 0 is all a static mesh needs for
+// LOD selection and keys, sector 1 is what instance data adds.  clusters.cu reads the transforms of the lights from them.
+struct alignas(64) SkEntity {
+	double pos[3];        // Transform::pos
+	uint32_t model_flags; // model index (24 bits) | LB200_SK_* flags << 24
+	float lod;            // ModelInstance::lod (smoothing state, updated by the pass)
+	float rot[4];         // Transform::rot
+	float scale[3];       // Transform::scale
+	uint32_t pose_frame;  // Pose::frame (0xffffffff = never)
+};
+static_assert(sizeof(SkEntity) == 64, "one burst per entity");
+// sortkeys.cu: the records of sk (max_entities of them) and whether set_transforms[_device] or a spawn has written transforms into them
+struct SortKeysRecords {
+	lb200_ctx* ctx;
+	const SkEntity* records;
+	uint32_t max_entities;
+	bool have_transforms;
+};
+void lb200_sortkeys_internal_records(const lb200_sortkeys* sk, SortKeysRecords* out);
 // context.cu: *out = blocks of a cooperative kernel that can be co-resident on the context's device (threads per block, dynamic smem)
 int lb200_coop_grid_limit(lb200_ctx* ctx, const void* kernel, int threads, size_t smem, uint32_t* out);
 // radix_sort.cu: scratch for sorts of up to min(blocks, co-resident blocks) blocks; on failure `out` is left as it was

@@ -49,17 +49,6 @@ enum { DRAW_MESH = 0, DRAW_AUTOINSTANCED = 1, DRAW_SKINNED = 2, DRAW_DECAL = 3, 
 enum { RT_MESH = 0, RT_DECAL = 1, RT_LOCAL_LIGHT = 2, RT_CURVE_DECAL = 3 };                                // render_module.h:293-301
 enum { CNT_KEYS = 0, CNT_RECS, CNT_INST, CNT_POSE, CNT_DIRTY, CNT_WORDS = 8 };
 
-// One entity = one 64-byte DRAM burst.  Sector 0 is all a static mesh needs for LOD selection and keys, sector 1 is what instance data adds.
-struct alignas(64) SkEntity {
-	double pos[3];        // Transform::pos
-	uint32_t model_flags; // model index (24 bits) | LB200_SK_* flags << 24
-	float lod;            // ModelInstance::lod (smoothing state, updated by the pass)
-	float rot[4];         // Transform::rot
-	float scale[3];       // Transform::scale
-	uint32_t pose_frame;  // Pose::frame (0xffffffff = never)
-};
-static_assert(sizeof(SkEntity) == 64, "one burst per entity");
-
 constexpr uint32_t SK_MAX_VIEWS = LB200_CULL_MAX_VIEWS;
 // One view's lb200_sk_view without its tables (those are in EmitArgs::tables, SK_TABLE_WORDS per view)
 struct ViewScalars {
@@ -1020,6 +1009,10 @@ __global__ void __launch_bounds__(PAL_THREADS) pal_build_kernel(const __grid_con
 }
 
 } // namespace
+
+void lb200_sortkeys_internal_records(const lb200_sortkeys* sk, SortKeysRecords* out) {
+	*out = {sk->ctx, sk->d_ent, sk->max_entities, sk->have_transforms};
+}
 
 extern "C" {
 
