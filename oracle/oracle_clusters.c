@@ -1,7 +1,7 @@
 /* TEST INFRASTRUCTURE — C restatement of PipelineImpl::fillClusters (src/renderer/pipeline.cpp:3327-3684) up to the host's atlas step:
  * the ClusterLight records (:3388-3396), AtlasSorter::push (:2375-2401) with computeShadowPriority (:3322-3325), the lights the host
  * removes from the atlas (:3405-3407), the planes (:3468-3495), range() (:3540-3561) and the count / offset / map passes (:3563-3666).
- * Built by oracle/build_oracle_clusters.sh with the reference's flags (SSE2, no FMA, no fast-math); pinned to the reference's own code
+ * Built by oracle/Makefile with the reference's flags (SSE2, no FMA, no fast-math); pinned to the reference's own code
  * (oracle/_ref/libclusters_shim_b200.so) and to tests/golden/clusters_kat.npz by tests/test_clusters_cpu.py.
  *
  * Inputs are per light, in light order: entity, world position (fp64), rotation, the PointLight fields (32 bytes, lb200_point_light) and

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — CPU restatement of the IK instructions of an animator's blend stack (see oracle_math.h for the rules of use),
- * built into oracle/liboracle_ik.so by oracle/build_oracle_ik.sh on top of the pose restatement of oracle_anim.c (liboracle_lumix.so):
+ * built into oracle/liboracle_ik.so by oracle/Makefile on top of the pose restatement of oracle_anim.c (liboracle_lumix.so):
  *
  *   src/animation/controller.cpp:159-164        getAbsolutePosition (ik_absolute)
  *   src/animation/controller.cpp:166-265        evalIK (oracle_eval_ik)

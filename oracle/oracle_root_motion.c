@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — CPU restatement of root motion in the pose path (see oracle_math.h for the rules of use), built into
- * oracle/liboracle_root_motion.so by oracle/build_oracle_root_motion.sh on top of the pose restatement of oracle_anim.c
+ * oracle/liboracle_root_motion.so by oracle/Makefile on top of the pose restatement of oracle_anim.c
  * (liboracle_lumix.so) and the IK restatement of oracle_ik.c (liboracle_ik.so):
  *
  *   src/animation/animation.cpp:214-270   Animation::setRootMotionBone on a freshly loaded Animation (oracle_root_motion_tables)

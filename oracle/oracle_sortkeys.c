@@ -14,7 +14,7 @@
  * The reference runs createSortKeys on every job worker with one AutoInstancer per worker; the instancer index goes into the sort value
  * of a group (makeAutoInstancedSortValue) and the groups of one mesh are split over the workers.  This restatement is the one-worker
  * run: a single instancer (index 0), every mesh's instances in one group.  Pinned pieces (tests/golden/sortkeys_kat.npz, reference-run):
- * the packers, getLODMeshIndices and radixSort, which oracle/build_ref.sh compiles from the reference file itself. */
+ * the packers, getLODMeshIndices and radixSort, which oracle/build_ref.py compiles from the reference file itself. */
 #include "oracle.h"
 
 #include <math.h>

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — CPU restatement of the SAMPLE instructions of an animator's blend stack (see oracle_math.h for the rules of use),
- * built into oracle/liboracle_stack.so by oracle/build_oracle_stack.sh on top of the pose restatement of oracle_anim.c
+ * built into oracle/liboracle_stack.so by oracle/Makefile on top of the pose restatement of oracle_anim.c
  * (liboracle_lumix.so):
  *
  *   src/animation/animation_module.cpp:623-625  updateAnimator: Model::getRelativePose, evalBlendStack, Pose::computeAbsolute

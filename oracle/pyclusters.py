@@ -1,13 +1,15 @@
 """TEST INFRASTRUCTURE — ctypes wrappers of the fillClusters restatement (oracle/liboracle_clusters.so, oracle_clusters.c) and of the
-reference's own fillClusters code (oracle/_ref/libclusters_shim_b200.so, oracle/build_clusters_shim.sh).  Both take the same inputs, per
+reference's own fillClusters code (oracle/_ref/libclusters_shim_b200.so, oracle/build_ref.py).  Both take the same inputs, per
 light in light order, and give the same outputs."""
 import ctypes as C
 import os
 
 import numpy as np
 
+from . import pyoracle as po
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-RESTATEMENT = os.path.join(HERE, "liboracle_clusters.so")
+RESTATEMENT = os.path.join(HERE, "liboracle_clusters.so")  # made by oracle/Makefile on first use
 SHIM = os.path.join(HERE, "_ref", "libclusters_shim_b200.so")
 
 POINT_LIGHT = np.dtype([("color", np.float32, 3), ("intensity", np.float32), ("fov", np.float32), ("attenuation_param", np.float32),
@@ -24,9 +26,9 @@ _libs = {}
 
 
 def load(which="restatement"):
-    """'restatement' or 'shim'; None if that library has not been built."""
-    path = RESTATEMENT if which == "restatement" else SHIM
+    """'restatement' (made by oracle/Makefile on first use) or 'shim'; None if the shim has not been built."""
     if which not in _libs:
+        path = po.make(os.path.basename(RESTATEMENT)) if which == "restatement" else SHIM
         if not os.path.exists(path):
             return None
         L = C.CDLL(path)
@@ -45,7 +47,7 @@ def _p(a):
 
 def cluster_planes(points, w, h):
     """The restatement's xplanes[65], yplanes[65], zplanes[17] (f32[., 4])."""
-    L = C.CDLL(RESTATEMENT)
+    L = C.CDLL(po.make(os.path.basename(RESTATEMENT)))
     x, y, z = np.zeros((65, 4), np.float32), np.zeros((65, 4), np.float32), np.zeros((17, 4), np.float32)
     L.oc_cluster_planes(_p(np.ascontiguousarray(points, np.float32)), C.c_int(w), C.c_int(h), _p(x), _p(y), _p(z))
     return x, y, z

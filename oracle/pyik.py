@@ -1,25 +1,18 @@
 """ctypes wrapper of oracle/liboracle_ik.so (oracle_ik.c): the IK instructions of an animator's blend stack, with its SAMPLE instructions,
-restated on the CPU.  Types and helpers are pyoracle's; the library is built by oracle/build_oracle_ik.sh (build() runs it)."""
+restated on the CPU.  Types and helpers are pyoracle's; oracle/Makefile builds the library (lib() runs make)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import pyoracle as po
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-IK_SO = os.path.join(HERE, "liboracle_ik.so")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        po.lib()  # liboracle_lumix.so, which the IK library links
-        if not os.path.exists(IK_SO):
-            subprocess.check_call(["bash", os.path.join(HERE, "build_oracle_ik.sh")])
-        _lib = C.CDLL(IK_SO)
+        _lib = C.CDLL(po.make("liboracle_ik.so"))
     return _lib
 
 

@@ -13,23 +13,27 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_SO = os.path.join(HERE, "liboracle_lumix.so")
 REF_SO = os.path.join(HERE, "_ref", "libref_lumix.so")
+# the reference's animation code next to the animation binding (oracle/ref/ref_root_motion_harness.cpp and the harnesses it includes)
+ANIMATION_SHIM_SO = os.path.join(HERE, "_ref", "libanimation_shim_b200.so")
 
 u8p = C.POINTER(C.c_uint8)
 vp = C.c_void_p
+_made = set()
+
+
+def make(target):
+    """Bring one restatement library of oracle/Makefile up to date, once per process; -> its path."""
+    if target not in _made:
+        subprocess.check_call(["make", "-s", "-C", HERE, target])
+        _made.add(target)
+    return os.path.join(HERE, target)
 
 
 def build(force=False):
-    """Compile the C restatement (and oracle/_ref when /root/reference is present)."""
-    if force or not os.path.exists(ORACLE_SO) or any(
-        os.path.getmtime(os.path.join(HERE, f)) > os.path.getmtime(ORACLE_SO)
-        for f in ("oracle_cull.c", "oracle_propagate.c", "oracle_anim.c", "oracle_sortkeys.c", "oracle.h", "oracle_math.h")
-    ):
-        subprocess.check_call(["make", "-s", "-C", HERE])
-    ref_root = os.environ.get("LUMIX_REFERENCE", "/root/reference")
-    if os.path.isdir(os.path.join(ref_root, "src", "core")):
-        srcs = [os.path.join(HERE, "build_ref.sh")] + [os.path.join(HERE, "ref", f) for f in ("ref_harness.cpp", "ref_stubs.cpp", "ref_sortkeys_harness.cpp")]
-        if force or not os.path.exists(REF_SO) or any(os.path.getmtime(s) > os.path.getmtime(REF_SO) for s in srcs):
-            subprocess.check_call(["bash", os.path.join(HERE, "build_ref.sh")])
+    """Compile the C restatements and, where the reference tree is, oracle/_ref (oracle/build_ref.py); each only when stale."""
+    from . import build_ref
+    subprocess.check_call(["make", "-s", "-C", HERE] + (["-B"] if force else []))
+    build_ref.build(force)
 
 
 def _ptr(a):
@@ -78,9 +82,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        if not os.path.exists(ORACLE_SO):
-            build()
-        L = C.CDLL(ORACLE_SO)
+        L = C.CDLL(make("liboracle_lumix.so"))
         L.oracle_culling_create.restype = vp
         L.oracle_culling_cull.restype = C.c_uint32
         L.oracle_culling_page_count.restype = C.c_uint32

@@ -1,17 +1,12 @@
 """ctypes wrapper of oracle/liboracle_root_motion.so (oracle_root_motion.c): Animation::setRootMotionBone and the sampling of clips whose
-root-motion tracks it replaced, restated on the CPU.  Types and helpers are pyoracle's; the library is built by
-oracle/build_oracle_root_motion.sh (build() runs it)."""
+root-motion tracks it replaced, restated on the CPU.  Types and helpers are pyoracle's; oracle/Makefile builds the
+library (lib() runs make)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import pyik
 from . import pyoracle as po
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-RM_SO = os.path.join(HERE, "liboracle_root_motion.so")
 ROOT_MOTION_DTYPE = np.dtype([("flags", np.uint32), ("translation_track", np.int32), ("rotation_track", np.int32)])  # lb200_root_motion
 _lib = None
 
@@ -19,10 +14,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        pyik.lib()  # liboracle_ik.so and liboracle_lumix.so, which the root-motion library links
-        if not os.path.exists(RM_SO):
-            subprocess.check_call(["bash", os.path.join(HERE, "build_oracle_root_motion.sh")])
-        _lib = C.CDLL(RM_SO)
+        _lib = C.CDLL(po.make("liboracle_root_motion.so"))
     return _lib
 
 

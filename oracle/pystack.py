@@ -1,25 +1,18 @@
 """ctypes wrapper of oracle/liboracle_stack.so (oracle_stack.c): the SAMPLE instructions of an animator's blend stack restated on the CPU.
-Types and helpers are pyoracle's; the library is built by oracle/build_oracle_stack.sh (build() runs it)."""
+Types and helpers are pyoracle's; oracle/Makefile builds the library (lib() runs make)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import pyoracle as po
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-STACK_SO = os.path.join(HERE, "liboracle_stack.so")
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        po.lib()  # liboracle_lumix.so, which the stack library links
-        if not os.path.exists(STACK_SO):
-            subprocess.check_call(["bash", os.path.join(HERE, "build_oracle_stack.sh")])
-        _lib = C.CDLL(STACK_SO)
+        _lib = C.CDLL(po.make("liboracle_stack.so"))
     return _lib
 
 

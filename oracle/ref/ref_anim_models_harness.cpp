@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — not product code.  The animation binding (lumixengine_b200/host/animation_b200.inl) over the animables of SEVERAL
 // real Lumix::Models at once, next to the reference's own updateAnimable body per animable: AnimablesB200 keeps one group per model and
-// poses all of them in one lb200_animation_update_many call.  Built into oracle/_ref/libanim_models_shim_b200.so by
-// oracle/build_anim_models_shim.sh, against the same overlay of the reference and the same patched animation.h as ref_anim_shim_harness.cpp,
+// poses all of them in one lb200_animation_update_many call.  Built (through ref_root_motion_harness.cpp) into
+// oracle/_ref/libanimation_shim_b200.so by oracle/build_ref.py, against the same overlay of the reference and the same patched animation.h as ref_anim_shim_harness.cpp,
 // whose stand-ins for Model / Animation construction (RawStorage, RefClip, buildAnimation ...) this file includes rather than repeats.
 #include "ref_anim_shim_harness.cpp"
 

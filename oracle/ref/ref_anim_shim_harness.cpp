@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE — not product code.  Runs the animation binding (lumixengine_b200/host/animation_b200.inl, compiled against the
-// reference's own headers with the accessors of animation_b200_decl.inl patched into a temporary copy of animation.h by oracle/build_ref.sh)
+// reference's own headers with the accessors of animation_b200_decl.inl patched into a temporary copy of animation.h by oracle/build_ref.py)
 // over REAL Lumix::Model / Lumix::Animation / Lumix::Pose objects and next to the reference's own per-animable path:
 //   side A: the body of AnimationModuleImpl::updateAnimable (animation_module.cpp:439-472) per animable — Model::getRelativePose,
 //           Animation::getRelativePose (the reference's animation.cpp), Pose::computeAbsolute (the reference's pose.cpp), the time step

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE — not product code.  The animator binding (AnimatorsB200, lumixengine_b200/host/animation_b200.inl) over real
-// Lumix::Model / Lumix::Animation / Lumix::Pose objects and scripted blend stacks, next to the reference's own evalBlendStack.  Built into
-// oracle/_ref/libanimators_shim_b200.so by oracle/build_animators_shim.sh, which cuts getPose .. evalBlendStack (controller.cpp) and the
+// Lumix::Model / Lumix::Animation / Lumix::Pose objects and scripted blend stacks, next to the reference's own evalBlendStack.  Built (through
+// ref_root_motion_harness.cpp) into oracle/_ref/libanimation_shim_b200.so by oracle/build_ref.py, which cuts getPose .. evalBlendStack (controller.cpp) and the
 // RuntimeContext constructor (nodes.cpp) out of the reference at build time into the overlay this file includes them from.
 //   ref_pose_stack:      Model::getRelativePose + evalBlendStack + Pose::computeAbsolute on one scripted stack (tests/golden/stack_kat.npz)
 //   ashim_run_animators: per frame, side A runs updateAnimator's :623-627 for every animator, side B runs AnimatorsB200::update and the

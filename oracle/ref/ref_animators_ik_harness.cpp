@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — not product code.  The animator harness (ref_animators_harness.cpp, included whole: its Model / Animation /
 // Controller stand-ins and its updateAnimator reference path) with IK instructions, over Models that have a bone map (bone i named
-// BoneNameHash::fromU64(IK_BONE_HASH + i)), so that the reference's own evalIK finds its leaf.  Built into
-// oracle/_ref/libanimators_ik_shim_b200.so by oracle/build_animators_ik_shim.sh.
+// BoneNameHash::fromU64(IK_BONE_HASH + i)), so that the reference's own evalIK finds its leaf.  Built (through
+// ref_root_motion_harness.cpp) into oracle/_ref/libanimation_shim_b200.so by oracle/build_ref.py.
 //   ref_pose_stack_ik:      Model::getRelativePose + evalBlendStack + Pose::computeAbsolute on one scripted stack of SAMPLE and IK
 //                           instructions (tests/golden/ik_kat.npz)
 //   ashim_run_animators_ik: ashim_run_animators with IK instructions and ctx.weight per animator (tests/test_animation_animators_ik_gpu.py)

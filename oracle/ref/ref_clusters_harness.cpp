@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE — runs the reference's own fillClusters code on plain inputs (oracle/build_clusters_shim.sh compiles it into
+// TEST INFRASTRUCTURE — runs the reference's own fillClusters code on plain inputs (oracle/build_ref.py compiles it into
 // oracle/_ref/libclusters_shim_b200.so).  The build cuts AtlasSorter, computeShadowPriority, the Cluster* structs, the plane construction and
 // range() + the for_each_*_pair lambdas + the count / offset / map passes out of the reference's pipeline.cpp into .inl files next to its
 // sources; this file supplies the scope those pieces expect (lights, clusters, size, frustum, the probe arrays and a frame allocator).

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE — not product code.  Drives the GPU cull THROUGH THE ENGINE'S OWN C++ INTERFACE: the reference's job system, allocators
-// and PageAllocator (compiled from /root/reference by oracle/build_ref.sh) linked with lumixengine_b200/host/culling_system_b200.cpp, which
+// and PageAllocator (compiled from /root/reference by oracle/build_ref.py) linked with lumixengine_b200/host/culling_system_b200.cpp, which
 // supplies CullingSystem::create (the single construction site is render_module.cpp:3569) and CullResult::free.  Everything below talks to
 // the abstract CullingSystem (culling_system.h:58-77) exactly as the renderer does: cull() from job-system fibers for several views at once
 // (pipeline.cpp:1036-1041), CullResult page chains from the engine's PageAllocator, CullResult::free by the caller (pipeline.cpp:1045).

@@ -6,7 +6,7 @@
 //   * overlay build of src/renderer/culling_system.cpp on src/core/job_system.cpp
 //     (SURVEY.md §8(c): 3 header/source edits + ref_stubs.cpp) — the stronger cull oracle and the
 //     "reference" CPU baseline of bench.py.
-// No reference source is copied into this repository; build_ref.sh compiles it from where it lies.
+// No reference source is copied into this repository; oracle/build_ref.py compiles it from where it lies.
 #include "core/allocator.h"
 #include "core/default_allocator.h"
 #include "core/geometry.h"

@@ -2,7 +2,7 @@
 // (src/renderer/pipeline.cpp:2680-2745: 4-wide SIMD batches through simd_math.h + the scalar tail) to pin
 // oracle_palette_dual_quats as a whole, not only its primitives.
 //
-// pipeline.cpp cannot be compiled here (DX12 renderer), so oracle/build_ref.sh cuts that one member function out of the
+// pipeline.cpp cannot be compiled here (DX12 renderer), so oracle/build_ref.py cuts that one member function out of the
 // reference file AT BUILD TIME into the temporary overlay (renderer/extracted_compute_skeleton_dual_quats.inl, deleted with
 // the overlay; never stored in this repository) and this file includes it into a holder struct.  Model / Pose are filled
 // through `#define private public` as in ref_anim_harness.cpp; only data members are read.

@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE — not product code.  Animations with root motion: the IK animator harness (ref_animators_ik_harness.cpp, included
 // whole: its Model / Animation stand-ins, bone maps, scripted stacks and reference paths) with Animation::m_root_motion constructed, every
 // track named after its bone (BoneNameHash IK_BONE_HASH + bone index, the names of the bone map) and the reference's own
-// Animation::setRootMotionBone run once on the freshly built clip.  Built into oracle/_ref/libroot_motion_shim_b200.so by
-// oracle/build_root_motion_shim.sh.
+// Animation::setRootMotionBone run once on the freshly built clip.  Built into oracle/_ref/libanimation_shim_b200.so by
+// oracle/build_ref.py, with the harnesses it includes in turn: one library for all of them.
 //   ref_rm_tables:         setRootMotionBone's pose_translations / pose_rotations and track indices (tests/golden/root_motion_kat.npz)
 //   ref_rm_pose_stack:     Model::getRelativePose + evalBlendStack + Pose::computeAbsolute on one stack of samples over such clips
 //   ref_rm_math:           the reference's normalize(Quat) and Animation::getRotation on arrays

@@ -2,7 +2,7 @@
 // floatFlip, make*SortKey / make*SortValue), its Histogram + PipelineImpl::radixSort (:4020-4144) and Model::getLODMeshIndices
 // (model.h:173-179) to pin oracle_sortkeys.c.
 //
-// pipeline.cpp cannot be compiled here (DX12 renderer), so oracle/build_ref.sh cuts those two regions out of the reference file AT BUILD
+// pipeline.cpp cannot be compiled here (DX12 renderer), so oracle/build_ref.py cuts those two regions out of the reference file AT BUILD
 // TIME into the temporary overlay (renderer/extracted_sort_key_packers.inl, renderer/extracted_radix_sort.inl; deleted with the overlay,
 // never stored in this repository) and this file includes them.
 #define private public

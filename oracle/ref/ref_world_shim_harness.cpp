@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE — not product code.  Runs the World patch (lumixengine_b200/host/world_b200.inl appended to a temporary copy of the
-// reference's own src/engine/world.cpp by oracle/build_ref.sh) inside real Lumix::World objects: two worlds get the same entities, the same
+// reference's own src/engine/world.cpp by oracle/build_ref.py) inside real Lumix::World objects: two worlds get the same entities, the same
 // hierarchy (World::setParent, world.cpp:619-701) and the same local transforms; then the same root moves go
 //   world A: World::setTransform per root — the reference recursion World::transformEntity (world.cpp:255-282)
 //   world B: World::setTransformsDeferredB200 + World::propagateHierarchyB200 — one level-order pass on the GPU through liblumix_b200.so

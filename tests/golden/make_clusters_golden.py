@@ -1,5 +1,5 @@
 """Generates tests/golden/clusters_kat.npz from the REFERENCE'S OWN fillClusters code (oracle/_ref/libclusters_shim_b200.so, built by
-oracle/build_clusters_shim.sh; entry ref_clusters_fill).  Run in the build container only:  python tests/golden/make_clusters_golden.py
+oracle/build_ref.py; entry ref_clusters_fill).  Run in the build container only:  python tests/golden/make_clusters_golden.py
 
 The inputs are the named cases of tests/test_clusters_cpu.py (CASES, case()), rebuilt there from the same seeds; per case the fixture
 holds the bytes of lights[], clusters[], map[], the AtlasSorter list and the uncast-in-atlas list."""

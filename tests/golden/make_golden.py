@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz from the REFERENCE'S OWN compiled code (oracle/_ref/libref_lumix.so, built by
-oracle/build_ref.sh from /root/reference).  Run in the build container only:  python tests/golden/make_golden.py
+oracle/build_ref.py from /root/reference).  Run in the build container only:  python tests/golden/make_golden.py
 
 The reference has no golden vectors of its own for this path (SURVEY.md F9), so these reference-run outputs are the pin:
 inputs are seeded numpy draws, outputs come from unmodified math.cpp / geometry.cpp / culling_system.cpp / pose.cpp /
@@ -286,7 +286,7 @@ def ani_kat():
 
 def sortkeys_kat():
     """The reference's own sort-key packers, Model::getLODMeshIndices and PipelineImpl::radixSort (pipeline.cpp:53-143, 4020-4144; model.h:173-179),
-    compiled from the reference file by oracle/build_ref.sh."""
+    compiled from the reference file by oracle/build_ref.py."""
     rng = np.random.default_rng(2024)
     R = po.sortkey_packers("ref")
     n = 600

@@ -1,6 +1,6 @@
 """Generates tests/golden/ik_kat.npz from the REFERENCE'S OWN evalBlendStack / evalIK (controller.cpp:159-293) and math (Quat::vec3ToVec3,
 nlerp, LocalRigidTransform::inverted, length, Quat::conjugated), cut out of the reference at build time into
-oracle/_ref/libanimators_ik_shim_b200.so (oracle/build_animators_ik_shim.sh; entries ref_pose_stack_ik, ref_ik_math).  Run in the build
+oracle/_ref/libanimation_shim_b200.so (oracle/build_ref.py; entries ref_pose_stack_ik, ref_ik_math).  Run in the build
 container only:  python tests/golden/make_ik_golden.py
 
 Each stack is the bind pose + its SAMPLE and IK instructions in order + Pose::computeAbsolute, on a Model with a bone map, for the
@@ -15,13 +15,14 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+from oracle import pyoracle as po  # noqa: E402
 from test_animation_ik_cpu import ik_kat_inputs, ik_math_inputs, run_ref_stack_ik  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
 def ik_kat():
-    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libanimators_ik_shim_b200.so"))
+    L = C.CDLL(po.ANIMATION_SHIM_SO)
     d = {}
     for name, (sk, clips, cases) in ik_kat_inputs().items():
         for k, case in enumerate(cases):

@@ -1,6 +1,6 @@
 """Generates tests/golden/root_motion_kat.npz from the REFERENCE'S OWN Animation::setRootMotionBone, Animation::getRotation, normalize(Quat)
 and, for whole poses, Model::getRelativePose + evalBlendStack + Pose::computeAbsolute over Animation objects whose root motion
-setRootMotionBone set (oracle/_ref/libroot_motion_shim_b200.so, built by oracle/build_root_motion_shim.sh; entries ref_rm_tables,
+setRootMotionBone set (oracle/_ref/libanimation_shim_b200.so, built by oracle/build_ref.py; entries ref_rm_tables,
 ref_rm_pose_stack, ref_rm_math).  Run in the build container only:  python tests/golden/make_root_motion_golden.py
 
 The inputs are root_motion_inputs (tests/test_animation_root_motion_cpu.py rebuilds them from the same seeds): per input, the tracks
@@ -15,6 +15,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+from oracle import pyoracle as po  # noqa: E402
 from test_animation_root_motion_cpu import (INPUTS, math_inputs, pose_cases, rotation_inputs, run_ref_math, run_ref_pose_stack,  # noqa: E402
                                             run_ref_tables)
 
@@ -22,7 +23,7 @@ OUT = os.path.dirname(os.path.abspath(__file__))
 
 
 def root_motion_kat():
-    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libroot_motion_shim_b200.so"))
+    L = C.CDLL(po.ANIMATION_SHIM_SO)
     d = {}
     for s_idx, (name, (sk, clips, bone, flags, tt, rt)) in enumerate(INPUTS.items()):
         tracks = np.zeros((len(clips), 2), np.int32)

@@ -1,5 +1,5 @@
 """Generates tests/golden/stack_kat.npz from the REFERENCE'S OWN getPose / evalBlendStack (controller.cpp:142-157, 267-293), cut out of
-controller.cpp at build time into oracle/_ref/libanimators_shim_b200.so (oracle/build_animators_shim.sh; entry ref_pose_stack).  Run in
+controller.cpp at build time into oracle/_ref/libanimation_shim_b200.so (oracle/build_ref.py; entry ref_pose_stack).  Run in
 the build container only:  python tests/golden/make_stack_golden.py
 
 Each stack is the bind pose + its SAMPLE instructions + Pose::computeAbsolute, on the skeletons and clips of stack_kat_inputs
@@ -21,7 +21,7 @@ OUT = os.path.dirname(os.path.abspath(__file__))
 
 
 def stack_kat():
-    L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libanimators_shim_b200.so"))
+    L = C.CDLL(po.ANIMATION_SHIM_SO)
     d = {}
     for B, (sk, clips, cases) in stack_kat_inputs().items():
         arr = (Clip * len(clips))(*[c.as_struct(Clip) for c in clips])

@@ -1,5 +1,5 @@
 """The animator binding (AnimatorsB200, host/animators_b200.inl) executed over real Model / Animation / Pose objects and scripted blend
-stacks (oracle/_ref/libanimators_shim_b200.so, built by oracle/build_animators_shim.sh where the reference tree exists; skipped elsewhere).
+stacks (oracle/_ref/libanimation_shim_b200.so, built by oracle/build_ref.py where the reference tree exists; skipped elsewhere).
 Over several frames and three models, every pose must be bit-equal to the reference's getRelativePose + evalBlendStack + computeAbsolute;
 animators with an IK instruction or a controller with bone masks must land on referencePath(); every animator gets one lock
 and one unlock per frame."""
@@ -16,7 +16,7 @@ from bitexact import assert_bits_equal
 
 pytestmark = pytest.mark.gpu
 
-SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libanimators_shim_b200.so")
+SO = po.ANIMATION_SHIM_SO
 BELOW = float(np.nextafter(np.float32(0.9999), np.float32(0)))
 
 

@@ -1,5 +1,5 @@
 """The animator binding (AnimatorsB200, host/animators_b200.inl) with IK instructions, over real Model / Animation / Pose objects whose
-Models have a bone map (oracle/_ref/libanimators_ik_shim_b200.so, entry ashim_run_animators_ik, built by oracle/build_animators_ik_shim.sh where
+Models have a bone map (oracle/_ref/libanimation_shim_b200.so, entry ashim_run_animators_ik, built by oracle/build_ref.py where
 the reference tree exists; skipped elsewhere).  Over several frames and three models, every pose must be bit-equal to the reference's
 getRelativePose + evalBlendStack + computeAbsolute; IK animators stay off referencePath() unless an IK instruction's leaf bone is
 missing, its bone count is 0 or above 32, or its chain leaves the skeleton (or the controller has bone masks); every animator gets one
@@ -18,7 +18,7 @@ from test_animation_ik_cpu import depths
 
 pytestmark = pytest.mark.gpu
 
-SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libanimators_ik_shim_b200.so")
+SO = po.ANIMATION_SHIM_SO
 
 
 @pytest.mark.skipif(not os.path.exists(SO), reason="animator harness not built (no reference tree where build() ran)")

@@ -33,8 +33,7 @@ from oracle import pystack
 
 from bitexact import assert_bits_equal
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SHIM = os.path.join(ROOT, "oracle", "_ref", "libroot_motion_shim_b200.so")
+SHIM = po.ANIMATION_SHIM_SO
 U32_MAX = 0xFFFFFFFF
 BELOW = float(np.nextafter(np.float32(0.9999), np.float32(0)))
 

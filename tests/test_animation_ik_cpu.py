@@ -22,7 +22,7 @@ from bitexact import assert_bits_equal
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "ik_kat.npz")
-SHIM = os.path.join(ROOT, "oracle", "_ref", "libanimators_ik_shim_b200.so")
+SHIM = po.ANIMATION_SHIM_SO
 BELOW_0001 = float(np.nextafter(np.float32(0.001), np.float32(0)))  # the float just below 0.001f
 ALPHAS = [0.0, BELOW_0001, 0.001, 0.5, 1.0]
 CHAIN_LENGTHS = (1, 2, 3, 8, 32)

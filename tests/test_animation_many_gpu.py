@@ -16,6 +16,7 @@ import pytest
 import lumixengine_b200 as lb
 from lumixengine_b200 import scenes
 from bitexact import assert_bits_equal
+from oracle import pyoracle as po
 
 pytestmark = pytest.mark.gpu
 
@@ -318,14 +319,14 @@ def test_consumers_after_a_batched_update(ctx):
         t.close()
 
 
-SHIM = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libanim_models_shim_b200.so")
+SHIM = po.ANIMATION_SHIM_SO
 
 
 def test_binding_over_several_models(oracle):
     """host/animation_b200.inl over the animables of three real Lumix::Models of 48, 17 and 130 bones (one group each, all posed by one
     lb200_animation_update_many) against the reference's updateAnimable body per animable, bit for bit."""
     if not os.path.exists(SHIM):
-        pytest.skip("oracle/_ref/libanim_models_shim_b200.so not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/libanimation_shim_b200.so not built (needs /root/reference at build time)")
     from lumixengine_b200 import _lib
     L = C.CDLL(SHIM)
     os.environ["LB200_ENGINE_SHIM_LOADED"] = "1"  # tests/conftest.py leaves with os._exit once the shim is loaded

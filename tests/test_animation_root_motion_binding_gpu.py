@@ -1,6 +1,6 @@
 """The engine bindings (AnimablesB200, AnimatorsB200) over real Animation objects whose root motion the reference's own
-Animation::setRootMotionBone set (oracle/_ref/libroot_motion_shim_b200.so, entries ashim_run_animables_rm / ashim_run_animators_rm, built
-by oracle/build_root_motion_shim.sh where the reference tree exists; skipped elsewhere).  Over several frames every pose (and animable
+Animation::setRootMotionBone set (oracle/_ref/libanimation_shim_b200.so, entries ashim_run_animables_rm / ashim_run_animators_rm, built
+by oracle/build_ref.py where the reference tree exists; skipped elsewhere).  Over several frames every pose (and animable
 time) must be bit-equal to the reference's updateAnimable / evalBlendStack; AnimablesB200 poses every animable itself, animators with
 root-motion clips stay off AnimatorsB200::referencePath() while bone masks and unresolvable IK instructions still go there; every entity
 gets one lock and one unlock per frame."""
@@ -19,7 +19,7 @@ from test_animation_root_motion_cpu import INPUTS, rm_clip
 
 pytestmark = pytest.mark.gpu
 
-SO = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libroot_motion_shim_b200.so")
+SO = po.ANIMATION_SHIM_SO
 needs_shim = pytest.mark.skipif(not os.path.exists(SO), reason="root-motion harness not built (no reference tree where build() ran)")
 P = po._ptr
 

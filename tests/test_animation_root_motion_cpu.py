@@ -21,7 +21,7 @@ from bitexact import assert_bits_equal
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KAT = os.path.join(ROOT, "tests", "golden", "root_motion_kat.npz")
-SHIM = os.path.join(ROOT, "oracle", "_ref", "libroot_motion_shim_b200.so")
+SHIM = po.ANIMATION_SHIM_SO
 FLAG_SETS = list(range(8))  # every subset of Y_ROOT_TRANSLATION | XZ_ROOT_TRANSLATION | ROOT_ROTATION
 KINDS = ("both", "translation", "rotation", "constant")
 

@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from lumixengine_b200 import scenes
-from oracle import pystack
+from oracle import build_ref, pystack
 from bitexact import assert_bits_equal
 from test_integration_compile import GXX, REF, ROOT, _copy_headers
 
@@ -58,18 +58,15 @@ def test_animator_binding_compiles_against_render_module():
     host/animation_b200_decl.inl as INTEGRATION.md section 3 says."""
     host = os.path.join(ROOT, "lumixengine_b200", "host")
     with tempfile.TemporaryDirectory() as tmp:
-        _copy_headers(tmp, ("core", "engine", "renderer", "animation"))
-        ah = os.path.join(tmp, "src", "animation", "animation.h")
-        text = open(ah).read()
-        anchor = "\tconst Array<TranslationTrack>& getTranslations() const { return m_translations; }"
-        assert anchor in text
-        open(ah, "w").write(text.replace(anchor, open(os.path.join(host, "animation_b200_decl.inl")).read() + anchor))
+        src = _copy_headers(tmp)
+        patched = os.path.join(tmp, "patched")
+        build_ref.patch_animation(src, patched)  # asserts the anchor of INTEGRATION.md section 3; controller.h beside the patched copy
         tu = os.path.join(tmp, "tu.cpp")
         open(tu, "w").write('#include "animation/animation.h"\n#include "animation/animation_module.h"\n#include "animation/controller.h"\n#include "core/log.h"\n'
                             '#include "core/stream.h"\n#include "renderer/model.h"\n#include "renderer/pose.h"\n#include "renderer/render_module.h"\n#include <string.h>\n'
                             '#include "animators_b200.inl"\nnamespace Lumix { template struct AnimatorsB200<RenderModule>; template struct AnimablesB200<RenderModule>; }\n')
         obj = os.path.join(tmp, "tu.o")
-        cmd = GXX + ["-I", os.path.join(tmp, "src"), "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), "-I", host, tu, "-o", obj]
+        cmd = GXX + ["-I", patched, "-I", src, "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), "-I", host, tu, "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
         syms = subprocess.run(["nm", "-C", obj], capture_output=True, text=True).stdout

@@ -6,7 +6,6 @@ The cases (shared with tests/golden/make_clusters_golden.py): random lights and 
 lb200_frustum_from_viewport, lights exactly at dist == +-r of a plane, range 0, lights behind the near plane and beyond the far plane,
 viewports of 1x1, 63, 64, 65 and 4096 px, more than 64 casters with equal priorities, and NaN priorities."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -20,8 +19,6 @@ OUTPUTS = ("lights", "clusters", "map", "shadow", "uncast")
 
 
 def restatement():
-    if not os.path.exists(pc.RESTATEMENT):
-        subprocess.check_call(["bash", os.path.join(ROOT, "oracle", "build_oracle_clusters.sh")])
     return pc.load("restatement")
 
 

@@ -1,5 +1,5 @@
 """The drop-in boundary, executed: lumixengine_b200/host/culling_system_b200.cpp linked with the reference's own job system, allocators and
-PageAllocator (oracle/_ref/libengine_shim_b200.so, built by oracle/build_ref.sh from /root/reference + this repository's shim).  The GPU is
+PageAllocator (oracle/_ref/libengine_shim_b200.so, built by oracle/build_ref.py from /root/reference + this repository's shim).  The GPU is
 driven through the engine's abstract CullingSystem (culling_system.h:58-77): CullingSystem::create(allocator, page_allocator), add / set /
 remove, cull() from job-system fibers for several views at once (pipeline.cpp:1036-1041), the CullResult page chain (one renderable
 type per 4 KB page, <= 1020 ids, pages from the engine's PageAllocator) walked and freed by the caller (pipeline.cpp:1045)."""
@@ -94,7 +94,7 @@ def _wshim(L):
 
 @pytest.mark.parametrize("n,depth,fanout,reparent", [(20_000, 6, 3, 0), (60_000, 8, 4, 1)])
 def test_world_patch_runs_inside_the_reference_world(shim, oracle, n, depth, fanout, reparent):
-    """host/world_b200.inl inside the reference's own World (world.cpp + the patch, compiled by oracle/build_ref.sh): root moves through
+    """host/world_b200.inl inside the reference's own World (world.cpp + the patch, compiled by oracle/build_ref.py): root moves through
     World::setTransformsDeferredB200 + World::propagateHierarchyB200 (GPU) against the same moves through World::setTransform — the
     reference recursion transformEntity (world.cpp:255-282) — in a second World of the same process.  Every Transform bit for bit, and the
     `transformed` delegates (world.h:139, what RenderModule::onModelInstanceMoved hangs on) fire for the same entities the same number of

@@ -2,29 +2,24 @@
 (same vtable, same types, same ownership calls) and the World patch (appended to a temporary copy of world.cpp, as INTEGRATION.md
 says a maintainer would).  Only where /root/reference is present (this container)."""
 import os
-import shutil
 import subprocess
 import tempfile
 
 import pytest
 
+from oracle import build_ref
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("LUMIX_REFERENCE", "/root/reference")
+REF = build_ref.reference()
 
 
-def _copy_headers(tmp, subs):
-    for sub in subs:
-        dst = os.path.join(tmp, "src", sub)
-        os.makedirs(dst)
-        for dirpath, _, files in os.walk(os.path.join(REF, "src", sub)):
-            rel = os.path.relpath(dirpath, os.path.join(REF, "src", sub))
-            for f in files:
-                if f.endswith((".h", ".inl")):
-                    os.makedirs(os.path.join(dst, rel), exist_ok=True)
-                    shutil.copy(os.path.join(dirpath, f), os.path.join(dst, rel, f))
-    sp = os.path.join(tmp, "src", "core", "sync.h")
-    text = open(sp).read().replace('#error "Not implemented"', "pthread_rwlock_t lock;")
-    open(sp, "w").write(text)
+def _copy_headers(tmp):
+    """The reference files of oracle/build_ref.py's overlay, copied into tmp/src, with its sync.h edit (the Linux port of the reference
+    lacks an SRWLock body, src/core/sync.h:22-24, SURVEY F8)."""
+    src = os.path.join(tmp, "src")
+    build_ref.copy_sources(REF, src)
+    build_ref.patch_sync(src)
+    return src
 
 
 GXX = ["/usr/bin/g++", "-std=c++20", "-DSTATIC_PLUGINS", "-DNDEBUG", "-fno-exceptions", "-fno-rtti", "-msse2", "-w", "-c"]
@@ -34,22 +29,12 @@ GXX = ["/usr/bin/g++", "-std=c++20", "-DSTATIC_PLUGINS", "-DNDEBUG", "-fno-excep
 def test_world_patch_compiles_inside_world_cpp():
     """host/world_b200_decl.inl goes into `struct World`, host/world_b200.inl is appended to world.cpp: the result must compile with
     the reference's own flags and define World::propagateHierarchyB200 next to the untouched World::transformEntity."""
-    host = os.path.join(ROOT, "lumixengine_b200", "host")
     with tempfile.TemporaryDirectory() as tmp:
-        _copy_headers(tmp, ("core", "engine"))
-        wh = os.path.join(tmp, "src", "engine", "world.h")
-        text = open(wh).read()
-        anchor = "private:\n\tvoid transformEntity(EntityRef entity, bool update_local);"
-        assert anchor in text, "world.h changed: INTEGRATION.md section 2 needs another anchor"
-        text = text.replace(anchor, open(os.path.join(host, "world_b200_decl.inl")).read() + anchor)
-        assert text.count("namespace Lumix {") >= 1
-        text = text.replace("namespace Lumix {", "struct lb200_ctx; // include/lumix_b200.h\nnamespace Lumix {", 1)
-        open(wh, "w").write(text)
-        wc = os.path.join(tmp, "src", "engine", "world.cpp")
-        body = open(os.path.join(REF, "src", "engine", "world.cpp")).read() + "\n" + open(os.path.join(host, "world_b200.inl")).read()
-        open(wc, "w").write(body)
+        src = _copy_headers(tmp)
+        build_ref.patch_world(src)  # asserts the anchors of INTEGRATION.md section 2
+        wc = os.path.join(src, "engine", "world.cpp")
         obj = os.path.join(tmp, "world.o")
-        cmd = GXX + ["-I", os.path.join(tmp, "src"), "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), wc, "-o", obj]
+        cmd = GXX + ["-I", src, "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), wc, "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
         syms = subprocess.run(["nm", "-C", obj], capture_output=True, text=True).stdout
@@ -64,9 +49,9 @@ def test_world_patch_compiles_inside_world_cpp():
 def test_plugin_entry_compiles_against_engine_headers():
     """host/b200_system.cpp: the ISystem + LUMIX_PLUGIN_ENTRY the engine's SystemManager loads (plugin.h:64-96), static-plugin flavour."""
     with tempfile.TemporaryDirectory() as tmp:
-        _copy_headers(tmp, ("core", "engine"))
+        src = _copy_headers(tmp)
         obj = os.path.join(tmp, "b200_system.o")
-        cmd = GXX + ["-I", os.path.join(tmp, "src"), "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"),
+        cmd = GXX + ["-I", src, "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"),
                      os.path.join(ROOT, "lumixengine_b200", "host", "b200_system.cpp"), "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
@@ -78,26 +63,11 @@ def test_plugin_entry_compiles_against_engine_headers():
 
 @pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "src", "renderer")), reason="reference tree not present")
 def test_shim_compiles_against_engine_headers():
-    # the Linux port of the reference lacks an SRWLock body (src/core/sync.h:22-24, SURVEY F8): give the preprocessor the one-line
-    # overlay build_ref.sh uses, through a shadow include dir that only holds the patched sync.h
     with tempfile.TemporaryDirectory() as tmp:
-        # headers only, copied to a temp dir so that sync.h can carry the overlay (never into this repository)
-        for sub in ("core", "engine", "renderer"):
-            dst = os.path.join(tmp, "src", sub)
-            os.makedirs(dst)
-            for dirpath, _, files in os.walk(os.path.join(REF, "src", sub)):
-                rel = os.path.relpath(dirpath, os.path.join(REF, "src", sub))
-                for f in files:
-                    if f.endswith((".h", ".inl")):
-                        os.makedirs(os.path.join(dst, rel), exist_ok=True)
-                        shutil.copy(os.path.join(dirpath, f), os.path.join(dst, rel, f))
-        sp = os.path.join(tmp, "src", "core", "sync.h")
-        text = open(sp).read().replace('#error "Not implemented"', "pthread_rwlock_t lock;")
-        open(sp, "w").write(text)
+        src = _copy_headers(tmp)  # copied to a temp dir so that sync.h can carry the overlay (never into this repository)
         obj = os.path.join(tmp, "shim.o")
-        cmd = ["/usr/bin/g++", "-std=c++20", "-DSTATIC_PLUGINS", "-DNDEBUG", "-fno-exceptions", "-fno-rtti", "-msse2", "-w", "-c",
-               "-I", os.path.join(tmp, "src"), "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"),
-               os.path.join(ROOT, "lumixengine_b200", "host", "culling_system_b200.cpp"), "-o", obj]
+        cmd = GXX + ["-I", src, "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"),
+                     os.path.join(ROOT, "lumixengine_b200", "host", "culling_system_b200.cpp"), "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
         syms = subprocess.run(["nm", "-C", obj], capture_output=True, text=True).stdout
@@ -111,18 +81,15 @@ def test_animation_binding_compiles_against_render_module():
     getModelInstanceModel), animation.h patched with host/animation_b200_decl.inl as INTEGRATION.md section 3 says."""
     host = os.path.join(ROOT, "lumixengine_b200", "host")
     with tempfile.TemporaryDirectory() as tmp:
-        _copy_headers(tmp, ("core", "engine", "renderer", "animation"))
-        ah = os.path.join(tmp, "src", "animation", "animation.h")
-        text = open(ah).read()
-        anchor = "\tconst Array<TranslationTrack>& getTranslations() const { return m_translations; }"
-        assert anchor in text, "animation.h changed: INTEGRATION.md section 3 needs another anchor"
-        open(ah, "w").write(text.replace(anchor, open(os.path.join(host, "animation_b200_decl.inl")).read() + anchor))
+        src = _copy_headers(tmp)
+        patched = os.path.join(tmp, "patched")
+        build_ref.patch_animation(src, patched)  # asserts the anchor of INTEGRATION.md section 3
         tu = os.path.join(tmp, "tu.cpp")
         open(tu, "w").write('#include "animation/animation.h"\n#include "animation/animation_module.h"\n#include "core/log.h"\n#include "renderer/model.h"\n'
                             '#include "renderer/pose.h"\n#include "renderer/render_module.h"\n#include <string.h>\n#include "animation_b200.inl"\n'
                             'namespace Lumix { template struct AnimablesB200<RenderModule>; }\n')
         obj = os.path.join(tmp, "tu.o")
-        cmd = GXX + ["-I", os.path.join(tmp, "src"), "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), "-I", host, tu, "-o", obj]
+        cmd = GXX + ["-I", patched, "-I", src, "-I", os.path.join(REF, "external"), "-I", os.path.join(ROOT, "include"), "-I", host, tu, "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
         syms = subprocess.run(["nm", "-C", obj], capture_output=True, text=True).stdout

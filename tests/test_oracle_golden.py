@@ -133,7 +133,7 @@ def test_pose_sampling_and_absolute(oracle):
             ab = np.concatenate(oracle.pose_evaluate(sk, clip, t, compute_absolute=True), axis=1)
             assert np.array_equal(bits(ab), bits(g[f"c{k}_abs"][j])), (k, t)
             # dual-quaternion palette of that pose: the reference's own PipelineImpl::computeSkeletonDualQuats (4-wide SIMD batches +
-            # scalar tail, pipeline.cpp:2680-2745), cut out of pipeline.cpp at build time by oracle/build_ref.sh
+            # scalar tail, pipeline.cpp:2680-2745), cut out of pipeline.cpp at build time by oracle/build_ref.py
             dq, mtx = oracle.palettes(sk, ab[:, :3], ab[:, 3:])
             assert np.array_equal(bits(dq), bits(g[f"c{k}_dq"][j])), (k, t)
             if j < len(g[f"c{k}_mtx"]):  # computeSkinMatrices (model.cpp:132-137), and evaluateSkin (model.cpp:103-109) on a 300-vertex mesh

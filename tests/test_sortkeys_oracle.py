@@ -1,5 +1,5 @@
 """CPU: the sort-key oracle (oracle/oracle_sortkeys.c) against vectors the reference's own code produced (tests/golden/sortkeys_kat.npz:
-packers, Model::getLODMeshIndices and PipelineImpl::radixSort cut out of pipeline.cpp / model.h by oracle/build_ref.sh), live against
+packers, Model::getLODMeshIndices and PipelineImpl::radixSort cut out of pipeline.cpp / model.h by oracle/build_ref.py), live against
 that build where it exists, and properties of the createSortKeys restatement."""
 import ctypes as C
 import os
