@@ -892,7 +892,8 @@ LB200_API int lb200_clusters_set_atlas(lb200_clusters* cl, const int32_t* entiti
  *  - lights[i] and light_entities[i] for the i-th id of the segment, transforms from sk's entity records (set_transforms[_device],
  *    move_device and spawns keep them current);
  *  - result->shadow: the list AtlasSorter::push leaves after the CAST_SHADOWS lights are pushed in light order with
- *    computeShadowPriority (:3322-3325), ties and NaN priorities included; result->uncast: what :3405-3407 removes from the atlas;
+ *    computeShadowPriority (:3322-3325), ties and NaN priorities included (a NaN fov gives the device's canonical NaN, bits
+ *    0x7fffffff, as the priority, where x86 keeps the input's payload); result->uncast: what :3405-3407 removes from the atlas;
  *  - the planes of :3468-3495 (built on the host in fp32, as the reference builds them), range() per axis (:3540-3561) for every light
  *    (radius = range), env probe (length(outer_range)) and refl probe (length(half_extents)), and clusters[] / map[] exactly as the
  *    count, offset and scatter passes of :3628-3666 leave them.
@@ -912,6 +913,13 @@ LB200_API int lb200_clusters_fill(lb200_clusters* cl, lb200_sortkeys* sk, lb200_
 LB200_API int lb200_clusters_patch_atlas(lb200_clusters* cl, const uint32_t* light_idx, const int32_t* atlas_idx, uint32_t n);
 /* Device pointers of the last fill's lights, clusters, map and light entities (LB200_ERR_STATE before a fill). */
 LB200_API int lb200_clusters_outputs(lb200_clusters* cl, lb200_cluster_outputs* out);
+/* Grid of clusters_items_kernel in later fills.  blocks: 0 = the default (one block per 256 items the cull can emit plus the probes,
+ * at most every co-resident block), -1 = every co-resident block, n > 0 = min(n, co-resident blocks); only 0 caps the grid by the work.
+ * Any other value is LB200_ERR_INVALID, with nothing changed.  Outputs do not depend on the grid.  get_launch reports the last fill: its
+ * items-kernel grid and the tiles of 256 items per block, ceil(ceil(n_items / grid) / 256) for the fill's lights and probes (both 0
+ * before the first fill). */
+LB200_API int lb200_clusters_set_launch(lb200_clusters* cl, int blocks);
+LB200_API int lb200_clusters_get_launch(lb200_clusters* cl, uint32_t* grid, uint32_t* tiles_per_block);
 
 #ifdef __cplusplus
 }

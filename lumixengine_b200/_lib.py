@@ -109,7 +109,7 @@ SYMBOLS = [
     "lb200_sortkeys_spawn_instances_device", "lb200_sortkeys_spawn_decals_device", "lb200_sortkeys_clear_dirty_device", "lb200_radix_sort_device", "lb200_animation_bone_attachments_device",
     "lb200_animation_set_entities", "lb200_sortkeys_build_palettes",
     "lb200_clusters_create", "lb200_clusters_destroy", "lb200_clusters_set_point_lights", "lb200_clusters_set_atlas", "lb200_clusters_fill",
-    "lb200_clusters_patch_atlas", "lb200_clusters_outputs",
+    "lb200_clusters_patch_atlas", "lb200_clusters_outputs", "lb200_clusters_set_launch", "lb200_clusters_get_launch",
     "lb200_hierarchy_create", "lb200_hierarchy_destroy", "lb200_hierarchy_depth",
     "lb200_hierarchy_set_parents", "lb200_hierarchy_set_parents_device", "lb200_hierarchy_get_level_order", "lb200_hierarchy_set_locals", "lb200_hierarchy_set_root_globals", "lb200_hierarchy_set_subset",
     "lb200_hierarchy_propagate", "lb200_hierarchy_get_globals", "lb200_hierarchy_get_spheres", "lb200_hierarchy_refresh_spheres", "lb200_hierarchy_get_relative_matrices", "lb200_hierarchy_set_globals", "lb200_hierarchy_compute_locals", "lb200_hierarchy_get_locals", "lb200_hierarchy_algorithmic_bytes",

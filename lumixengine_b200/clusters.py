@@ -103,6 +103,17 @@ class Clusters:
         assert len(li) == len(a)
         self._err(self.L.lb200_clusters_patch_atlas(self.h, ptr(li), ptr(a), C.c_uint32(len(li))))
 
+    def setLaunch(self, blocks=0):
+        """Grid of the items kernel in later fills (lb200_clusters_set_launch): 0 = the default rule, -1 = every co-resident block,
+        n > 0 = min(n, co-resident blocks)."""
+        self._err(self.L.lb200_clusters_set_launch(self.h, C.c_int(blocks)))
+
+    def lastLaunch(self):
+        """(items-kernel grid, tiles of 256 items per block) of the last fill; (0, 0) before the first."""
+        g, t = C.c_uint32(), C.c_uint32()
+        self._err(self.L.lb200_clusters_get_launch(self.h, C.byref(g), C.byref(t)))
+        return g.value, t.value
+
     def outputs(self):
         o = ClusterOutputs()
         self._err(self.L.lb200_clusters_outputs(self.h, C.byref(o)))

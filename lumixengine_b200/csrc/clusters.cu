@@ -526,6 +526,10 @@ struct lb200_clusters {
 	DeviceArray<GridBar> d_bar;
 	RadixSortScratch sort;
 	uint32_t items_limit = 0; // co-resident blocks of clusters_items_kernel
+	// lb200_clusters_set_launch (0 = the default rule, -1 = every co-resident block, n > 0 = min(n, co-resident)) and what the last fill
+	// launched (lb200_clusters_get_launch)
+	int launch_blocks = 0;
+	uint32_t last_grid = 0, last_tiles = 0;
 	bool filled = false;
 	uint32_t n_lights = 0;    // of the last fill
 };
@@ -556,8 +560,8 @@ int ensure_pairs(lb200_clusters* cl, size_t pairs) {
 	return LB200_OK;
 }
 
-// the four launches of one fill, on the context stream
-int launch_fill(lb200_clusters* cl, ItemsParams& P, uint32_t n_items_bound, uint32_t n_clusters) {
+// the four launches of one fill, on the context stream; *items_grid = the items kernel's grid
+int launch_fill(lb200_clusters* cl, ItemsParams& P, uint32_t n_items_bound, uint32_t n_clusters, uint32_t* items_grid) {
 	lb200_ctx* ctx = cl->ctx;
 	cudaStream_t s = ctx->stream;
 	P.keys = cl->d_keys; P.values = cl->d_values; P.pair_cap = (uint32_t)cl->d_keys.size();
@@ -566,7 +570,10 @@ int launch_fill(lb200_clusters* cl, ItemsParams& P, uint32_t n_items_bound, uint
 	P.res = cl->d_res; P.bar = cl->d_bar;
 	LB200_CUDA(ctx, cudaMemsetAsync(cl->d_res, 0, sizeof(DevResult), s));
 	LB200_CUDA(ctx, cudaMemsetAsync(cl->d_bar, 0, sizeof(GridBar), s));
-	const uint32_t grid = std::max(1u, std::min(cl->items_limit, (n_items_bound + CL_THREADS - 1) / CL_THREADS));
+	uint32_t grid = std::max(1u, std::min(cl->items_limit, (n_items_bound + CL_THREADS - 1) / CL_THREADS));
+	if (cl->launch_blocks < 0) grid = cl->items_limit; // not capped by the work: blocks without items still take part
+	else if (cl->launch_blocks > 0) grid = std::min((uint32_t)cl->launch_blocks, cl->items_limit);
+	*items_grid = grid;
 	void* args[] = {&P};
 	LB200_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)clusters_items_kernel, dim3(grid), dim3(CL_THREADS), args, 0, s));
 	LB200_CHECK_LAUNCH(ctx);
@@ -759,14 +766,18 @@ int lb200_clusters_fill(lb200_clusters* cl, lb200_sortkeys* sk, lb200_culling* c
 	P.n_env = n_env; P.n_refl = n_refl;
 	P.probes = cl->d_probes;
 	P.ent = recs.records; P.pl = cl->d_pl; P.atlas = cl->d_atlas;
-	rc = launch_fill(cl, P, (uint32_t)n_items, n_clusters);
+	uint32_t grid = 0;
+	rc = launch_fill(cl, P, (uint32_t)n_items, n_clusters, &grid);
 	if (rc) return rc;
 	if (cl->h_res.get()->n_pairs > cl->d_keys.size()) { // the map grows: the same work again into room for all of it
 		rc = ensure_pairs(cl, (size_t)cl->h_res.get()->n_pairs);
-		if (!rc) rc = launch_fill(cl, P, (uint32_t)n_items, n_clusters);
+		if (!rc) rc = launch_fill(cl, P, (uint32_t)n_items, n_clusters, &grid);
 		if (rc) { cl->filled = false; return rc; }
 	}
 	const DevResult& d = *cl->h_res.get();
+	const uint32_t items = d.n_lights + n_env + n_refl, chunk = (items + grid - 1) / grid; // as the items kernel splits them
+	cl->last_grid = grid;
+	cl->last_tiles = (chunk + CL_THREADS - 1) / CL_THREADS;
 	memset(result, 0, sizeof(*result));
 	result->n_lights = d.n_lights;
 	result->n_clusters = n_clusters;
@@ -802,6 +813,20 @@ int lb200_clusters_patch_atlas(lb200_clusters* cl, const uint32_t* light_idx, co
 		clusters_patch_kernel<<<1, 32, 0, ctx->stream>>>(cl->d_lights, P);
 		LB200_CHECK_LAUNCH(ctx);
 	}
+	return LB200_OK;
+}
+
+int lb200_clusters_set_launch(lb200_clusters* cl, int blocks) {
+	if (!cl) return LB200_ERR_INVALID;
+	if (blocks < -1) { lb200_set_error(cl->ctx, "clusters_set_launch: blocks %d is not -1, 0 or a block count", blocks); return LB200_ERR_INVALID; }
+	cl->launch_blocks = blocks;
+	return LB200_OK;
+}
+
+int lb200_clusters_get_launch(lb200_clusters* cl, uint32_t* grid, uint32_t* tiles_per_block) {
+	if (!cl) return LB200_ERR_INVALID;
+	if (grid) *grid = cl->last_grid;
+	if (tiles_per_block) *tiles_per_block = cl->last_tiles;
 	return LB200_OK;
 }
 
