@@ -60,41 +60,7 @@ __device__ __forceinline__ Track load_track(const DevTrack* __restrict__ p) {
 	return t;
 }
 
-struct AnimParams {
-	const DevClip* clips;
-	const DevTrack* tracks;
-	const float4* const_t;        // xyz value, w = bone index bits
-	const float4* const_r_value;  // quaternion
-	const uint32_t* const_r_bone;
-	const uint32_t* stream; // all bit streams, word-addressed
-	const float4* key_pos; const float4* key_rot; // decoded keyframes (decode_clips_kernel)
-	const unsigned char* key_flags;               // per (clip, bone): bit0 / bit1 translation / rotation animated, bit2 / bit3 constant track
-	const float4* bind_pos; const float4* bind_rot;         // Bone::relative_transform
-	const float4* inv_bind_pos; const float4* inv_bind_rot; // inverse bind transforms
-	const short* parents;
-	const unsigned char* level_bones; // bones of depth >= 1 sorted by depth (bone_count <= 196 fits a byte)
-	const uint32_t* level_start;      // [max_level + 2]: level l occupies level_bones[level_start[l] .. level_start[l + 1])
-	uint32_t bone_count;
-	uint32_t max_level;
-	uint32_t n_instances;
-	union { const uint32_t* clip_index; const uint32_t* sample_offsets; }; // sample lists: [n_instances + 1] CSR offsets
-	union { uint32_t* time_ticks; const uint32_t* ik_offsets; };           // sample lists: [n_instances + 1] CSR offsets of the IK ops, or null
-	float* out_dq;    // n * B * 8 or null
-	float* out_mtx;   // n * B * 16 or null
-	float* out_pos;   // n * B * 3 or null
-	float* out_rot;   // n * B * 4 or null
-	uint32_t dt_ticks;   // |time_delta| in ticks
-	int dt_negative;
-	int advance;
-	// blend layers on top of the base clip (lb200_animation_set_layers): [instance][n_layers]; n_layers == SAMPLE_LISTS: the system is
-	// in sample-list mode (lb200_animation_set_samples) and the layer fields hold the lists and the bind pose instead
-	uint32_t n_layers;
-	union { const uint32_t* layer_clip; const uint4* samples; };     // sample lists: lb200_sample entries
-	union { const uint32_t* layer_time; const float4* bind_pose; };  // sample lists: bind pos[B], then bind rot[B]
-	union { const float* layer_weight; const uint4* iks; };          // sample lists: the IK ops (IkOp) and their bone paths
-};
-
-// AnimParams::n_layers of a system in sample-list mode (set_layers allows at most 16 layers)
+// AnimSysParams::n_layers of a system in sample-list mode (set_layers allows at most 16 layers)
 constexpr uint32_t SAMPLE_LISTS = 0xffffffffu;
 
 // The device form of one lb200_ik, two 128-bit loads: {after, path_len, bone_count, alpha} {target xyz, path_off}.  path_off is the byte
@@ -424,52 +390,60 @@ __global__ void __launch_bounds__(128) root_motion_tables_kernel(const __grid_co
 
 constexpr int POSE_THREADS = 128;
 
-// The fields of AnimParams that differ from system to system, for pose_palette_many_kernel: the pose kernel reads no other table
-// of a system (the bit streams and track descriptors are only read by decode_clips_kernel).
+// One system as every pose kernel reads it: the pose path reads no other table of a system (the bit streams and track descriptors
+// are only read by decode_clips_kernel).  A system in sample-list mode (lb200_animation_set_samples) has n_layers == SAMPLE_LISTS, and
+// the unions hold its lists, IK ops and bind pose over fields that only clip mode reads.
 struct AnimSysParams {
 	const DevClip* clips;
-	const float4* key_pos; const float4* key_rot;
-	const unsigned char* key_flags;
-	const float4* inv_bind_pos; const float4* inv_bind_rot;
+	const float4* key_pos; const float4* key_rot; // decoded keyframes (decode_clips_kernel)
+	const unsigned char* key_flags;               // per (clip, bone): bit0 / bit1 translation / rotation animated, bit2 / bit3 constant track
+	const float4* inv_bind_pos; const float4* inv_bind_rot; // inverse bind transforms
 	const short* parents;
-	const unsigned char* level_bones;
-	const uint32_t* level_start;
+	const unsigned char* level_bones; // bones of depth >= 1 sorted by depth (bone_count <= 196 fits a byte)
+	const uint32_t* level_start;      // [max_level + 2]: level l occupies level_bones[level_start[l] .. level_start[l + 1])
 	uint32_t bone_count;
 	uint32_t max_level;
 	uint32_t n_instances;
-	uint32_t n_layers;   // SAMPLE_LISTS: sample-list mode, the unions hold what AnimParams' unions hold
-	union { const uint32_t* clip_index; const uint32_t* sample_offsets; };
-	union { uint32_t* time_ticks; const uint32_t* ik_offsets; };
+	uint32_t n_layers; // blend layers on top of the base clip (lb200_animation_set_layers): [instance][n_layers], or SAMPLE_LISTS
+	union { const uint32_t* clip_index; const uint32_t* sample_offsets; }; // sample lists: [n_instances + 1] CSR offsets
+	union { uint32_t* time_ticks; const uint32_t* ik_offsets; };           // sample lists: [n_instances + 1] CSR offsets of the IK ops, or null
 	float* out_dq; float* out_mtx; float* out_pos; float* out_rot; // null where the palette flags do not ask for the output
-	union { const uint32_t* layer_clip; const uint4* samples; };
-	union { const uint32_t* layer_time; const float4* bind_pose; };
-	union { const float* layer_weight; const uint4* iks; };
+	union { const uint32_t* layer_clip; const uint4* samples; };     // sample lists: lb200_sample entries
+	union { const uint32_t* layer_time; const float4* bind_pose; };  // sample lists: bind pos[B], then bind rot[B]
+	union { const float* layer_weight; const uint4* iks; };          // sample lists: the IK ops (IkOp) and their bone paths
 };
 static_assert(sizeof(AnimSysParams) == 160, "");
+
+// One time step for every system of an update
+struct PoseStep {
+	uint32_t dt_ticks; // |time_delta| in ticks
+	int dt_negative;
+	int advance;
+};
 
 // Systems per pose_palette_many_kernel launch (DESIGN.md §4.3): the parameter block is 16 + 164 x cap bytes, 10.5 KB at 64;
 // longer lists run as consecutive launches on the context stream.
 constexpr uint32_t POSE_MANY_CAP = 64;
 
 struct AnimManyParams {
-	uint32_t dt_ticks;   // as AnimParams: one time step for every system
-	int dt_negative;
-	int advance;
+	PoseStep step;
 	uint32_t n_systems;
 	uint32_t block_end[POSE_MANY_CAP]; // inclusive prefix of block counts: system s owns blocks [block_end[s - 1], block_end[s])
 	AnimSysParams sys[POSE_MANY_CAP];
 };
+static_assert(offsetof(AnimManyParams, n_systems) == 12 && offsetof(AnimManyParams, block_end) == 16 &&
+	offsetof(AnimManyParams, sys) == 16 + 4 * POSE_MANY_CAP && sizeof(AnimManyParams) == 16 + 164 * POSE_MANY_CAP, "");
 
 // One instance group of G lanes: sample, blend layers, computeAbsolute, palettes and the time advance of every instance of block
-// `block` of a system.  P holds the system's tables (AnimParams or AnimSysParams), A the time step (dt_ticks, dt_negative, advance).
+// `block` of a system.  P holds the system's tables, A the time step.
 // pose_palette_kernel and pose_palette_many_kernel both run it, so the reference arithmetic exists once.
 // Which start and sample source the body compiles: POSE_EITHER reads the mode of each system (pose_palette_many_kernel); the per-system
 // kernel compiles one mode per instantiation, so that clip mode runs the code it ran before sample lists existed.  IK compiles the
 // IK ops of sample lists in (pose_palette_ik_kernel, pose_palette_many_ik_kernel); the kernels without it run the code they ran before.
 enum PoseMode { POSE_CLIPS, POSE_LISTS, POSE_EITHER };
 
-template <int G, int MODE, class SP, class AP, bool IK = false>
-__device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, const uint32_t block) {
+template <int G, int MODE, bool IK = false>
+__device__ __forceinline__ void pose_palette_body(const AnimSysParams& P, const PoseStep& A, const uint32_t block) {
 	extern __shared__ float4 smem4[];
 	constexpr int INST_PER_BLOCK = POSE_THREADS / G;
 	const int lane = threadIdx.x & 31;
@@ -687,15 +661,15 @@ __device__ __forceinline__ void pose_palette_body(const SP& P, const AP& A, cons
 // walks depth levels with up to G bones of a level in flight.  G is 8 unless LB200_POSE_LANES or lb200_animation_set_launch asks
 // for another (lb200_animation_update).
 template <int G, bool LISTS>
-__global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimParams P) {
-	pose_palette_body<G, LISTS ? POSE_LISTS : POSE_CLIPS>(P, P, blockIdx.x);
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_kernel(const __grid_constant__ AnimSysParams P, const __grid_constant__ PoseStep A) {
+	pose_palette_body<G, LISTS ? POSE_LISTS : POSE_CLIPS>(P, A, blockIdx.x);
 }
 
 // The same for up to POSE_MANY_CAP systems in one grid (lb200_animation_update_many): each block finds its system by a binary search
 // over the prefix of block counts (uniform across the block, once per block) and runs the system's block as pose_palette_kernel would.
 // Dynamic shared memory is sized for the launch's largest skeleton.
-template <int G>
-__global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const __grid_constant__ AnimManyParams M) {
+template <int G, bool IK>
+__device__ __forceinline__ void pose_many_block(const AnimManyParams& M) {
 	uint32_t lo = 0, hi = M.n_systems - 1;
 	while (lo < hi) {
 		const uint32_t mid = (lo + hi) >> 1;
@@ -703,26 +677,24 @@ __global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const _
 		else lo = mid + 1;
 	}
 	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
-	pose_palette_body<G, POSE_EITHER>(M.sys[lo], M, blockIdx.x - first_block);
+	pose_palette_body<G, POSE_EITHER, IK>(M.sys[lo], M.step, blockIdx.x - first_block);
+}
+
+template <int G>
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_kernel(const __grid_constant__ AnimManyParams M) {
+	pose_many_block<G, false>(M);
 }
 
 // pose_palette_kernel<G, true> with the IK ops of the lists (lb200_animation_set_stacks): chosen only for a system that has IK ops
 template <int G>
-__global__ void __launch_bounds__(POSE_THREADS) pose_palette_ik_kernel(const __grid_constant__ AnimParams P) {
-	pose_palette_body<G, POSE_LISTS, AnimParams, AnimParams, true>(P, P, blockIdx.x);
+__global__ void __launch_bounds__(POSE_THREADS) pose_palette_ik_kernel(const __grid_constant__ AnimSysParams P, const __grid_constant__ PoseStep A) {
+	pose_palette_body<G, POSE_LISTS, true>(P, A, blockIdx.x);
 }
 
 // pose_palette_many_kernel<G> with the IK ops: chosen only for a launch in which some system has IK ops
 template <int G>
 __global__ void __launch_bounds__(POSE_THREADS) pose_palette_many_ik_kernel(const __grid_constant__ AnimManyParams M) {
-	uint32_t lo = 0, hi = M.n_systems - 1;
-	while (lo < hi) {
-		const uint32_t mid = (lo + hi) >> 1;
-		if (blockIdx.x < M.block_end[mid]) hi = mid;
-		else lo = mid + 1;
-	}
-	const uint32_t first_block = lo ? M.block_end[lo - 1] : 0u;
-	pose_palette_body<G, POSE_EITHER, AnimSysParams, AnimManyParams, true>(M.sys[lo], M, blockIdx.x - first_block);
+	pose_many_block<G, true>(M);
 }
 
 // ---- skinning ------------------------------------------------------------------------------------------------
@@ -773,6 +745,19 @@ __global__ void __launch_bounds__(SKIN_THREADS) skin_kernel(const float* __restr
 		dst[0] = o[0]; dst[1] = o[1]; dst[2] = o[2];
 	}
 }
+
+// Each kernel family by launch shape, at shapeIndex(G) for G = 4, 8, 16, 32 lanes per instance (the skin kernel: 4, 8, 16 instances
+// per block).  Launches index these tables, and lb200_animation_create sets every kernel's shared memory from them.
+using PoseKernel = void (*)(AnimSysParams, PoseStep);
+using PoseManyKernel = void (*)(AnimManyParams);
+using SkinKernel = void (*)(const float*, const float*, const float4*, const short*, uint32_t, uint32_t, uint32_t, float*);
+const PoseKernel POSE_CLIP_KERNELS[] = {pose_palette_kernel<4, false>, pose_palette_kernel<8, false>, pose_palette_kernel<16, false>, pose_palette_kernel<32, false>};
+const PoseKernel POSE_LIST_KERNELS[] = {pose_palette_kernel<4, true>, pose_palette_kernel<8, true>, pose_palette_kernel<16, true>, pose_palette_kernel<32, true>};
+const PoseKernel POSE_IK_KERNELS[] = {pose_palette_ik_kernel<4>, pose_palette_ik_kernel<8>, pose_palette_ik_kernel<16>, pose_palette_ik_kernel<32>};
+const PoseManyKernel POSE_MANY_KERNELS[] = {pose_palette_many_kernel<4>, pose_palette_many_kernel<8>, pose_palette_many_kernel<16>, pose_palette_many_kernel<32>};
+const PoseManyKernel POSE_MANY_IK_KERNELS[] = {pose_palette_many_ik_kernel<4>, pose_palette_many_ik_kernel<8>, pose_palette_many_ik_kernel<16>, pose_palette_many_ik_kernel<32>};
+const SkinKernel SKIN_KERNELS[] = {skin_kernel<4>, skin_kernel<8>, skin_kernel<16>};
+int shapeIndex(int n) { return __builtin_ctz((unsigned)n) - 2; }
 
 __global__ void __launch_bounds__(256) checksum_kernel(const uint32_t* __restrict__ data, size_t n, unsigned long long* __restrict__ out) {
 	unsigned long long acc = 0;
@@ -1132,31 +1117,14 @@ int lb200_animation_create(lb200_ctx* ctx, const lb200_skeleton* sk, const lb200
 		if (rc) return rc;
 	}
 	LB200_CUDA(ctx, cudaStreamSynchronize(st));
-	{
-		const int smem_max = (int)(sizeof(float4) * (2 * 196 * (POSE_THREADS / 8) + 2 * 196 + 128));
-		const int smem_max4 = (int)std::min<size_t>(220 * 1024, sizeof(float4) * (2 * 196 * (POSE_THREADS / 4) + 2 * 196 + 128));
-		for (int lists = 0; lists < 2; ++lists) {
-			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<4, true> : pose_palette_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
-			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<8, true> : pose_palette_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<16, true> : pose_palette_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-			LB200_CUDA(ctx, cudaFuncSetAttribute(lists ? pose_palette_kernel<32, true> : pose_palette_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		}
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_ik_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max4));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
-		LB200_CUDA(ctx, cudaFuncSetAttribute(pose_palette_many_ik_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max));
+	const int smem_max = (int)(sizeof(float4) * (2 * 196 * (POSE_THREADS / 8) + 2 * 196 + 128));
+	const int smem_max4 = (int)std::min<size_t>(220 * 1024, sizeof(float4) * (2 * 196 * (POSE_THREADS / 4) + 2 * 196 + 128));
+	for (int i = 0; i < 4; ++i) {
+		const int smem = i == shapeIndex(4) ? smem_max4 : smem_max;
+		for (PoseKernel k : {POSE_CLIP_KERNELS[i], POSE_LIST_KERNELS[i], POSE_IK_KERNELS[i]}) LB200_CUDA(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+		for (PoseManyKernel k : {POSE_MANY_KERNELS[i], POSE_MANY_IK_KERNELS[i]}) LB200_CUDA(ctx, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
 	}
-	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * 196 * 3 * sizeof(float4))));
-	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(8 * 196 * 3 * sizeof(float4))));
-	LB200_CUDA(ctx, cudaFuncSetAttribute(skin_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(16 * 196 * 3 * sizeof(float4))));
+	for (int i = 0; i < 3; ++i) LB200_CUDA(ctx, cudaFuncSetAttribute(SKIN_KERNELS[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((4 << i) * 196 * 3 * sizeof(float4))));
 	*out = a.release();
 	return LB200_OK;
 }
@@ -1362,74 +1330,46 @@ size_t poseSmemBytes(const lb200_animation* a, unsigned per_block) {
 // Time::fromSeconds: u32(time * ONE_SECOND), animation.h:21-24 (:462 uses -time_delta for rewinds)
 // animation_module.cpp:458 `if (time_delta > 0) ... else ...`: zero takes the rewind branch too, which leaves a time below the clip
 // length alone and wraps one at or beyond it (time % length), exactly as the reference does on every update
-template <class T> void setTimeStep(T& A, float time_delta) {
+PoseStep timeStep(float time_delta) {
+	PoseStep A;
 	A.dt_negative = !(time_delta > 0);
 	A.dt_ticks = (uint32_t)((A.dt_negative ? -time_delta : time_delta) * (float)(1 << 15));
 	A.advance = 1;
+	return A;
 }
-// what the pose body samples: the base clips and layers of clip mode, or the sample lists and the bind pose (AnimParams' unions)
-template <class T> void setSources(T& P, const lb200_animation* a) {
-	P.layer_weight = a->d_layer_weight;
+// A system's tables for the pose kernels, with the outputs `flags` asks for.  The pose body samples the base clips and layers of clip
+// mode, or the sample lists and the bind pose, whose fields share the unions.
+AnimSysParams sysParams(const lb200_animation* a, uint32_t flags) {
+	AnimSysParams S;
+	S.clips = a->d_clips; S.key_pos = a->d_key_pos; S.key_rot = a->d_key_rot; S.key_flags = a->d_key_flags;
+	S.inv_bind_pos = a->d_bind + 2 * a->bone_count; S.inv_bind_rot = a->d_bind + 3 * a->bone_count;
+	S.parents = a->d_parents; S.level_bones = a->d_level_bones; S.level_start = a->d_level_start;
+	S.bone_count = a->bone_count; S.max_level = a->max_level; S.n_instances = a->n_instances;
+	S.time_ticks = a->d_time;
+	S.layer_weight = a->d_layer_weight;
 	if (a->sample_lists) {
-		P.n_layers = SAMPLE_LISTS;
-		P.sample_offsets = a->d_sample_offsets; P.samples = reinterpret_cast<const uint4*>(a->d_samples.get()); P.bind_pose = a->d_bind;
-		P.ik_offsets = a->n_ik ? a->d_ik_offsets.get() : nullptr; P.iks = a->d_iks; // over time_ticks and layer_weight, which lists do not read
+		S.n_layers = SAMPLE_LISTS;
+		S.sample_offsets = a->d_sample_offsets; S.samples = reinterpret_cast<const uint4*>(a->d_samples.get()); S.bind_pose = a->d_bind;
+		S.ik_offsets = a->n_ik ? a->d_ik_offsets.get() : nullptr; S.iks = a->d_iks; // over time_ticks and layer_weight, which lists do not read
 	}
 	else {
-		P.n_layers = a->n_layers;
-		P.clip_index = a->d_clip_index; P.layer_clip = a->d_layer_clip; P.layer_time = a->d_layer_time;
+		S.n_layers = a->n_layers;
+		S.clip_index = a->d_clip_index; S.layer_clip = a->d_layer_clip; S.layer_time = a->d_layer_time;
 	}
+	S.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
+	S.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
+	S.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
+	S.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
+	return S;
 }
 // whether a system runs the IK kernels: sample lists with IK ops
 bool hasIk(const lb200_animation* a) { return a->sample_lists && a->n_ik; }
-// pose_palette_kernel<G> (pose_palette_ik_kernel<G> for a system with IK ops) over one system's instances (the caller checks the launch)
-void launchPose(const lb200_animation* a, int G, float time_delta, uint32_t flags) {
-	AnimParams P;
-	P.clips = a->d_clips; P.tracks = a->d_tracks; P.const_t = a->d_const_t; P.const_r_value = a->d_const_r_value; P.const_r_bone = a->d_const_r_bone; P.stream = a->d_stream;
-	P.key_pos = a->d_key_pos; P.key_rot = a->d_key_rot; P.key_flags = a->d_key_flags;
-	P.bind_pos = a->d_bind; P.bind_rot = a->d_bind + a->bone_count; P.inv_bind_pos = a->d_bind + 2 * a->bone_count; P.inv_bind_rot = a->d_bind + 3 * a->bone_count; P.parents = a->d_parents; P.level_bones = a->d_level_bones; P.level_start = a->d_level_start;
-	P.bone_count = a->bone_count; P.max_level = a->max_level; P.n_instances = a->n_instances;
-	P.time_ticks = a->d_time;
-	setSources(P, a);
-	P.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
-	P.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
-	P.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
-	P.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
-	setTimeStep(P, time_delta);
-	const unsigned per_block = POSE_THREADS / G;
-	const unsigned blocks = (a->n_instances + per_block - 1) / per_block;
-	const size_t smem = poseSmemBytes(a, per_block);
-	cudaStream_t st = a->ctx->stream;
-	const bool lists = a->sample_lists;
-	if (hasIk(a)) {
-		if (G == 4) pose_palette_ik_kernel<4><<<blocks, POSE_THREADS, smem, st>>>(P);
-		else if (G == 8) pose_palette_ik_kernel<8><<<blocks, POSE_THREADS, smem, st>>>(P);
-		else if (G == 16) pose_palette_ik_kernel<16><<<blocks, POSE_THREADS, smem, st>>>(P);
-		else pose_palette_ik_kernel<32><<<blocks, POSE_THREADS, smem, st>>>(P);
-		return;
-	}
-	if (G == 4) (lists ? pose_palette_kernel<4, true> : pose_palette_kernel<4, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
-	else if (G == 8) (lists ? pose_palette_kernel<8, true> : pose_palette_kernel<8, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
-	else if (G == 16) (lists ? pose_palette_kernel<16, true> : pose_palette_kernel<16, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
-	else (lists ? pose_palette_kernel<32, true> : pose_palette_kernel<32, false>)<<<blocks, POSE_THREADS, smem, st>>>(P);
-}
 } // namespace
 
 extern "C" {
 
 int lb200_animation_update(lb200_animation* a, float time_delta, uint32_t flags) {
-	lb200_range range("update animables"); // animation_module.cpp:743
-	if (!a) return LB200_ERR_INVALID;
-	lb200_ctx* ctx = a->ctx;
-	if (!a->n_instances) return LB200_OK;
-	LB200_CUDA(ctx, cudaSetDevice(ctx->device));
-	const int rc = allocOutputs(a, flags);
-	if (rc) return rc;
-	const int G = fitLanes(requestedLanes(a), a->bone_count);
-	launchPose(a, G, time_delta, flags);
-	LB200_CHECK_LAUNCH(ctx);
-	a->last_pose_lanes = G;
-	return LB200_OK;
+	return lb200_animation_update_many(&a, 1, time_delta, flags);
 }
 
 int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, float time_delta, uint32_t flags) {
@@ -1446,7 +1386,7 @@ int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, flo
 		std::sort(sorted.begin(), sorted.end());
 		if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) { lb200_set_error(ctx, "update_many: a system is listed twice"); return LB200_ERR_INVALID; }
 	}
-	// systems without instances are skipped, as lb200_animation_update skips them; the others agree on one G or run 8
+	// systems without instances are skipped; the others agree on one G or run 8
 	std::vector<lb200_animation*> run;
 	run.reserve(n);
 	uint32_t max_bones = 0;
@@ -1466,48 +1406,29 @@ int lb200_animation_update_many(lb200_animation* const* systems, uint32_t n, flo
 		if (rc) return rc;
 	}
 	G = fitLanes(G, max_bones);
+	const int lanes = shapeIndex(G);
 	const unsigned per_block = POSE_THREADS / G;
 	AnimManyParams M;
-	setTimeStep(M, time_delta);
+	M.step = timeStep(time_delta);
 	for (size_t first = 0; first < run.size(); first += POSE_MANY_CAP) {
 		const uint32_t count = (uint32_t)std::min<size_t>(POSE_MANY_CAP, run.size() - first);
-		if (count == 1) { // a launch of one system is the per-system kernel: no search, parameters read at fixed offsets
-			launchPose(run[first], G, time_delta, flags);
-			LB200_CHECK_LAUNCH(ctx);
-			continue;
-		}
 		M.n_systems = count;
 		uint32_t blocks = 0;
 		size_t smem = 0;
-		bool ik = false; // some system of the launch has IK ops: pose_palette_many_ik_kernel
+		bool ik = false; // some system of the launch has IK ops: the IK kernels
 		for (uint32_t s = 0; s < count; ++s) {
 			const lb200_animation* a = run[first + s];
 			ik = ik || hasIk(a);
-			AnimSysParams& S = M.sys[s];
-			S.clips = a->d_clips; S.key_pos = a->d_key_pos; S.key_rot = a->d_key_rot; S.key_flags = a->d_key_flags;
-			S.inv_bind_pos = a->d_bind + 2 * a->bone_count; S.inv_bind_rot = a->d_bind + 3 * a->bone_count;
-			S.parents = a->d_parents; S.level_bones = a->d_level_bones; S.level_start = a->d_level_start;
-			S.bone_count = a->bone_count; S.max_level = a->max_level; S.n_instances = a->n_instances;
-			S.time_ticks = a->d_time;
-			setSources(S, a);
-			S.out_dq = (flags & LB200_PALETTE_DUAL_QUAT) ? a->d_dq.get() : nullptr;
-			S.out_mtx = (flags & LB200_PALETTE_MATRIX) ? a->d_mtx.get() : nullptr;
-			S.out_pos = (flags & LB200_PALETTE_POSE) ? a->d_pos.get() : nullptr;
-			S.out_rot = (flags & LB200_PALETTE_POSE) ? a->d_rot.get() : nullptr;
+			M.sys[s] = sysParams(a, flags);
 			blocks += (a->n_instances + per_block - 1) / per_block;
 			M.block_end[s] = blocks;
 			smem = std::max(smem, poseSmemBytes(a, per_block));
 		}
-		if (ik) {
-			if (G == 4) pose_palette_many_ik_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-			else if (G == 8) pose_palette_many_ik_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-			else if (G == 16) pose_palette_many_ik_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-			else pose_palette_many_ik_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		if (count == 1) { // a launch of one system is the per-system kernel: no search, parameters read at fixed offsets
+			const PoseKernel* family = ik ? POSE_IK_KERNELS : run[first]->sample_lists ? POSE_LIST_KERNELS : POSE_CLIP_KERNELS;
+			family[lanes]<<<blocks, POSE_THREADS, smem, ctx->stream>>>(M.sys[0], M.step);
 		}
-		else if (G == 4) pose_palette_many_kernel<4><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-		else if (G == 8) pose_palette_many_kernel<8><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-		else if (G == 16) pose_palette_many_kernel<16><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
-		else pose_palette_many_kernel<32><<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
+		else (ik ? POSE_MANY_IK_KERNELS : POSE_MANY_KERNELS)[lanes]<<<blocks, POSE_THREADS, smem, ctx->stream>>>(M);
 		LB200_CHECK_LAUNCH(ctx);
 	}
 	for (lb200_animation* a : run) a->last_pose_lanes = G;
@@ -1527,9 +1448,8 @@ int lb200_animation_skin(lb200_animation* a) {
 	const dim3 grid((a->n_vertices + SKIN_THREADS - 1) / SKIN_THREADS, (a->n_instances + group - 1) / group);
 	if (grid.y > 65535) { lb200_set_error(ctx, "too many instances for one skin launch"); return LB200_ERR_INVALID; }
 	const size_t smem = sizeof(float4) * 3 * a->bone_count * group;
-#define LB200_SKIN_LAUNCH(G) skin_kernel<G><<<grid, SKIN_THREADS, smem, ctx->stream>>>(a->d_mtx, a->d_mesh_pos, a->d_mesh_w, a->d_mesh_idx, a->n_vertices, a->bone_count, a->n_instances, a->d_skinned)
-	if (group == 4) LB200_SKIN_LAUNCH(4); else if (group == 16) LB200_SKIN_LAUNCH(16); else LB200_SKIN_LAUNCH(8);
-#undef LB200_SKIN_LAUNCH
+	SKIN_KERNELS[shapeIndex(group)]<<<grid, SKIN_THREADS, smem, ctx->stream>>>(a->d_mtx, a->d_mesh_pos, a->d_mesh_w, a->d_mesh_idx, a->n_vertices,
+		a->bone_count, a->n_instances, a->d_skinned);
 	LB200_CHECK_LAUNCH(ctx);
 	a->last_skin_group = group;
 	return LB200_OK;
